@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""bench.py — paths/sec of batched TOPP-RA (7-DOF, 200 gridpoints, vel+accel) on N B200s vs the reference CPU
-seidel path.  Contract: see the task statement; one JSON line on stdout (rank 0).
+"""bench.py — paths/sec of batched TOPP-RA (7-DOF, 200 gridpoints, vel+accel) on N H100s vs the reference CPU
+seidel path.  Prints one JSON line on stdout (rank 0).
 
   python bench.py [--gpus N] [--steps K] [--warmup W]            # this repo (CUDA kernels)
   python bench.py --impl reference [--gpus N] [--steps K] ...    # the reference's own CPU path on the host cores
+  python bench.py ... --dump-outputs DIR                          # also write the last timed step's results as DIR/*.npy
 
 A "step" = one pass of the hot path over one batch of `--batch` synthetic paths per GPU (BASELINE.json configs[1]:
 4096 random 7-DOF spline paths, 200 gridpoints, vel+acc): K0 spline fit -> K1 coefficient records -> K2
@@ -24,10 +25,11 @@ sys.path.insert(0, os.path.join(ROOT, "tests"))
 
 METRIC = "paths/sec (7-DOF, 200 gridpoints, vel+accel)"
 UNIT = "paths/s"
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet (HBM3); the roofline fractions are against this figure
 
 
 def workload_text(B, dof, G):
-    """One string for both arms (the driver compares the arms' `config.workload`)."""
+    """One string for both arms (results of the two arms are matched by `config.workload`)."""
     return ("configs[1]: batch %d random %d-DOF cubic-spline paths (5 waypoints), %d gridpoints, "
             "JointVelocity+JointAcceleration(interp), per GPU" % (B, dof, G))
 
@@ -35,7 +37,7 @@ def workload_text(B, dof, G):
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--steps", type=int, default=20, help="timed steps (>= 1)")
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--batch", type=int, default=4096, help="paths per GPU per step (BASELINE configs[1]: 4096)")
@@ -47,7 +49,38 @@ def parse_args():
                     "headline cfg 2 (comma list out of 1,3,4,5; 'none' to skip)")
     ap.add_argument("--cfg3-batch", type=int, default=65536)
     ap.add_argument("--cfg5-batch", type=int, default=1 << 20)
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (K, sd, sdd, status, fail_stage "
+                         "of the headline batch) as DIR/<name>.npy in float64; under torchrun rank 0 writes its own "
+                         "shard (its paths are seeded by rank 0's seed); not available with --impl reference")
+    args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs applies to the GPU path; --impl reference times the CPU arm only")
+    return args
+
+
+DUMP_LIMIT_BYTES = 64 * 1000 * 1000
+
+
+def dump_outputs(out_dir, out):
+    """Write the arrays a caller of the timed path receives (`engine.scan_velacc`'s dict, `u` saved as `sdd`) as float64
+    .npy files.  When they exceed DUMP_LIMIT_BYTES, a fixed seeded sample of paths is written instead, with the sampled
+    path indices in `path_index.npy`; the inputs are seeded too, so two builds can be compared file by file."""
+    arrays = {"K": out["K"], "sd": out["sd"], "sdd": out["u"], "status": out["status"], "fail_stage": out["fail_stage"]}
+    B = out["status"].shape[0]
+    per_path = sum(8 * (t[0].numel() if B else 0) for t in arrays.values())
+    idx = None
+    if per_path * B > DUMP_LIMIT_BYTES:
+        keep = max(1, (DUMP_LIMIT_BYTES - 8 * B - 4096) // per_path)   # room for path_index.npy and the .npy headers
+        idx = np.sort(np.random.RandomState(0).choice(B, keep, replace=False))
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy().astype(np.float64)
+        np.save(os.path.join(out_dir, name + ".npy"), a if idx is None else a[idx])
+    if idx is not None:
+        np.save(os.path.join(out_dir, "path_index.npy"), idx.astype(np.float64))
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -431,7 +464,7 @@ def extra_configs(args, torch, dist, ta, dev, world, rank, peak):
         d_way, d_ss = torch.as_tensor(way).to(dev), torch.as_tensor(ss).to(dev)
         d_vlim, d_alim = torch.as_tensor(vlim).to(dev), torch.as_tensor(alim).to(dev)
         d_grid = torch.as_tensor(np.linspace(0, 1, G)).to(dev)
-        # chunks of >= 32768 paths where the shard allows it (the scan's large-batch forward pass starts at 24576 paths)
+        # chunks of >= 32768 paths where the shard allows it (the scan's large-batch forward pass starts at 16384 paths)
         solver = ShardedSolver(Btot, G, dev, nchunks=max(2, min(8, shard // 32768)), gather=True)
 
         ms, full = timed(lambda: solver.solve(d_ss, d_way, d_grid, d_vlim, d_alim), 3, 2)
@@ -488,7 +521,7 @@ def run_b200(args):
     dev = torch.device("cuda", local_rank)
     if world > 1:
         # NCCL's copy kernels share the SMs with the scan (whose resident one-warp CTAs hold the whole register file); the
-        # high-priority NCCL stream is the cheap half of the remedy (measured at N = 8: no change on its own, DESIGN.md 7)
+        # high-priority NCCL stream is the cheap half of the remedy (DESIGN.md 7)
         opts = None
         try:
             opts = dist.ProcessGroupNCCL.Options(is_high_priority_stream=True)
@@ -514,7 +547,7 @@ def run_b200(args):
 
     h_sets = [pinned_set(), pinned_set()]   # a pipelined caller alternates between two result buffers
     h_out = h_sets[0]
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # 256 MB > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # 256 MB > 50 MB L2 of an H100
     W = engine.record_doubles(R)
     records = torch.empty((B, G, W), dtype=torch.float64, device=dev)
     gathered = torch.empty((world * B, G), dtype=torch.float64, device=dev) if world > 1 else None
@@ -523,6 +556,7 @@ def run_b200(args):
     k_events = []  # (k0_start, k1_start, k2_start, k2_end) per timed step
 
     scan_mode = {"fast_lower": False}
+    last_timed = {}  # results of the last timed headline step (for --dump-outputs)
 
     xbound = torch.empty((B, G, 2), dtype=torch.float64, device=dev)
 
@@ -539,6 +573,7 @@ def run_b200(args):
         if e:
             e[3].record()
             k_events.append(e)
+            last_timed["out"] = out
         return out
 
     rec_events = []
@@ -685,18 +720,14 @@ def run_b200(args):
     k1 = float(np.mean([e[1].elapsed_time(e[2]) for e in k_events]))
     k2 = float(np.mean([e[2].elapsed_time(e[3]) for e in k_events]))
 
-    peaks0 = {}
-    try:
-        peaks0 = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
+    peak = HBM_PEAK_GBS
     # per-rank K2 time (SCALE: explains the max-over-ranks step time)
     k2_ranks = torch.tensor([k2, -k2], dtype=torch.float64, device=dev)
     if world > 1:
         dist.all_reduce(k2_ranks, op=dist.ReduceOp.MAX)
     k2_min, k2_max = -float(k2_ranks[1].item()), float(k2_ranks[0].item())
     try:
-        configs = extra_configs(args, torch, dist, ta, dev, world, rank, float(peaks0.get("hbm_gbs", 6650.0)))
+        configs = extra_configs(args, torch, dist, ta, dev, world, rank, peak)
     except Exception as exc:  # never lose the headline line
         configs = {"error": repr(exc)}
 
@@ -707,26 +738,20 @@ def run_b200(args):
 
     # roofline of the dominant kernel: the fused scan (tb_scan_velacc).  SURVEY.md section 8d's contract: report against the
     # MATERIALISED-record algorithmic bytes (rows read twice + outputs) and note what the fused form really moves.
-    peak = float(peaks0.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks0 else "fallback 6.65 TB/s"
+    peak_src = "H100 SXM data sheet: 3.35 TB/s HBM3"
     bytes_k1 = (4 * (nway - 1) * dof * 8 + G * (3 * R + 2) * 8) * B
     bytes_k2 = (2 * G * (3 * R + 2) * 8 + G * 16 + G * 8 + (G - 1) * 8 + 8) * B
     bytes_fused = (4 * (nway - 1) * dof * 8 + G * 16 + G * 16 + G * 8 + (G - 1) * 8 + 8) * B
     bytes_xb = (4 * (nway - 1) * dof * 8 + G * 16) * B
-    traffic = None
-    try:
-        traffic = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        pass
     roof = {"kernel": "scan_kernel<FUSED> (tb_scan_velacc: K1 rows built inside K2)", "bound": "hbm",
             "achieved": bytes_k2 / (k2 * 1e-3) / 1e9, "peak": peak,
             "unit": "GB/s", "frac": bytes_k2 / (k2 * 1e-3) / 1e9 / peak,
-            "traffic": (traffic or {}).get("scan_velacc_bytes_per_launch"), "peak_source": peak_src,
+            "peak_source": peak_src,
             "algorithmic_bytes_per_launch": bytes_k2, "ms_per_launch": k2,
             "fused_bytes_per_launch": bytes_fused,
             "note": "algorithmic bytes = the materialised-record figure of SURVEY 8d (281,600 B/path); the fused kernel "
                     "itself reads spline + velocity bound and writes K, sd, u (fused_bytes_per_launch): the scan is a "
-                    "latency/issue-bound chain of 597 dependent LPs per path, see lp_solves_per_s and profiles/"}
+                    "latency/issue-bound chain of 597 dependent LPs per path, see lp_solves_per_s"}
     roof_k1 = {"kernel": "xbound_velocity_kernel (K1 of the fused path: velocity bound only)", "bound": "hbm",
                "achieved": bytes_xb / (k1 * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                "frac": bytes_xb / (k1 * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_launch": bytes_xb, "ms_per_launch": k1}
@@ -739,11 +764,9 @@ def run_b200(args):
                 "K2 record scan); not part of `value`",
         "ms_per_step": ms_rec / args.steps, "kernels_ms": {"K0": rk0, "K1_coeff_velacc": rk1, "K2_scan_records": rk2},
         "roofline_k1": {"bound": "hbm", "achieved": bytes_k1 / (rk1 * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-                        "frac": bytes_k1 / (rk1 * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_launch": bytes_k1,
-                        "traffic": (traffic or {}).get("coeff_velacc_kernel_bytes_per_launch")},
+                        "frac": bytes_k1 / (rk1 * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_launch": bytes_k1},
         "roofline_k2": {"bound": "hbm", "achieved": bytes_k2 / (rk2 * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
-                        "frac": bytes_k2 / (rk2 * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_launch": bytes_k2,
-                        "traffic": (traffic or {}).get("scan_kernel_bytes_per_launch")}}
+                        "frac": bytes_k2 / (rk2 * 1e-3) / 1e9 / peak, "algorithmic_bytes_per_launch": bytes_k2}}
 
     h2d = int(h_way.numel() + h_vlim.numel() + h_alim.numel() + h_ss.numel() + h_grid.numel()) * 8
     d2h = int(h_out["K"].numel() + h_out["sd"].numel() + h_out["sdd"].numel()) * 8 + int(h_out["status"].numel()) * 8
@@ -780,6 +803,8 @@ def run_b200(args):
         "cpu_baseline": cpu,
     }
     print(json.dumps(line), flush=True)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last_timed["out"])
     if world > 1:
         dist.destroy_process_group()
 

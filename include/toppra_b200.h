@@ -1,6 +1,6 @@
 /*
  * toppra_b200.h — C-ABI of libtoppra_b200.so: batched TOPP-RA (time-optimal path
- * parameterisation by reachability analysis) on NVIDIA B200 (sm_100a).
+ * parameterisation by reachability analysis) on NVIDIA H100 (sm_90a).
  *
  * This is the drop-in boundary for the hot path of hungpham2511/toppra v0.6.2
  * (paths below are relative to the reference tree):

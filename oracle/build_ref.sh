@@ -1,6 +1,8 @@
 #!/usr/bin/env bash
 # TEST INFRASTRUCTURE ONLY — builds the UNMODIFIED reference (hungpham2511/toppra v0.6.2)
-# from the sources where they lie under /root/reference into oracle/_ref/ (git-ignored).
+# from the checkout named by $TOPPRA_REFERENCE (default /root/reference), where its sources lie, into oracle/_ref/
+# (git-ignored).  Used by the tests that run the reference's own classes and files, by bench.py's CPU baseline and to
+# regenerate tests/golden (tests/golden/make_golden.py).
 #
 # Recipe (SURVEY.md §8c):
 #   1. stage toppra/ + setup.py + VERSION + README.md into a scratch dir under /tmp
@@ -9,14 +11,13 @@
 #      compile against numpy >= 2 -> `np.int64_t` (the same C type np.int_t had on Linux x86-64);
 #   3. `python setup.py build_ext --inplace` (the reference's own flags: -O1);
 #   4. install the built package (py + .so) into oracle/_ref/toppra.
-# Nothing from the reference is committed to this repository; oracle/_ref/ is in .gitignore
-# (NOT in .gpurunignore, so the built package travels to the GPU box for the CPU baseline).
+# Nothing from the reference is committed to this repository; oracle/_ref/ is in .gitignore.
 set -euo pipefail
 HERE="$(cd "$(dirname "${BASH_SOURCE[0]}")" && pwd)"
 REF="${TOPPRA_REFERENCE:-/root/reference}"
 OUT="$HERE/_ref"
 if [ ! -d "$REF/toppra" ]; then
-  echo "[build_ref] $REF not present (GPU box?) - keeping prebuilt $OUT" >&2
+  echo "[build_ref] no reference checkout at '$REF' (set TOPPRA_REFERENCE) - keeping $OUT as it is" >&2
   exit 0
 fi
 SCRATCH="$(mktemp -d /tmp/toppra_ref_build.XXXXXX)"

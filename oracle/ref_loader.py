@@ -16,7 +16,7 @@ def reference_available():
 def load_reference():
     """Return the reference `toppra` package (imported from oracle/_ref)."""
     if not reference_available():
-        raise ImportError("oracle/_ref/toppra missing: run oracle/build_ref.sh where /root/reference exists")
+        raise ImportError("oracle/_ref/toppra missing: run oracle/build_ref.sh (TOPPRA_REFERENCE=<toppra checkout>, default /root/reference)")
     try:
         import matplotlib.pyplot  # noqa: F401
     except Exception:  # matplotlib absent -> stub (algorithm.py:14 imports pyplot unconditionally)

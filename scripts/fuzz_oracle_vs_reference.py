@@ -5,7 +5,7 @@ UNMODIFIED reference build (oracle/_ref) on randomly SHAPED problems — far mor
 and interpolation, active velocity bounds, non-zero boundary velocities (admissible or not), near-degenerate paths.
 Any mismatch is printed with the seed that reproduces it.
 
-usage: python scripts/fuzz_oracle_vs_reference.py [--minutes M] [--seed S]      (needs oracle/_ref, i.e. this container)"""
+usage: python scripts/fuzz_oracle_vs_reference.py [--minutes M] [--seed S]      (needs oracle/_ref, see oracle/build_ref.sh)"""
 import argparse
 import os
 import sys
@@ -19,13 +19,17 @@ sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 warnings.filterwarnings("ignore")
 
 from oracle import oracle as orc  # noqa: E402
-from oracle.ref_loader import load_reference  # noqa: E402
 
-ta = load_reference()
-import toppra.algorithm as algo  # noqa: E402
-import toppra.constraint as constraint  # noqa: E402
-import toppra.interpolator as interp  # noqa: E402
-from toppra.parametrizer import ParametrizeSpline  # noqa: E402
+# the reference package and its modules; set by use()
+ta = algo = constraint = interp = par = None
+
+
+def use(toppra):
+    """Run the checks against `toppra`: the reference package (oracle.ref_loader.load_reference()), or a recording /
+    replay of it (tests/ref_replay.py)."""
+    global ta, algo, constraint, interp, par
+    ta = toppra
+    algo, constraint, interp, par = ta.algorithm, ta.constraint, ta.interpolator, ta.parametrizer
 
 
 def eq(a, b):
@@ -95,7 +99,7 @@ def check_frows(p, rng):
         if rng.rand() < 0.3:
             vel[G // 3:G // 3 + 2] = 1e10
         try:
-            traj = ParametrizeSpline(path, p["grid"], vel)
+            traj = par.ParametrizeSpline(path, p["grid"], vel)
         except Exception:
             return
         t, s, nk = cpu_engine.spline_time_stamps(torch.from_numpy(vel[None]), torch.from_numpy(p["grid"]))
@@ -176,14 +180,13 @@ def check_parametrizers(p, rng):
     (knot times bit for bit, the clamped re-fit and its evaluations to rounding) on the solved velocity profile."""
     if p["bc"] != "not-a-knot" or len(p["ss"]) == 3 or len(p["grid"]) < 3:
         return
-    from toppra.parametrizer import ParametrizeConstAccel
     tb = mine()
     theirs, ours = ta.SplineInterpolator(p["ss"], p["way"]), tb.SplineInterpolator(p["ss"], p["way"])
     cons = [constraint.JointVelocityConstraint(p["vlim"]), constraint.JointAccelerationConstraint(p["alim"], p["interp"])]
     _, sd, _ = algo.TOPPRA(cons, theirs, gridpoints=p["grid"], solver_wrapper="seidel").compute_parameterization(0, 0)
     if sd is None or not np.all(sd[1:] + sd[:-1] > 0):
         return
-    a, b = ParametrizeConstAccel(theirs, p["grid"], sd), tb.ParametrizeConstAccel(ours, p["grid"], sd)
+    a, b = par.ParametrizeConstAccel(theirs, p["grid"], sd), tb.ParametrizeConstAccel(ours, p["grid"], sd)
     count("ParametrizeConstAccel")
     assert eq(a._ts, b._ts) and eq(a._us, b._us) and a.duration == b.duration, "ConstAccel time grid"
     ts = np.r_[0.0, np.sort(rng.uniform(0, a.duration, 30)), a.duration]
@@ -192,7 +195,7 @@ def check_parametrizers(p, rng):
         want = a(ts, order)
         np.testing.assert_allclose(b(ts, order), want, rtol=tol, atol=tol * max(scale, np.abs(want).max()),
                                    err_msg="ConstAccel order %d" % order)
-    sa, sb = ParametrizeSpline(theirs, p["grid"], sd), tb.ParametrizeSpline(ours, p["grid"], sd)
+    sa, sb = par.ParametrizeSpline(theirs, p["grid"], sd), tb.ParametrizeSpline(ours, p["grid"], sd)
     count("ParametrizeSpline")
     assert eq(sa.ss_waypoints, sb.ss_waypoints) and sa.duration == sb.duration, "ParametrizeSpline knots"
     ts = np.linspace(0, sa.duration, 25)
@@ -361,6 +364,8 @@ def main():
     ap.add_argument("--minutes", type=float, default=5.0)
     ap.add_argument("--seed", type=int, default=0)
     args = ap.parse_args()
+    from oracle.ref_loader import load_reference
+    use(load_reference())
     t_end = time.time() + 60 * args.minutes
     seed, bad, hist = args.seed, [], {}
     while time.time() < t_end:

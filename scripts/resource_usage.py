@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Registers / stack / shared memory per kernel of the BUILT library (cuobjdump -res-usage), demangled and sorted.
-usage: python scripts/resource_usage.py [toppra_b200/libtoppra_b200.so] > profiles/rNN_resource_usage.txt"""
+usage: python scripts/resource_usage.py [toppra_b200/libtoppra_b200.so] > resource_usage.txt"""
 import re
 import subprocess
 import sys
@@ -20,7 +20,7 @@ for line in text.splitlines():
     if m and name:
         rows.append((name,) + tuple(int(x) for x in m.groups()))
         name = None
-print("# %s: %d kernels (sm_100a).  stack = bytes of local memory per thread (spills of the register-capped scan builds,"
+print("# %s: %d kernels (sm_90a).  stack = bytes of local memory per thread (spills of the register-capped scan builds,"
       " run-time indexed arrays elsewhere); shared = static shared memory incl. the 1 KB the system reserves per CTA." % (so, len(rows)))
 print("%-86s %5s %6s %7s" % ("kernel", "regs", "stack", "shared"))
 for name, reg, stack, shared, local in sorted(rows):

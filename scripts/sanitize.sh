@@ -2,9 +2,13 @@
 # compute-sanitizer over a small end-to-end solve (K0, K1, K2 record scan + fused scan + ragged, K2r, K3, LP shims, the row-f
 # kernels of round 2: propose_gridpoints, reachable sets, TOPPRAsd bisection, spline time stamps, torque rows, ubound
 # records): memcheck + racecheck + synccheck.
+# usage: bash scripts/sanitize.sh [OUT_DIR]      (summary -> OUT_DIR/sanitizer.txt, default OUT_DIR = sanitizer_out)
 set -u
-mkdir -p gpurun_out
-cat > /tmp/san_case.py <<'PY'
+OUT="${1:-sanitizer_out}"
+mkdir -p "$OUT"
+CASE="$(mktemp /tmp/san_case.XXXXXX.py)"
+trap 'rm -f "$CASE"' EXIT
+cat > "$CASE" <<'PY'
 import sys, numpy as np
 sys.path.insert(0, "."); sys.path.insert(0, "tests")
 import toppra_b200 as ta
@@ -41,5 +45,5 @@ print("ok", int((res.status != 0).sum()), int((rob.status != 0).sum()), float(bp
 PY
 for tool in memcheck racecheck synccheck; do
   echo "== compute-sanitizer --tool $tool"
-  timeout 900 compute-sanitizer --tool $tool --error-exitcode 7 python /tmp/san_case.py 2>&1 | grep -E "ERROR SUMMARY|RACECHECK SUMMARY|^ok|error|Error" | head -8
-done 2>&1 | tee gpurun_out/sanitizer_r02.txt
+  timeout 900 compute-sanitizer --tool $tool --error-exitcode 7 python "$CASE" 2>&1 | grep -E "ERROR SUMMARY|RACECHECK SUMMARY|^ok|error|Error" | head -8
+done 2>&1 | tee "$OUT/sanitizer.txt"

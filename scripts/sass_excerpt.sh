@@ -2,7 +2,7 @@
 # SASS evidence from the built library (no GPU needed): which instructions the scan kernels are made of.
 LIB=toppra_b200/libtoppra_b200.so
 cuobjdump -sass $LIB > /tmp/tb_lib.sass 2>/dev/null
-echo "# $LIB  ($(cuobjdump -lelf $LIB | grep -c sm_100a) sm_100a cubin(s), $(grep -c 'Function :' /tmp/tb_lib.sass) kernels)"
+echo "# $LIB  ($(cuobjdump -lelf $LIB | grep -c sm_90a) sm_90a cubin(s), $(grep -c 'Function :' /tmp/tb_lib.sass) kernels)"
 echo "# mnemonic counts over all kernels"
 for op in UBLKCP SYNCS.ARRIVE SYNCS.PHASECHK REDUX SHFL.IDX SHFL.BFLY VOTE MUFU.RCP64H MUFU.RSQ64H DFMA DADD DMUL DSETP ELECT HMMA UTCHMMA; do
   printf "%-16s %s\n" "$op" "$(grep -c "$op" /tmp/tb_lib.sass)"

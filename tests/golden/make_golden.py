@@ -1,10 +1,10 @@
 """Generates tests/golden/*.npz by running the UNMODIFIED reference (oracle/_ref, built by
-oracle/build_ref.sh from /root/reference) and scipy.  Run where /root/reference exists:
+oracle/build_ref.sh from a checkout of the original toppra) and scipy:
 
-    python tests/golden/make_golden.py
+    bash oracle/build_ref.sh && python tests/golden/make_golden.py [case]    # TOPPRA_REFERENCE: default /root/reference
 
 The fixtures pin the oracle (tests/test_oracle_vs_golden.py, CPU) and the CUDA path
-(tests/test_gpu_*.py) to the reference's own outputs; /root/reference is not needed to RUN the tests.
+(tests/test_gpu_*.py) to the reference's own outputs; the reference is not needed to RUN the tests.
 Inputs follow SURVEY.md §8d (cfg 1/2, parity sets P1-P6) and the reference's own test fixtures
 (cited per case)."""
 import os
@@ -28,7 +28,7 @@ import toppra.constraint as constraint  # noqa: E402
 import toppra.solverwrapper.cy_seidel_solverwrapper as seidel  # noqa: E402
 from scipy.interpolate import CubicSpline  # noqa: E402
 
-REF_TESTS = "/root/reference/tests/tests"
+REF_TESTS = os.path.join(os.environ.get("TOPPRA_REFERENCE", "/root/reference"), "tests", "tests")
 
 
 def solve_ref(ss, way, vlim, alim, grid, sd_start=0.0, sd_end=0.0, scheme=1, bc_type="not-a-knot"):
@@ -364,7 +364,6 @@ def shortcut_rows_case():
                     self.xb.copy())
 
     codes = list(algo.ParameterizationReturnCode)
-    data = {}
     for name, (gen, args) in SHORTCUT_SETS.items():
         rows, xb = gen(*args)
         B, G = rows.shape[:2]
@@ -378,9 +377,10 @@ def shortcut_rows_case():
             status[i] = codes.index(inst.problem_data.return_code)
             if s_ is not None:
                 sd[i], sdd[i] = s_, u_
-        data.update({name + "_K": K, name + "_sd": sd, name + "_sdd": sdd, name + "_status": status})
+        # one file per set keeps each fixture under 1 MB
+        np.savez_compressed(os.path.join(HERE, "shortcut_rows_%s.npz" % name),
+                            **{name + "_K": K, name + "_sd": sd, name + "_sdd": sdd, name + "_status": status})
         print("shortcut rows", name, "status histogram", np.bincount(status, minlength=5))
-    np.savez_compressed(os.path.join(HERE, "shortcut_rows.npz"), **data)
 
 
 def joint_torque_case():
@@ -588,6 +588,95 @@ def frows_batch_case():
           "| ubound status", ub_status)
 
 
+def oracle_vs_reference_case():
+    """oracle_vs_reference.npz: the reference's solves for tests/test_reference_plugin.py's batched entry, and its public
+    API (per module, its public toppra classes -- member -> argument names, None where not a plain callable -- and
+    functions, in dir() order) as UTF-8 JSON for tests/test_oracle_vs_reference.py.  The other tests of that module
+    record their reference session themselves: TB_RECORD_REFERENCE=1 python -m pytest tests/test_oracle_vs_reference.py"""
+    import json
+    import inspect
+    data = {}
+    # tests/test_reference_plugin.py::test_plugin_batched_entry_equals_reference
+    from problems import make_batch
+    bss, bway, bvlim, balim = make_batch(24, 1000)
+    for b in range(24):
+        inst = algo.TOPPRA([constraint.JointVelocityConstraint(bvlim[b]), constraint.JointAccelerationConstraint(balim[b])],
+                           ta.SplineInterpolator(bss, bway[b]), gridpoints=np.linspace(0, 1, 120), solver_wrapper="seidel")
+        sdd, sd, _, K = inst.compute_parameterization(0, 0, return_data=True)
+        data.update({"plugin%d_K" % b: K, "plugin%d_sd" % b: sd, "plugin%d_sdd" % b: sdd})
+
+    def params(f):
+        try:
+            return [q for q in inspect.signature(f).parameters if q not in ("args", "kwargs")]
+        except (TypeError, ValueError):
+            return None
+
+    import toppra.interpolator
+    import toppra.parametrizer
+    import toppra.simplepath
+    import toppra.solverwrapper
+    api = []
+    for modname in ("toppra", "toppra.algorithm", "toppra.constraint", "toppra.parametrizer", "toppra.interpolator",
+                    "toppra.simplepath", "toppra.solverwrapper"):
+        mod = sys.modules[modname]
+        entries = []
+        for name in dir(mod):
+            obj = getattr(mod, name)
+            if name.startswith("_"):
+                continue
+            if inspect.isclass(obj) and obj.__module__.startswith("toppra"):
+                members = {}
+                for member in ["__init__"] + [m for m in dir(obj) if not m.startswith("_")]:
+                    f = getattr(obj, member)
+                    members[member] = params(f) if callable(f) and not isinstance(f, type) else None
+                entries.append({"name": name, "kind": "class", "members": members})
+            elif inspect.isfunction(obj) and obj.__module__.startswith("toppra"):
+                entries.append({"name": name, "kind": "function", "params": params(obj)})
+        api.append({"module": modname, "entries": entries})
+    data["reference_api"] = np.frombuffer(json.dumps(api, sort_keys=True).encode(), dtype=np.uint8)
+    np.savez_compressed(os.path.join(HERE, "oracle_vs_reference.npz"), **data)
+    print("oracle_vs_reference: %d arrays; reference_api: %d modules" % (len(data), len(api)))
+
+
+FUZZ_SEEDS = range(400000, 400120)
+FUZZ_PARTS = 8
+
+
+def fuzz_case():
+    """The reference's side of tests/test_oracle_vs_reference.py::test_randomly_shaped_problems_vs_reference: the checks of
+    scripts/fuzz_oracle_vs_reference.py on seeds FUZZ_SEEDS, run against a recording of the reference
+    (tests/ref_replay.py) -> fuzz_slice_<part>.npz (one log per seed, seeds dealt round-robin over the parts)."""
+    import importlib.util
+    from ref_replay import Recorder, save_logs
+    spec = importlib.util.spec_from_file_location("fuzz_oracle_vs_reference",
+                                                  os.path.join(ROOT, "scripts", "fuzz_oracle_vs_reference.py"))
+    fuzz = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(fuzz)
+    logs = {}
+    try:
+        for seed in FUZZ_SEEDS:
+            rec = Recorder(ta)
+            fuzz.use(rec)
+            rng = np.random.RandomState(seed)
+            p = fuzz.random_problem(rng)
+            try:
+                for check in (fuzz.check_solve, fuzz.check_frows, fuzz.check_sd_and_reachable, fuzz.check_torque,
+                              fuzz.check_parametrizers, fuzz.check_ubound, fuzz.check_other_constraints, fuzz.check_batch,
+                              fuzz.check_robust_params):
+                    check(p) if check is fuzz.check_solve else check(p, rng)
+            except AssertionError:
+                raise
+            except Exception:
+                pass
+            logs[str(seed)] = rec.log
+    finally:
+        fuzz.release()
+    keys = list(logs)
+    for part in range(FUZZ_PARTS):               # several files keep each fixture under 1 MB
+        save_logs(os.path.join(HERE, "fuzz_slice_%d.npz" % part), {k: logs[k] for k in keys[part::FUZZ_PARTS]})
+    print("fuzz slice: %d seeds, %d logged operations, checks %s" % (len(logs), sum(map(len, logs.values())), fuzz.COUNTS))
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1 and sys.argv[1] == "shortcut_rows":
         shortcut_rows_case()
@@ -601,9 +690,15 @@ if __name__ == "__main__":
         frows_batch_case()
     elif len(sys.argv) > 1 and sys.argv[1] == "periodic":
         periodic_case()
+    elif len(sys.argv) > 1 and sys.argv[1] == "oracle_vs_reference":
+        oracle_vs_reference_case()
+    elif len(sys.argv) > 1 and sys.argv[1] == "fuzz":
+        fuzz_case()
     else:
         main()
         joint_torque_case()
         other_paths_case()
         frows_batch_case()
         periodic_case()
+        oracle_vs_reference_case()
+        fuzz_case()

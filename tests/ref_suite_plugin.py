@@ -1,5 +1,5 @@
 """pytest plugin (-p ref_suite_plugin) used by tests/test_reference_suite_dropin.py: makes `import toppra` resolve to
-toppra_b200, so that the reference's OWN, unmodified test files (read in place from /root/reference/tests, never copied)
+toppra_b200, so that the reference's OWN, unmodified test files (read in place from the reference checkout, never copied)
 exercise this package's reference-facing API.  Without a GPU the kernels are replaced by the oracle-backed test double
 (tests/cpu_engine.py) — what such a run proves is the API surface: names, argument meaning, return shapes, error
 behaviour.  With TB_REF_SUITE_ENGINE=gpu the real engine is used."""

@@ -1,7 +1,7 @@
 """CPU: the ctypes layer between the Python host and the C-ABI, checked without a GPU.
 
 1. Every prototype in toppra_b200/_lib.py agrees with the declaration in include/toppra_b200.h (argument count and kind:
-   pointer / int / double) — a mismatch there would be undefined behaviour on the GPU box, not an exception.
+   pointer / int / double) — a mismatch there would be undefined behaviour on the GPU, not an exception.
 2. Every tensor-level function of toppra_b200/engine.py is run on CPU tensors against a RECORDING library: no kernel runs,
    but the call each function would make is checked against its prototype (count, ints are ints, pointers are tensors'
    data pointers or NULL), the launch flags are checked for the modes that have them, and the shape / dtype validation is

@@ -1,25 +1,37 @@
-"""CPU: live differential test of the oracle against the UNMODIFIED reference build (oracle/_ref), on random
-problems beyond the committed fixtures.  Skipped where oracle/_ref was not built (run oracle/build_ref.sh
-where /root/reference exists; the build travels to the GPU box)."""
+"""CPU: differential test of the oracle (and of the package's host code on the engine double) against the UNMODIFIED
+reference on random problems beyond the other fixtures.  The reference's side of each test is replayed from its recorded
+session (tests/ref_replay.py): tests/golden/reference_session.npz, tests/golden/fuzz_slice_*.npz and the public API in
+tests/golden/oracle_vs_reference.npz.  Re-record with TB_RECORD_REFERENCE=1 where oracle/_ref is built (the
+campaign slice and the API: tests/golden/make_golden.py fuzz / oracle_vs_reference)."""
+import os
 import warnings
 
 import numpy as np
 import pytest
 
 from oracle import oracle as orc
-from oracle.ref_loader import load_reference, reference_available
 from problems import make_path
+from ref_replay import Recorder, Replayer, load_logs, save_logs
 
-pytestmark = pytest.mark.skipif(not reference_available(), reason="oracle/_ref not built")
+SESSION = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_session.npz")
 
 
-@pytest.fixture(scope="module")
-def ref():
-    warnings.filterwarnings("ignore")
-    ta = load_reference()
-    import toppra.algorithm as algo
-    import toppra.constraint as constraint
-    return ta, algo, constraint
+@pytest.fixture
+def ref(request):
+    """(toppra, toppra.algorithm, toppra.constraint) of the reference for one test: replayed from SESSION, or, with
+    TB_RECORD_REFERENCE=1, the live build (oracle/_ref) recorded into SESSION."""
+    if os.environ.get("TB_RECORD_REFERENCE"):
+        from oracle.ref_loader import load_reference
+        warnings.filterwarnings("ignore")
+        ta = Recorder(load_reference())
+        yield ta, ta.algorithm, ta.constraint
+        logs = load_logs(SESSION) if os.path.exists(SESSION) else {}
+        logs[request.node.name] = ta.log
+        save_logs(SESSION, logs)
+    else:
+        ta = Replayer(load_logs(SESSION)[request.node.name])
+        yield ta, ta.algorithm, ta.constraint
+        assert ta.done(), "the recorded session has more steps than the test asked for"
 
 
 @pytest.mark.parametrize("vel_active", [False, True])
@@ -47,7 +59,7 @@ def test_random_paths_bit_exact(ref, vel_active):
 
 def test_lp_shims_random(ref):
     """Random LPs with random warm-start pairs through the reference's solve_lp2d shim (pyx:65-87)."""
-    import toppra.solverwrapper.cy_seidel_solverwrapper as seidel
+    seidel = ref[0].solverwrapper.cy_seidel_solverwrapper
     rng = np.random.RandomState(0)
     for trial in range(300):
         n = rng.randint(1, 40)
@@ -145,9 +157,8 @@ def test_propose_gridpoints_and_spline_time_stamps_random_vs_reference(ref, monk
     recurrence against the reference on random paths / velocity profiles with stalls and dropped knots."""
     ta, algo, constraint = ref
     import torch
-    import toppra.interpolator as interp
-    from toppra.parametrizer import ParametrizeSpline
     import cpu_engine
+    interp, ParametrizeSpline = ta.interpolator, ta.parametrizer.ParametrizeSpline
     ss = np.linspace(0, 1, 5)
     rng = np.random.RandomState(23)
     for seed in range(7000, 7008):
@@ -229,14 +240,20 @@ def test_univariate_spline_interpolator_vs_reference(ref, monkeypatch):
         np.testing.assert_allclose(sdd2, sdd, rtol=1e-6, atol=1e-7)
 
 
-def test_randomly_shaped_problems_vs_reference(ref):
+def test_randomly_shaped_problems_vs_reference(golden):
     """A slice of the campaign of scripts/fuzz_oracle_vs_reference.py (dof 1..14, 2..12 knots, 2..400 gridpoints, non-uniform
     knots and grids, every boundary condition, both discretisations, non-zero boundary velocities, tiny motions): spline
     coefficients, K, sd, u, status, feasible sets, propose_gridpoints, time stamps, TOPPRAsd, reachable sets, torque rows,
     both output parametrizers —
-    bit for bit against the reference (31 000 + 10 000 problems in the full runs, profiles/r02_fuzz_oracle_vs_reference.txt)."""
+    bit for bit against the reference.  The reference's side of every check is replayed from its recorded session
+    (tests/golden/fuzz_slice_*.npz, tests/ref_replay.py; tests/golden/make_golden.py fuzz); a check that asks the
+    reference anything the recording did not see fails with ReplayOutOfStep."""
     import importlib.util
     import os
+    from ref_replay import Replayer, load_logs
+    logs = {}
+    for part in range(8):
+        logs.update(load_logs(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "fuzz_slice_%d.npz" % part)))
     spec = importlib.util.spec_from_file_location(
         "fuzz_oracle_vs_reference", os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "scripts",
                                                  "fuzz_oracle_vs_reference.py"))
@@ -244,6 +261,8 @@ def test_randomly_shaped_problems_vs_reference(ref):
     spec.loader.exec_module(fuzz)
     try:
         for seed in range(400000, 400120):
+            reference = Replayer(logs[str(seed)])
+            fuzz.use(reference)
             rng = np.random.RandomState(seed)
             p = fuzz.random_problem(rng)
             try:
@@ -260,22 +279,19 @@ def test_randomly_shaped_problems_vs_reference(ref):
                 raise AssertionError("seed %d: %s" % (seed, e))
             except Exception:
                 pass            # the reference itself rejected the input (as in the campaign)
+            assert reference.done(), "seed %d: the recorded session has more steps than the replay asked for" % seed
     finally:
         fuzz.release()          # the campaign installs the engine double process-wide
     assert fuzz.COUNTS.get("TOPPRAsd", 0) >= 10 and fuzz.COUNTS.get("propose_gridpoints", 0) >= 80
 
 
-def test_public_classes_have_the_reference_methods_and_arguments(ref):
-    """Introspection of the reference build against this package: every public class the two share has the reference's public
-    methods / properties, and every shared callable takes the reference's argument names in the reference's order."""
+def test_public_classes_have_the_reference_methods_and_arguments(golden):
+    """Introspection of the reference build (its public API as stored in tests/golden/oracle_vs_reference.npz) against this
+    package: every public class the two share has the reference's public methods / properties, and every shared callable
+    takes the reference's argument names in the reference's order."""
     import inspect
-    import toppra
-    import toppra.algorithm
-    import toppra.constraint
-    import toppra.interpolator
-    import toppra.parametrizer
-    import toppra.simplepath
-    import toppra.solverwrapper
+    import json
+    import os
     import toppra_b200 as tb
     import toppra_b200.simplepath
 
@@ -285,34 +301,36 @@ def test_public_classes_have_the_reference_methods_and_arguments(ref):
         except (TypeError, ValueError):
             return None
 
+    api = json.loads(golden("oracle_vs_reference")["reference_api"].tobytes().decode())
     openrave_only = {"compute_rave_trajectory"}
     seen, problems = set(), []
-    pairs = ((toppra, tb), (toppra.algorithm, tb.algorithm), (toppra.constraint, tb.constraint),
-             (toppra.parametrizer, tb.parametrizer), (toppra.interpolator, tb.interpolator),
-             (toppra.simplepath, tb.simplepath), (toppra.solverwrapper, tb.solverwrapper))
-    for mod_r, mod_t in pairs:
-        for name in dir(mod_r):
-            obj = getattr(mod_r, name)
-            if name.startswith("_") or name in seen or not hasattr(mod_t, name):
+    mods = {"toppra": tb, "toppra.algorithm": tb.algorithm, "toppra.constraint": tb.constraint,
+            "toppra.parametrizer": tb.parametrizer, "toppra.interpolator": tb.interpolator,
+            "toppra.simplepath": tb.simplepath, "toppra.solverwrapper": tb.solverwrapper}
+    assert [m["module"] for m in api] == list(mods)
+    for mod in api:
+        mod_t = mods[mod["module"]]
+        for entry in mod["entries"]:
+            name = entry["name"]
+            if name in seen or not hasattr(mod_t, name):
                 continue
             mine = getattr(mod_t, name)
-            if inspect.isclass(obj) and obj.__module__.startswith("toppra"):
+            if entry["kind"] == "class":
                 seen.add(name)
-                for member in ["__init__"] + [m for m in dir(obj) if not m.startswith("_")]:
+                for member, pr in entry["members"].items():
                     if member in openrave_only:
                         continue
                     if not hasattr(mine, member):
                         problems.append("%s.%s missing" % (name, member))
                         continue
-                    fr, ft = getattr(obj, member), getattr(mine, member)
-                    pr, pt = (params(fr), params(ft)) if callable(fr) and not isinstance(fr, type) else (None, None)
+                    pt = params(getattr(mine, member)) if pr is not None else None
                     if pr is not None and pt is not None and [a for a in pr if a in pt] != pr:
                         problems.append("%s.%s(%s) vs (%s)" % (name, member, ", ".join(pr), ", ".join(pt)))
                     elif pr is not None and pt is not None and pt[:len(pr)] != pr and [a for a in pt if a in pr] != pr:
                         problems.append("%s.%s argument order" % (name, member))
-            elif inspect.isfunction(obj) and obj.__module__.startswith("toppra"):
+            else:
                 seen.add(name)
-                pr, pt = params(obj), params(mine)
+                pr, pt = entry["params"], params(mine)
                 if pr is not None and pt is not None and pt[:len(pr)] != pr:
                     problems.append("%s(%s) vs (%s)" % (name, ", ".join(pr), ", ".join(pt)))
     assert len(seen) >= 25, sorted(seen)

@@ -1,8 +1,9 @@
 """GPU (-m gpu): the drop-in claim of INTEGRATION.md section 2, executed.  The UNMODIFIED reference (oracle/_ref, built
-from /root/reference by oracle/build_ref.sh and shipped to the GPU box) gets the solver-wrapper name "b200" from
-examples/reference_plugin/b200_solverwrapper.py (pure ctypes over the C-ABI, no torch, none of this repo's Python
-package) and its OWN TOPPRA class must return identical arrays with solver_wrapper="b200" and "seidel" — controllable
-sets, velocities, accelerations, return code and the re-splined trajectory."""
+by oracle/build_ref.sh) gets the solver-wrapper name "b200" from examples/reference_plugin/b200_solverwrapper.py (pure
+ctypes over the C-ABI, no torch, none of this repo's Python package) and its OWN TOPPRA class must return identical
+arrays with solver_wrapper="b200" and "seidel" — controllable sets, velocities, accelerations, return code and the
+re-splined trajectory.  Those two tests run only where oracle/_ref is built; the plugin's batched entry is checked
+against the reference's stored results (tests/golden/oracle_vs_reference.npz) everywhere."""
 import importlib.util
 import os
 
@@ -16,15 +17,20 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
-def ref():
+def plugin():
+    spec = importlib.util.spec_from_file_location(
+        "b200_solverwrapper", os.path.join(ROOT, "examples", "reference_plugin", "b200_solverwrapper.py"))
+    module = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(module)
+    return module
+
+
+@pytest.fixture(scope="module")
+def ref(plugin):
     from oracle.ref_loader import load_reference, reference_available
     if not reference_available():
         pytest.skip("oracle/_ref (the built reference) is not present")
     ta = load_reference()
-    spec = importlib.util.spec_from_file_location(
-        "b200_solverwrapper", os.path.join(ROOT, "examples", "reference_plugin", "b200_solverwrapper.py"))
-    plugin = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(plugin)
     plugin.install(ta)
     return ta, plugin
 
@@ -75,18 +81,14 @@ def test_reference_compute_trajectory_through_b200(ref):
         assert np.array_equal(traj["b200"](ts, order), traj["seidel"](ts, order))
 
 
-def test_plugin_batched_entry_equals_reference(ref):
-    """solve_velacc(B paths) == the reference solved path by path."""
-    ta, plugin = ref
-    import toppra.algorithm as algo
-    import toppra.constraint as constraint
+def test_plugin_batched_entry_equals_reference(plugin, golden):
+    """solve_velacc(B paths) == the reference's TOPPRA(seidel) solved path by path (stored results)."""
     from problems import make_batch
+    g = golden("oracle_vs_reference")
     B, G = 24, 120
     ss, way, vlim, alim = make_batch(B, 1000)
     grid = np.linspace(0, 1, G)
     u, sd, K, status = plugin.solve_velacc(ss, way, grid, vlim, alim)
     for b in range(B):
-        inst = algo.TOPPRA([constraint.JointVelocityConstraint(vlim[b]), constraint.JointAccelerationConstraint(alim[b])],
-                           ta.SplineInterpolator(ss, way[b]), gridpoints=grid, solver_wrapper="seidel")
-        sdd_r, sd_r, _, K_r = inst.compute_parameterization(0, 0, return_data=True)
+        sdd_r, sd_r, K_r = g["plugin%d_sdd" % b], g["plugin%d_sd" % b], g["plugin%d_K" % b]
         assert status[b] == 0 and np.array_equal(K[b], K_r) and np.array_equal(sd[b], sd_r) and np.array_equal(u[b], sdd_r)

@@ -1,7 +1,8 @@
 """The reference's OWN test-suite, unmodified and read in place, run against this package.
 
 `tests/ref_suite_plugin.py` makes `import toppra` resolve to `toppra_b200`; pytest then collects the reference's test
-files where they lie (`/root/reference/tests/tests`, or $TB_REFERENCE_TESTS) — nothing is copied into this repository.
+files where they lie (`$TOPPRA_REFERENCE/tests/tests`, default /root/reference, or $TB_REFERENCE_TESTS) — nothing is
+copied into this repository.
 This is the drop-in claim in executable form: the reference's tests of its public API (interpolators, constraints,
 solver-wrapper interface incl. `cy_seidel_solverwrapper.solve_lp1d / solve_lp2d / seidelWrapper`, TOPPRA / TOPPRAsd,
 parametrizers, error behaviour) pass against toppra_b200.
@@ -19,7 +20,7 @@ independent solver rather than skip.
 
 Without a GPU the kernels are replaced by the oracle-backed double (tests/cpu_engine.py): what this run proves is the API
 surface and the host logic.  The `gpu` variant runs the same suite on the real engine wherever a reference checkout is
-available next to a GPU (on the round-end GPU box there is none: it skips)."""
+available next to a GPU, and skips where there is none."""
 import os
 import re
 import subprocess
@@ -29,7 +30,7 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF_TESTS = os.environ.get("TB_REFERENCE_TESTS", "/root/reference/tests")
+REF_TESTS = os.environ.get("TB_REFERENCE_TESTS", os.path.join(os.environ.get("TOPPRA_REFERENCE", "/root/reference"), "tests"))
 SUITE = os.path.join(REF_TESTS, "tests")
 DESELECT = "not qpoases and not cvxpy and not (test_basic_can_linear and ecos)"
 IGNORE = ["cpp", "solverwrapper/test_ecos_wrapper.py", "retime/robustness/test_robustness_main.py"]

@@ -1,8 +1,8 @@
-"""toppra_b200 — batched TOPP-RA (time-optimal path parameterisation by reachability analysis) on NVIDIA B200.
+"""toppra_b200 — batched TOPP-RA (time-optimal path parameterisation by reachability analysis) on NVIDIA H100.
 
 Keeps the public names of hungpham2511/toppra (`SplineInterpolator`, `constraint.*`, `algorithm.TOPPRA`,
 `ParametrizeSpline`, ...) and adds the batched entry points `BatchSplineInterpolator` / `BatchTOPPRA`.
-All numbers come from hand-written sm_100a CUDA kernels behind the C-ABI in include/toppra_b200.h; there is no
+All numbers come from hand-written sm_90a CUDA kernels behind the C-ABI in include/toppra_b200.h; there is no
 CPU fallback (importing works anywhere, computing needs the GPU and the built libtoppra_b200.so)."""
 import logging
 

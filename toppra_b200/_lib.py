@@ -77,7 +77,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 "toppra_b200: %s not found. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a). There is no CPU fallback." % LIB_PATH)
+                "(nvcc, sm_90a). There is no CPU fallback." % LIB_PATH)
         lib = ctypes.CDLL(LIB_PATH)
         for name, (argtypes, restype) in _PROTOS.items():
             fn = getattr(lib, name)  # AttributeError if the symbol is missing: loud on purpose
@@ -111,7 +111,7 @@ def ptr(t):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise RuntimeError("toppra_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise RuntimeError("toppra_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     return torch
 
 

@@ -25,6 +25,14 @@ int check_launch(const char *what) {
   return 0;
 }
 
+int num_sms() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      n <= 0)
+    return 132;
+  return n;
+}
+
 }  // namespace tb
 
 extern "C" int tb_version(void) { return TB_VERSION; }

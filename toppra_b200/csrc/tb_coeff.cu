@@ -530,7 +530,7 @@ extern "C" int tb_rows_canlinear(const double *a, const double *b, const double 
   const long total = (long)B * G * nrows;
   const int threads = 256;
   long blocks = (total + threads - 1) / threads;
-  if (blocks > 148L * 32) blocks = 148L * 32;
+  if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
   rows_canlinear_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(a, b, c, F, g, F_mode, B, G, m, k, grid,
                                                                                grid_shared, interp, records, W,
                                                                                R_total, row0);
@@ -543,7 +543,7 @@ extern "C" int tb_init_bounds(double *records, int B, int G, int W, int R_total,
   const long BG = (long)B * G;
   const int threads = 256;
   long blocks = (BG + threads - 1) / threads;
-  if (blocks > 148L * 32) blocks = 148L * 32;
+  if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
   init_bounds_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(records, BG, W, R_total);
   return check_launch("tb_init_bounds");
 }
@@ -560,7 +560,7 @@ extern "C" int tb_xbound_varying(const double *ppoly, const double *breaks, int 
   const long total = (long)B * G;
   const int threads = 128;
   long blocks = (total + threads - 1) / threads;
-  if (blocks > 148L * 64) blocks = 148L * 64;
+  if (blocks > (long)num_sms() * 64) blocks = (long)num_sms() * 64;
   xbound_varying_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(
       ppoly, breaks, breaks_shared, B, nseg, dof, grid, grid_shared, G, vlim_grid, vlim_shared, 1, records, W, R_total,
       write_xbound);
@@ -613,7 +613,7 @@ extern "C" int tb_xbound_velocity(const double *ppoly, const double *breaks, int
   const long total = (long)B * G;
   const int threads = 128;
   long blocks = (total + threads - 1) / threads;
-  if (blocks > 148L * 64) blocks = 148L * 64;
+  if (blocks > (long)num_sms() * 64) blocks = (long)num_sms() * 64;
   xbound_varying_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(
       ppoly, breaks, breaks_shared, B, nseg, dof, grid, grid_shared, G, vlim, lim_shared, 0, records, W, R_total,
       write_xbound);

@@ -1,4 +1,4 @@
-// tb_common.cuh — shared constants and helpers of libtoppra_b200 (sm_100a only).
+// tb_common.cuh — shared constants and helpers of libtoppra_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -65,5 +65,7 @@ __device__ __forceinline__ double ppoly_eval1(const double *__restrict__ c, cons
 
 void set_error(const char *fmt, ...);
 int check_launch(const char *what);
+// multiprocessor count of the current device (132 on an H100 SXM): sizes grid-stride launches and one-wave batches
+int num_sms();
 
 }  // namespace tb

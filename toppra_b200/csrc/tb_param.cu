@@ -104,7 +104,7 @@ extern "C" int tb_constaccel_eval(const double *ppoly, const double *breaks, int
   const long total = (long)B * M * dof;
   const int threads = 256;
   long blocks = (total + threads - 1) / threads;
-  if (blocks > 148L * 64) blocks = 148L * 64;
+  if (blocks > (long)num_sms() * 64) blocks = (long)num_sms() * 64;
   constaccel_eval_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(
       ppoly, breaks, breaks_shared, nseg, dof, grid, grid_shared, sd, t_grid, us, B, G, ts, ts_shared, M, order, out);
   return check_launch("tb_constaccel_eval");

@@ -7,7 +7,7 @@
 //   seidelWrapper.solve_stagewise_optim                           cy_seidel_solverwrapper.pyx:549-697
 //   cy_solve_lp2d / cy_solve_lp1d                                 cy_seidel_solverwrapper.pyx:149-390 / 93-144
 //
-// Design (B200): the stages of one path are strictly sequential (K[i] <- K[i+1], x[i+1] <- x[i]), so the
+// Design: the stages of one path are strictly sequential (K[i] <- K[i+1], x[i+1] <- x[i]), so the
 // parallelism is (i) across paths: one warp per path, and (ii) across the LP rows of a stage: one row per lane
 // (RPL rows per lane when nC > 32).  Seidel's incremental 2-variable LP keeps its exact row order (including
 // the reference's warm-start permutation) so results are bit-identical to the Cython solver:
@@ -999,11 +999,13 @@ constexpr int SCAN_WARPS = TB_SCAN_WARPS;  // 1: a finished path frees its slot 
 #endif
 
 #ifndef TB_SCAN_RPL2_WARPS_PER_SM
-#define TB_SCAN_RPL2_WARPS_PER_SM 20  // measured on cfg 3 (16384 x 500, nC = 50): free choice (150 regs) 19.0 ms, 16: 16.2, 20 (96 regs): 15.5, 24 (80 regs): 15.7
+// resident warps per SM for nC in (32, 64]; TB_SCAN_RPL2_OCC=16|20|24 overrides.  H100 80GB (400 W), cfg 3 scan (16384 x 500,
+// nC = 50), two runs: 16 -> 24.1 / 23.6 ms, 20 -> 23.1 / 22.9 ms, 24 (80 registers) -> 22.6 / 22.4 ms
+#define TB_SCAN_RPL2_WARPS_PER_SM 24
 #endif
 
 #ifndef TB_SCAN_FUSED_WARPS_PER_SM
-#define TB_SCAN_FUSED_WARPS_PER_SM 28  // 72 registers: 28 x 148 = 4144 resident paths still cover the 4096-path batch in one wave (measured r02: 1.317 vs 1.339 ms at 32)
+#define TB_SCAN_FUSED_WARPS_PER_SM 28  // 72 registers: 28 resident one-warp CTAs per SM
 #endif
 
 template <int RPL>
@@ -1014,7 +1016,7 @@ int launch_scan(const double *records, int W, int R, const double *grid, int gri
   const size_t smem = (size_t)SCAN_WARPS * SCAN_NBUF * W * sizeof(double) + SCAN_WARPS * SCAN_NBUF * sizeof(uint64_t) +
                       SCAN_WARPS * 4 * sizeof(void *);
   // Two register budgets for the common nC <= 32 case: 64 registers (32 one-warp CTAs per SM: the 4096-path batch
-  // of BASELINE cfg 2 is a single wave on 148 SMs) or the compiler's free choice.  TB_SCAN_OCC=free|dense overrides.
+  // of BASELINE cfg 2 is a single wave on 132 SMs) or the compiler's free choice.  TB_SCAN_OCC=free|dense overrides.
   static const char *occ_env = getenv("TB_SCAN_OCC");
   const bool dense = occ_env ? (occ_env[0] == 'd') : true;
   constexpr int MINB = (RPL == 1 ? TB_SCAN_WARPS_PER_SM / SCAN_WARPS : 1);
@@ -1034,8 +1036,8 @@ int launch_scan(const double *records, int W, int R, const double *grid, int gri
                   : scan_kernel<RPL, SCAN_WARPS, MINB, false, TB_SCAN_FORWARD_ONLY>;
   }
   if constexpr (RPL == 2) {
-    // nC in (32, 64] (BASELINE cfg 3: 50 rows).  Left alone the compiler takes 150 registers: 13 resident warps per SM
-    // and issue slots 54 % busy (profiles/r02_ncu_cfg3.txt).  Capped builds trade a few spills for residency.
+    // nC in (32, 64] (BASELINE cfg 3: 50 rows).  Left alone the compiler takes about 150 registers (13 resident warps
+    // per SM); capped builds trade a few spills for residency.
     static const char *rpl2_env = getenv("TB_SCAN_RPL2_OCC");
     const int occ2 = rpl2_env ? atoi(rpl2_env) : TB_SCAN_RPL2_WARPS_PER_SM;
     if (!fast && !counters) {
@@ -1087,11 +1089,12 @@ int launch_scan_velacc(const VelAccSrc &src, int W, int R, const double *grid, i
                        const double *sd_start, const double *sd_end, const double *sd_end_hi, int flags, double *K,
                        double *sd, double *u, int *status, int *fail_stage, int *counters, const int *glen,
                        cudaStream_t stream) {
-  // Register budget by batch size (measured r02, B200): up to 28 x 148 = 4144 paths the 72-register build holds the
-  // whole batch in one wave and wins (1.317 vs 1.339 ms at 4096 paths); larger batches are issue-bound and want the 32
-  // resident warps per SM of the 64-register build (2^20 paths: 290.7 vs 308.8 ms).  TB_SCAN_FUSED_OCC=28|32 overrides.
+  // Register budget by batch size: while 28 resident one-warp CTAs per SM cover the whole batch in one wave, the
+  // 72-register build is used; larger batches are issue-bound and want the 32 resident warps per SM of the 64-register
+  // build.  TB_SCAN_FUSED_OCC=28|32 overrides.
   static const char *occ_env = getenv("TB_SCAN_FUSED_OCC");
-  const int occ = occ_env ? atoi(occ_env) : ((long)B <= 148L * TB_SCAN_FUSED_WARPS_PER_SM ? TB_SCAN_FUSED_WARPS_PER_SM : 32);
+  const int occ = occ_env ? atoi(occ_env)
+                          : ((long)B <= (long)num_sms() * TB_SCAN_FUSED_WARPS_PER_SM ? TB_SCAN_FUSED_WARPS_PER_SM : 32);
   const int mode = flags & (TB_SCAN_BACKWARD_ONLY | TB_SCAN_SD_FORWARD | TB_SCAN_SD_SLOW | TB_SCAN_FORWARD_ONLY);
   if ((mode == 0 || mode == TB_SCAN_FORWARD_ONLY) && !counters && !glen && forward_threads_supported(src.dof, B)) {
     // large batches (issue-bound): the forward pass runs with one thread per path (tb_scan_fwd.cu) after a backward-only

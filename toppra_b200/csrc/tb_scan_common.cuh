@@ -61,7 +61,9 @@ bool scan_velacc_pair_supported(int dof, int interp, int nseg, int flags);
 // forward pass with one thread per path (tb_scan_fwd.cu), for large batches: reads K / status / fail_stage of a
 // TB_SCAN_BACKWARD_ONLY launch
 #ifndef TB_SCAN_FWD_THREADS_MIN_DEFAULT
-#define TB_SCAN_FWD_THREADS_MIN_DEFAULT 24576  // measured (B200, 7-DOF, 200 gridpoints): 16384 paths 4.78 vs 4.65 ms (warp form wins), 32768: 8.19 vs 8.98 ms, 65536: 16.1 vs 17.7, 2^20 in 131072-path chunks: 263 vs 289 ms
+// smallest batch (paths) that takes the thread-per-path forward pass.  H100 80GB (400 W), 7-DOF, 200 gridpoints, fused
+// scan: 16384 paths 5.17 vs 5.36 ms (warp form), 24576: 7.33 vs 7.95 ms, 32768: 9.40 vs 10.96 ms
+#define TB_SCAN_FWD_THREADS_MIN_DEFAULT 16384
 #endif
 bool forward_threads_supported(int dof, int B);
 int launch_forward_threads(const VelAccSrc &src, int interp, const double *grid, int grid_shared, int B, int G,

@@ -1,8 +1,7 @@
 // tb_scan_pair.cu — K2 for JointVelocity + JointAcceleration problems, TWO PATHS PER WARP.  EXPERIMENT, opt-in
 // (TB_SCAN_PAIR=1: divergent half-warps, TB_SCAN_PAIR=2: lockstep): both forms are bit-identical to the one-warp-per-path
-// kernel on the whole GPU test suite and both are SLOWER on a B200 (4096 paths: 1.68 / 1.71 ms vs 1.32 ms; 2^20 paths:
-// 2.5 / 2.75 M paths/s vs 3.6 M) — see profiles/r02_pair_*_experiment_ncu.txt and DESIGN.md section 10.  The default
-// launch path does not use this file.
+// kernel on the whole GPU test suite and both were measured slower than it (DESIGN.md section 10).  The default launch
+// path does not use this file.
 //
 // Replaces the same reference functions as tb_scan.cu (reachability_algorithm.py:166-376, time_optimal_algorithm.py:55-92,
 // cy_seidel_solverwrapper.pyx:93-144, 149-390, 549-697); results are bit-identical to it and to the one-warp-per-path
@@ -492,8 +491,7 @@ scan_pair_kernel(const VelAccSrc src, const int interp, const int Wc, const doub
 
 // ======================================================================================================================
 // LOCKSTEP form.  redux.sync and vote.sync deliver ONE result per warp, so with half-warp masks every collective of the
-// kernel above is executed once per half plus a convergence branch (measured: branch_resolving 26 % of the stall
-// samples, 1.67 ms).  Here both half-warps run ONE instruction stream: reductions are xor-butterflies of full-mask
+// kernel above is executed once per half plus a convergence branch.  Here both half-warps run ONE instruction stream: reductions are xor-butterflies of full-mask
 // shuffles (offsets 8, 4, 2, 1 stay inside a half), votes are one full-mask ballot from which each half reads its 16 bits,
 // and what differs between the two paths — number of re-solves, shortcut taken or not, failure — is predication on
 // per-half flags instead of branches.  Same arithmetic, same results.

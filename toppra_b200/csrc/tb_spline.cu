@@ -235,7 +235,7 @@ extern "C" int tb_ppoly_eval(const double *ppoly, const double *breaks, int brea
   const long total = (long)B * G * dof;
   const int threads = 256;
   long blocks = (total + threads - 1) / threads;
-  if (blocks > 148L * 64) blocks = 148L * 64;
+  if (blocks > (long)num_sms() * 64) blocks = (long)num_sms() * 64;
   ppoly_eval_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(ppoly, breaks, breaks_shared, B, nseg, dof, s,
                                                                            s_shared, G, order, out);
   return check_launch("tb_ppoly_eval");

@@ -1,7 +1,7 @@
 """Thin tensor-level front-end of the C-ABI (toppra_b200/_lib.py -> libtoppra_b200.so).
 
 PyTorch is used for storage (device tensors), streams and H2D/D2H copies only; every number is computed by the
-hand-written sm_100a kernels in toppra_b200/csrc.  No function here has a CPU fallback."""
+hand-written sm_90a kernels in toppra_b200/csrc.  No function here has a CPU fallback."""
 import ctypes
 
 import numpy as np
