@@ -9,13 +9,13 @@ for op in UBLKCP SYNCS.ARRIVE SYNCS.PHASECHK REDUX SHFL.IDX SHFL.BFLY VOTE MUFU.
 done
 echo "# (DFMA in a -fmad=false build: only inside the IEEE division / sqrt / sincos sequences; no tensor-core instructions: there is no dense contraction)"
 echo
-echo "# record scan scan_kernel<1,1,32,false,0,false,false>: bulk copy of a stage record + mbarrier wait + redux reductions"
-awk '/Function :/ {f = (index($0, "scan_kernelILi1ELi1ELi32ELb0ELi0ELb0ELb0E") > 0)} f' /tmp/tb_lib.sass | grep -E "UBLKCP|SYNCS|REDUX|ELECT" | head -16 | sed -E 's/ +\/\* 0x[0-9a-f]+ \*\///' | cut -c1-110
+echo "# record scan scan_kernel<1,32,false,0,false,false>: bulk copy of a stage record + mbarrier wait + redux reductions"
+awk '/Function :/ {f = (index($0, "scan_kernelILi1ELi32ELb0ELi0ELb0ELb0E") > 0)} f' /tmp/tb_lib.sass | grep -E "UBLKCP|SYNCS|REDUX|ELECT" | head -16 | sed -E 's/ +\/\* 0x[0-9a-f]+ \*\///' | cut -c1-110
 echo
-echo "# fused scan scan_kernel<1,1,28,false,0,true,false> (tb_scan_velacc): no bulk copies (rows are built from the spline), redux + shuffles"
-awk '/Function :/ {f = (index($0, "scan_kernelILi1ELi1ELi28ELb0ELi0ELb1ELb0E") > 0)} f' /tmp/tb_lib.sass | grep -E "REDUX|SHFL|MUFU.RCP64H|LDS.128" | head -14 | sed -E 's/ +\/\* 0x[0-9a-f]+ \*\///' | cut -c1-110
+echo "# fused scan scan_kernel<1,28,false,0,true,false> (tb_scan_velacc): no bulk copies (rows are built from the spline), redux + shuffles"
+awk '/Function :/ {f = (index($0, "scan_kernelILi1ELi28ELb0ELi0ELb1ELb0E") > 0)} f' /tmp/tb_lib.sass | grep -E "REDUX|SHFL|MUFU.RCP64H|LDS.128" | head -14 | sed -E 's/ +\/\* 0x[0-9a-f]+ \*\///' | cut -c1-110
 echo
 echo "# static size of the scan instantiations (instructions / S2R / LDL / STL / REDUX / SHFL / RCP64H)"
-for k in ILi1ELi1ELi28ELb0ELi0ELb1ELb0E ILi1ELi1ELi32ELb0ELi0ELb1ELb0E ILi1ELi1ELi32ELb0ELi0ELb0ELb0E ILi2ELi1ELi20ELb0ELin1ELb0ELb0E; do
+for k in ILi1ELi28ELb0ELi0ELb1ELb0E ILi1ELi32ELb0ELi0ELb1ELb0E ILi1ELi32ELb0ELi0ELb0ELb0E ILi2ELi24ELb0ELin1ELb0ELb0E; do
   printf "%-36s " "scan_kernel<$k>"; scripts/sass_stats.sh $k toppra_b200/csrc/tb_scan.o
 done

@@ -17,14 +17,8 @@
 namespace tb {
 namespace {
 
-#ifndef TB_COEFF_THREADS
-#define TB_COEFF_THREADS 128
-#endif
-#ifndef TB_COEFF_CH
-#define TB_COEFF_CH 32
-#endif
-constexpr int COEFF_THREADS = TB_COEFF_THREADS;
-constexpr int COEFF_CH_SMALL = 32, COEFF_CH_LARGE = TB_COEFF_CH;  // gridpoints per CTA
+constexpr int COEFF_THREADS = 128;
+constexpr int CH = 32;  // gridpoints per CTA
 
 __device__ __forceinline__ int R_total_or1(int R_total) { return R_total > 0 ? R_total : 1; }
 
@@ -36,7 +30,6 @@ __device__ __forceinline__ int R_total_or1(int R_total) { return R_total > 0 ? R
 //   tab  [W]            per record column: offset into vec (bit 15 = negate, 0x7fff = column not owned)
 // Phase 2: every thread owns one 16-byte column pair and walks down the gridpoints:
 //   rec[ci][col] = +-vec[ci][tab[col]]  -> two shared loads + one coalesced 16-byte store per iteration.
-template <int CH>
 __global__ void __launch_bounds__(COEFF_THREADS)
 coeff_velacc_kernel(const double *__restrict__ ppoly, const double *__restrict__ breaks, const int breaks_shared,
                     const int nseg, const int dof, const double *__restrict__ grid, const int grid_shared, const int G,
@@ -493,7 +486,6 @@ extern "C" int tb_coeff_velacc(const double *ppoly, const double *breaks, int br
   }
   if (R_total > MAX_ROWS) { set_error("tb_coeff_velacc: R=%d > %d", R_total, MAX_ROWS); return TB_ERR_UNSUPPORTED; }
   if (6 * dof + 3 >= 0x7fff) { set_error("tb_coeff_velacc: dof=%d too large", dof); return TB_ERR_UNSUPPORTED; }
-  const int CH = (G > 96) ? COEFF_CH_LARGE : COEFF_CH_SMALL;
   const int nchunks = (G + CH - 1) / CH;
   const long blocks = (long)B * nchunks;
   if (blocks > 0x7fffffffL) { set_error("tb_coeff_velacc: batch too large for one launch"); return TB_ERR_UNSUPPORTED; }
@@ -501,12 +493,11 @@ extern "C" int tb_coeff_velacc(const double *ppoly, const double *breaks, int br
   const int pp_in_smem = pp_doubles * sizeof(double) <= 32 * 1024;
   const size_t smem = (size_t)((CH + 1) * dof * 2 + CH * dof * 2 + CH * (6 * dof + 3) + CH + 1 +
                                (pp_in_smem ? pp_doubles : 0)) * sizeof(double) + (size_t)W * sizeof(unsigned short) + 16;
-  auto kern = (CH == COEFF_CH_LARGE) ? coeff_velacc_kernel<COEFF_CH_LARGE> : coeff_velacc_kernel<COEFF_CH_SMALL>;
   if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(coeff_velacc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("tb_coeff_velacc: dof=%d too large for shared memory", dof); return TB_ERR_UNSUPPORTED; }
   }
-  kern<<<(unsigned)blocks, COEFF_THREADS, smem, (cudaStream_t)stream>>>(
+  coeff_velacc_kernel<<<(unsigned)blocks, COEFF_THREADS, smem, (cudaStream_t)stream>>>(
       ppoly, breaks, breaks_shared, nseg, dof, grid, grid_shared, G, vlim, alim, lim_shared, interp, records, W,
       R_total, row0, write_xbound, nchunks, pp_in_smem);
   return check_launch("tb_coeff_velacc");

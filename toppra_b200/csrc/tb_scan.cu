@@ -13,12 +13,11 @@
 // the reference's warm-start permutation) so results are bit-identical to the Cython solver:
 //   * "first violated row in order"      -> per-lane position + redux.sync min
 //   * projection of earlier rows + box   -> one fp64 division per lane
-//   * 1-D LP (min of upper / max of lower limits) -> 5-step shuffle reductions
+//   * 1-D LP (min of upper / max of lower limits) -> redux.sync min / max on a two-word order-preserving key
 // The per-stage record (3R+2 doubles) is streamed HBM -> shared memory with cp.async.bulk (TMA bulk copy,
-// mbarrier complete_tx), double-buffered one stage ahead of the solve.
+// mbarrier complete_tx) into a ring of SCAN_NBUF = 4 buffers, three stages ahead of the solve.
 // Compiled with -fmad=false: no FMA contraction, same roundings as the x86-64 reference.
 #include <limits.h>
-#include <stdlib.h>
 
 #include "tb_common.cuh"
 #include "tb_scan_common.cuh"
@@ -79,10 +78,7 @@ __device__ __forceinline__ double warp_max(double v) {
   return __hiloint2double((int)(mh ^ (unsigned)(m2 | (int)0x80000000)), (int)(ml ^ (unsigned)m2));
 }
 
-#ifndef TB_SCAN_NBUF
-#define TB_SCAN_NBUF 4
-#endif
-constexpr int SCAN_NBUF = TB_SCAN_NBUF;  // record buffers per warp (NBUF-1 stages of look-ahead)
+constexpr int SCAN_NBUF = 4;  // record buffers per warp (NBUF-1 stages of look-ahead)
 
 // One projected constraint of the 1-D sub-problem (pyx:326-347): its limit on t as an upper bound `thi` (denom >
 // TINY) or a lower bound `tlo` (denom < -TINY); +-LP_INF = no limit of that kind (the 1-D LP's own bounds);
@@ -426,8 +422,10 @@ __device__ __forceinline__ void set_xnext_rows(const int lane, const double delt
 // UB: the stage records carry a u-bound pair (ulo, uhi) behind the x-bound pair (TB_SCAN_UBOUND: `ubound` of a
 // constraint, intersected into low/high[:, 0] by seidelWrapper.__init__, pyx:512-515); otherwise u in [-1e8, 1e8].
 // glen (optional): ragged batches, path p has glen[p] <= G gridpoints (strides stay G; outputs past glen[p] are NaN).
-template <int RPL, int WARPS, int MINB, bool FAST, int CFLAGS = -1, bool FUSED = false, bool UB = false>
-__global__ void __launch_bounds__(WARPS * 32, MINB)
+// One warp per CTA (block = path): a finished path frees its slot at once (measured best: 1 < 2 < 4 warps per CTA).
+// MINB = resident one-warp CTAs per SM the register budget is sized for.
+template <int RPL, int MINB, bool FAST, int CFLAGS = -1, bool FUSED = false, bool UB = false>
+__global__ void __launch_bounds__(32, MINB)
 scan_kernel(const double *__restrict__ records, const int W, const int R, const double *__restrict__ grid,
             const int grid_shared, const int B, const int G, const double *__restrict__ sd_start,
             const double *__restrict__ sd_end, const double *__restrict__ sd_end_hi, const int flags_arg,
@@ -437,21 +435,16 @@ scan_kernel(const double *__restrict__ records, const int W, const int R, const 
   static_assert(!FUSED || RPL == 1, "the fused row source holds one row per lane");
   static_assert(!(FUSED && UB), "velocity + acceleration problems have no u-bound");
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int warp = (WARPS == 1) ? 0 : (int)(threadIdx.x >> 5);
+  // the lane is read once and kept: the optimiser otherwise re-reads the special register (S2R, ~20 cycles) at every use
+  // when it runs short of registers
   int lane;
-  if (WARPS == 1) {
-    // read once and keep: the optimiser otherwise re-reads the special register (S2R, ~20 cycles) at every use when it
-    // runs short of registers
-    asm volatile("mov.u32 %0, %%tid.x;" : "=r"(lane));
-  } else {
-    lane = (int)(threadIdx.x & 31);
-  }
-  const long path = (long)blockIdx.x * WARPS + warp;
+  asm volatile("mov.u32 %0, %%tid.x;" : "=r"(lane));
+  const long path = blockIdx.x;
   if (path >= B) return;
-  // shared-memory plan per warp.  records: ring of SCAN_NBUF stage records + mbarriers; FUSED: derivative coefficients
+  // shared-memory plan.  records: ring of SCAN_NBUF stage records + mbarriers; FUSED: derivative coefficients
   // of the path's PPoly dco [nseg][dof][5] + breakpoints [nseg+1] (in W doubles; W = that size rounded up to even)
-  double *bufs = reinterpret_cast<double *>(smem_raw) + (size_t)warp * (FUSED ? 1 : SCAN_NBUF) * W;
-  uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)WARPS * (FUSED ? 1 : SCAN_NBUF) * W * sizeof(double)) + warp * SCAN_NBUF;
+  double *bufs = reinterpret_cast<double *>(smem_raw);
+  uint64_t *bars = reinterpret_cast<uint64_t *>(smem_raw + (size_t)(FUSED ? 1 : SCAN_NBUF) * W * sizeof(double));
   // ragged batches run on the run-time-flag build (CFLAGS < 0); the specialised builds keep G as the loop bound
   const int Gp = (CFLAGS < 0 && glen) ? min(max(glen[path], 1), G) : G;  // this path's gridpoints
   const int N = Gp - 1, nC = R + 2;
@@ -459,7 +452,7 @@ scan_kernel(const double *__restrict__ records, const int W, const int R, const 
   // Per-path base pointers live in shared memory: under the 64-register cap the compiler otherwise rebuilds them
   // from blockIdx and the kernel parameters (a chain of 64-bit multiplies) at every use inside the stage loops.
   const void *volatile *sptr = reinterpret_cast<const void *volatile *>(
-      smem_raw + (size_t)WARPS * (FUSED ? 1 : SCAN_NBUF) * W * sizeof(double) + (size_t)WARPS * SCAN_NBUF * sizeof(uint64_t)) + warp * 4;
+      smem_raw + (size_t)(FUSED ? 1 : SCAN_NBUF) * W * sizeof(double) + SCAN_NBUF * sizeof(uint64_t));
   if (lane == 0) {
     sptr[0] = FUSED ? static_cast<const void *>(src.xbound + (size_t)path * G * 2)
                     : static_cast<const void *>(records + (size_t)path * G * W);
@@ -759,14 +752,20 @@ scan_kernel(const double *__restrict__ records, const int W, const int R, const 
   }
 }
 
+// Path (or LP) of a one-warp CTA of feasible_kernel, reachable_kernel and lp2d_batch_kernel: blockIdx.x.  The term
+// threadIdx.x >> 5 is 0, but it keeps the index per-thread for the compiler: as a uniform value, ptxas moves the
+// per-path addressing to the uniform datapath, and the machine code of all three kernels changes (reachable_kernel<4>
+// then spills 20-32 bytes).
+__device__ __forceinline__ long warp_path() { return (long)blockIdx.x + (int)(threadIdx.x >> 5); }
+
 // compute_feasible_sets, reachability_algorithm.py:131-164: X[i] = [min x, max x] over stage i alone
 // (x in [-1e4, 1e4], x_next in [-1e4, 1e4]); warm-start slots chained over i like the reference.
-template <int RPL, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32)
+template <int RPL>
+__global__ void __launch_bounds__(32)
 feasible_kernel(const double *__restrict__ records, const int W, const int R, const double *__restrict__ grid,
                 const int grid_shared, const int B, const int G, const int ub, double *__restrict__ Xout) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long path = (long)blockIdx.x * WARPS + warp;
+  const int lane = threadIdx.x & 31;
+  const long path = warp_path();
   if (path >= B) return;
   const int N = G - 1, nC = R + 2;
   const double *rec_path = records + (size_t)path * G * W;
@@ -838,14 +837,14 @@ __device__ __forceinline__ bool lp1d_fixed_x_active_warp(const double v0, const 
 // Reference quirks kept: the objective and the x_next formula use deltas[i - 1] (deltas[N - 1] for i = 0, Python's
 // negative index, :389-404) while rows 0/1 of the stage use deltas[i]; a stage with L[i,0] == L[i,1] takes the 1-variable
 // branch of solve_stagewise_optim and stores its active index in slot [0] only; after a NaN the remaining L stay 0.
-template <int RPL, int WARPS, bool UB>
-__global__ void __launch_bounds__(WARPS * 32)
+template <int RPL, bool UB>
+__global__ void __launch_bounds__(32)
 reachable_kernel(const double *__restrict__ records, const int W, const int R, const double *__restrict__ grid,
                  const int grid_shared, const int B, const int G, const double *__restrict__ sdmin,
                  const double *__restrict__ sdmax, double *__restrict__ Xout, double *__restrict__ Lout,
                  int *__restrict__ fail_stage) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long path = (long)blockIdx.x * WARPS + warp;
+  const int lane = threadIdx.x & 31;
+  const long path = warp_path();
   if (path >= B) return;
   const int N = G - 1, nC = R + 2;
   const double *rec_path = records + (size_t)path * G * W;
@@ -917,14 +916,14 @@ reachable_kernel(const double *__restrict__ records, const int W, const int R, c
 // Batched stand-alone LPs (one warp per LP): the device counterparts of the reference's Python shims
 // solve_lp2d / solve_lp1d (cy_seidel_solverwrapper.pyx:42-87).  Used by B200SolverWrapper.solve_stagewise_optim
 // and by the LP-level known-answer / differential tests.
-template <int RPL, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32)
+template <int RPL>
+__global__ void __launch_bounds__(32)
 lp2d_batch_kernel(const double *__restrict__ v, const double *__restrict__ a, const double *__restrict__ b,
                   const double *__restrict__ c, const double *__restrict__ low, const double *__restrict__ high,
                   const int *__restrict__ active_in, const int B, const int n, int *__restrict__ result,
                   double *__restrict__ optval, double *__restrict__ optvar, int *__restrict__ active_out) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long p = (long)blockIdx.x * WARPS + warp;
+  const int lane = threadIdx.x & 31;
+  const long p = warp_path();
   if (p >= B) return;
   double ra[RPL], rb[RPL], rc[RPL];
 #pragma unroll
@@ -990,71 +989,61 @@ __global__ void lp1d_batch_kernel(const double *__restrict__ v, const double *__
   }
 }
 
-#ifndef TB_SCAN_WARPS
-#define TB_SCAN_WARPS 1
-#endif
-constexpr int SCAN_WARPS = TB_SCAN_WARPS;  // 1: a finished path frees its slot at once (measured best: 1 < 2 < 4)
-#ifndef TB_SCAN_WARPS_PER_SM
-#define TB_SCAN_WARPS_PER_SM 32  // register budget of the dense build: 65536 / (32 * 32) -> 64 registers/thread (measured: 32 > 28 > 24)
-#endif
+// Register budget of the record scan for nC <= 32: 65536 / (32 * 32) -> 64 registers/thread (measured: 32 > 28 > 24);
+// the 4096-path batch of BASELINE cfg 2 is then a single wave on 132 SMs
+constexpr int SCAN_WARPS_PER_SM = 32;
+// resident warps per SM for nC in (32, 64].  H100 80GB (400 W), cfg 3 scan (16384 x 500, nC = 50), two runs:
+// 16 -> 24.1 / 23.6 ms, 20 -> 23.1 / 22.9 ms, 24 (80 registers) -> 22.6 / 22.4 ms
+constexpr int SCAN_RPL2_WARPS_PER_SM = 24;
+constexpr int SCAN_FUSED_WARPS_PER_SM = 28;  // 72 registers: 28 resident one-warp CTAs per SM
 
-#ifndef TB_SCAN_RPL2_WARPS_PER_SM
-// resident warps per SM for nC in (32, 64]; TB_SCAN_RPL2_OCC=16|20|24 overrides.  H100 80GB (400 W), cfg 3 scan (16384 x 500,
-// nC = 50), two runs: 16 -> 24.1 / 23.6 ms, 20 -> 23.1 / 22.9 ms, 24 (80 registers) -> 22.6 / 22.4 ms
-#define TB_SCAN_RPL2_WARPS_PER_SM 24
-#endif
+using ScanKernel = decltype(&scan_kernel<1, SCAN_WARPS_PER_SM, false>);  // every build has this signature
 
-#ifndef TB_SCAN_FUSED_WARPS_PER_SM
-#define TB_SCAN_FUSED_WARPS_PER_SM 28  // 72 registers: 28 resident one-warp CTAs per SM
-#endif
+// The one-row-per-lane scan_kernel build of a launch.  The three launch kinds of the batched solver (full scan, backward
+// only, forward only) get their own build with the mode folded in; instrumented (counters) and ragged (glen) launches and
+// the TOPPRAsd modes run on the run-time-flag build.
+template <int MINB, bool FUSED>
+ScanKernel scan_build(const int flags, const bool counters_or_glen) {
+  const bool fast = (flags & TB_SCAN_FAST_LOWER) != 0;
+  const int mode = flags & (TB_SCAN_BACKWARD_ONLY | TB_SCAN_SD_FORWARD | TB_SCAN_SD_SLOW | TB_SCAN_FORWARD_ONLY);
+  if (!counters_or_glen) {
+    if (mode == 0) return fast ? scan_kernel<1, MINB, true, 0, FUSED> : scan_kernel<1, MINB, false, 0, FUSED>;
+    if (mode == TB_SCAN_BACKWARD_ONLY)
+      return fast ? scan_kernel<1, MINB, true, TB_SCAN_BACKWARD_ONLY, FUSED>
+                  : scan_kernel<1, MINB, false, TB_SCAN_BACKWARD_ONLY, FUSED>;
+    if (mode == TB_SCAN_FORWARD_ONLY)
+      return fast ? scan_kernel<1, MINB, true, TB_SCAN_FORWARD_ONLY, FUSED>
+                  : scan_kernel<1, MINB, false, TB_SCAN_FORWARD_ONLY, FUSED>;
+  }
+  return fast ? scan_kernel<1, MINB, true, -1, FUSED> : scan_kernel<1, MINB, false, -1, FUSED>;
+}
 
 template <int RPL>
 int launch_scan(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
                 const double *sd_start, const double *sd_end, const double *sd_end_hi, int flags, double *K,
                 double *sd, double *u, int *status, int *fail_stage, int *counters, const int *glen,
                 cudaStream_t stream) {
-  const size_t smem = (size_t)SCAN_WARPS * SCAN_NBUF * W * sizeof(double) + SCAN_WARPS * SCAN_NBUF * sizeof(uint64_t) +
-                      SCAN_WARPS * 4 * sizeof(void *);
-  // Two register budgets for the common nC <= 32 case: 64 registers (32 one-warp CTAs per SM: the 4096-path batch
-  // of BASELINE cfg 2 is a single wave on 132 SMs) or the compiler's free choice.  TB_SCAN_OCC=free|dense overrides.
-  static const char *occ_env = getenv("TB_SCAN_OCC");
-  const bool dense = occ_env ? (occ_env[0] == 'd') : true;
-  constexpr int MINB = (RPL == 1 ? TB_SCAN_WARPS_PER_SM / SCAN_WARPS : 1);
+  const size_t smem = (size_t)SCAN_NBUF * W * sizeof(double) + SCAN_NBUF * sizeof(uint64_t) + 4 * sizeof(void *);
   const bool fast = (flags & TB_SCAN_FAST_LOWER) != 0;
-  auto kern = (RPL == 1 && dense) ? (fast ? scan_kernel<RPL, SCAN_WARPS, MINB, true> : scan_kernel<RPL, SCAN_WARPS, MINB, false>)
-                                  : (fast ? scan_kernel<RPL, SCAN_WARPS, 1, true> : scan_kernel<RPL, SCAN_WARPS, 1, false>);
-  if (RPL == 1 && dense && !counters && !glen) {
-    // the three launch kinds of the batched solver get their own instantiation: full scan, backward only, forward only
-    const int mode = flags & (TB_SCAN_BACKWARD_ONLY | TB_SCAN_SD_FORWARD | TB_SCAN_SD_SLOW | TB_SCAN_FORWARD_ONLY);
-    if (mode == 0)
-      kern = fast ? scan_kernel<RPL, SCAN_WARPS, MINB, true, 0> : scan_kernel<RPL, SCAN_WARPS, MINB, false, 0>;
-    else if (mode == TB_SCAN_BACKWARD_ONLY)
-      kern = fast ? scan_kernel<RPL, SCAN_WARPS, MINB, true, TB_SCAN_BACKWARD_ONLY>
-                  : scan_kernel<RPL, SCAN_WARPS, MINB, false, TB_SCAN_BACKWARD_ONLY>;
-    else if (mode == TB_SCAN_FORWARD_ONLY)
-      kern = fast ? scan_kernel<RPL, SCAN_WARPS, MINB, true, TB_SCAN_FORWARD_ONLY>
-                  : scan_kernel<RPL, SCAN_WARPS, MINB, false, TB_SCAN_FORWARD_ONLY>;
+  ScanKernel kern;
+  if constexpr (RPL == 1) {
+    kern = scan_build<SCAN_WARPS_PER_SM, false>(flags, counters || glen);
+  } else {
+    kern = fast ? scan_kernel<RPL, 1, true> : scan_kernel<RPL, 1, false>;
   }
   if constexpr (RPL == 2) {
     // nC in (32, 64] (BASELINE cfg 3: 50 rows).  Left alone the compiler takes about 150 registers (13 resident warps
-    // per SM); capped builds trade a few spills for residency.
-    static const char *rpl2_env = getenv("TB_SCAN_RPL2_OCC");
-    const int occ2 = rpl2_env ? atoi(rpl2_env) : TB_SCAN_RPL2_WARPS_PER_SM;
-    if (!fast && !counters) {
-      if (occ2 == 16) kern = scan_kernel<RPL, SCAN_WARPS, 16, false>;
-      else if (occ2 == 20) kern = scan_kernel<RPL, SCAN_WARPS, 20, false>;
-      else if (occ2 == 24) kern = scan_kernel<RPL, SCAN_WARPS, 24, false>;
-    }
+    // per SM); the capped build trades a few spills for residency.
+    if (!fast && !counters) kern = scan_kernel<RPL, SCAN_RPL2_WARPS_PER_SM, false>;
   }
   if (flags & TB_SCAN_UBOUND)  // records with a u-bound pair: the generic build (exact mode only)
-    kern = scan_kernel<RPL, SCAN_WARPS, 1, false, -1, false, true>;
+    kern = scan_kernel<RPL, 1, false, -1, false, true>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) { set_error("tb_scan: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return (int)e; }
   }
-  const int blocks = (B + SCAN_WARPS - 1) / SCAN_WARPS;
-  kern<<<blocks, SCAN_WARPS * 32, smem, stream>>>(records, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi,
-                                                  flags, K, sd, u, status, fail_stage, counters, glen, VelAccSrc{});
+  kern<<<B, 32, smem, stream>>>(records, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u,
+                                status, fail_stage, counters, glen, VelAccSrc{});
   return check_launch("tb_scan");
 }
 
@@ -1064,24 +1053,10 @@ int launch_scan_velacc_occ(const VelAccSrc &src, int W, int R, const double *gri
                            const double *sd_start, const double *sd_end, const double *sd_end_hi, int flags, double *K,
                            double *sd, double *u, int *status, int *fail_stage, int *counters, const int *glen,
                            cudaStream_t stream) {
-  const size_t smem = (size_t)SCAN_WARPS * W * sizeof(double) + SCAN_WARPS * SCAN_NBUF * sizeof(uint64_t) +
-                      SCAN_WARPS * 4 * sizeof(void *);
-  const bool fast = (flags & TB_SCAN_FAST_LOWER) != 0;
-  const int mode = flags & (TB_SCAN_BACKWARD_ONLY | TB_SCAN_SD_FORWARD | TB_SCAN_SD_SLOW | TB_SCAN_FORWARD_ONLY);
-  auto kern = fast ? scan_kernel<1, SCAN_WARPS, MINB, true, -1, true> : scan_kernel<1, SCAN_WARPS, MINB, false, -1, true>;
-  if (counters || glen) {
-    // instrumented or ragged launch: the run-time-flag build
-  } else if (mode == 0)
-    kern = fast ? scan_kernel<1, SCAN_WARPS, MINB, true, 0, true> : scan_kernel<1, SCAN_WARPS, MINB, false, 0, true>;
-  else if (mode == TB_SCAN_BACKWARD_ONLY)
-    kern = fast ? scan_kernel<1, SCAN_WARPS, MINB, true, TB_SCAN_BACKWARD_ONLY, true>
-                : scan_kernel<1, SCAN_WARPS, MINB, false, TB_SCAN_BACKWARD_ONLY, true>;
-  else if (mode == TB_SCAN_FORWARD_ONLY)
-    kern = fast ? scan_kernel<1, SCAN_WARPS, MINB, true, TB_SCAN_FORWARD_ONLY, true>
-                : scan_kernel<1, SCAN_WARPS, MINB, false, TB_SCAN_FORWARD_ONLY, true>;
-  const int blocks = (B + SCAN_WARPS - 1) / SCAN_WARPS;
-  kern<<<blocks, SCAN_WARPS * 32, smem, stream>>>(nullptr, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi,
-                                                  flags, K, sd, u, status, fail_stage, counters, glen, src);
+  const size_t smem = (size_t)W * sizeof(double) + SCAN_NBUF * sizeof(uint64_t) + 4 * sizeof(void *);
+  const ScanKernel kern = scan_build<MINB, true>(flags, counters || glen);
+  kern<<<B, 32, smem, stream>>>(nullptr, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u,
+                                status, fail_stage, counters, glen, src);
   return check_launch("tb_scan_velacc");
 }
 
@@ -1091,37 +1066,30 @@ int launch_scan_velacc(const VelAccSrc &src, int W, int R, const double *grid, i
                        cudaStream_t stream) {
   // Register budget by batch size: while 28 resident one-warp CTAs per SM cover the whole batch in one wave, the
   // 72-register build is used; larger batches are issue-bound and want the 32 resident warps per SM of the 64-register
-  // build.  TB_SCAN_FUSED_OCC=28|32 overrides.
-  static const char *occ_env = getenv("TB_SCAN_FUSED_OCC");
-  const int occ = occ_env ? atoi(occ_env)
-                          : ((long)B <= (long)num_sms() * TB_SCAN_FUSED_WARPS_PER_SM ? TB_SCAN_FUSED_WARPS_PER_SM : 32);
+  // build.
+  const auto launch = ((long)B <= (long)num_sms() * SCAN_FUSED_WARPS_PER_SM)
+                          ? launch_scan_velacc_occ<SCAN_FUSED_WARPS_PER_SM>
+                          : launch_scan_velacc_occ<SCAN_WARPS_PER_SM>;
   const int mode = flags & (TB_SCAN_BACKWARD_ONLY | TB_SCAN_SD_FORWARD | TB_SCAN_SD_SLOW | TB_SCAN_FORWARD_ONLY);
   if ((mode == 0 || mode == TB_SCAN_FORWARD_ONLY) && !counters && !glen && forward_threads_supported(src.dof, B)) {
     // large batches (issue-bound): the forward pass runs with one thread per path (tb_scan_fwd.cu) after a backward-only
     // launch of this kernel
     if (mode == 0) {
       const int bflags = (flags & TB_SCAN_FAST_LOWER) | TB_SCAN_BACKWARD_ONLY;
-      const int rc = (occ == 28)
-          ? launch_scan_velacc_occ<28>(src, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, bflags, K, nullptr,
-                                       nullptr, status, fail_stage, nullptr, nullptr, stream)
-          : launch_scan_velacc_occ<32>(src, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, bflags, K, nullptr,
-                                       nullptr, status, fail_stage, nullptr, nullptr, stream);
+      const int rc = launch(src, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, bflags, K, nullptr, nullptr,
+                            status, fail_stage, nullptr, nullptr, stream);
       if (rc) return rc;
     }
     return launch_forward_threads(src, R == 4 * src.dof, grid, grid_shared, B, G, sd_start, K, sd, u, status, fail_stage, stream);
   }
-  if (occ == 28)
-    return launch_scan_velacc_occ<28>(src, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u,
-                                      status, fail_stage, counters, glen, stream);
-  return launch_scan_velacc_occ<32>(src, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u,
-                                    status, fail_stage, counters, glen, stream);
+  return launch(src, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u, status, fail_stage,
+                counters, glen, stream);
 }
 
 template <int RPL>
 int launch_feasible(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
                     int ub, double *X, cudaStream_t stream) {
-  const int blocks = (B + SCAN_WARPS - 1) / SCAN_WARPS;
-  feasible_kernel<RPL, SCAN_WARPS><<<blocks, SCAN_WARPS * 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, ub, X);
+  feasible_kernel<RPL><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, ub, X);
   return check_launch("tb_feasible_sets");
 }
 
@@ -1129,13 +1097,10 @@ template <int RPL>
 int launch_reachable(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
                      const double *sdmin, const double *sdmax, int flags, double *X, double *L, int *fail_stage,
                      cudaStream_t stream) {
-  const int blocks = (B + SCAN_WARPS - 1) / SCAN_WARPS;
   if (flags & TB_SCAN_UBOUND)
-    reachable_kernel<RPL, SCAN_WARPS, true><<<blocks, SCAN_WARPS * 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G,
-                                                                                   sdmin, sdmax, X, L, fail_stage);
+    reachable_kernel<RPL, true><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, X, L, fail_stage);
   else
-    reachable_kernel<RPL, SCAN_WARPS, false><<<blocks, SCAN_WARPS * 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G,
-                                                                                    sdmin, sdmax, X, L, fail_stage);
+    reachable_kernel<RPL, false><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, X, L, fail_stage);
   return check_launch("tb_reachable_sets");
 }
 
@@ -1200,11 +1165,6 @@ extern "C" int tb_scan_velacc_ragged(const double *ppoly, const double *breaks, 
     return TB_ERR_UNSUPPORTED;
   }
   const VelAccSrc src{ppoly, breaks, alim, xbound, breaks_shared, nseg, dof, lim_shared};
-  // the two-paths-per-warp build (tb_scan_pair.cu) takes every dense launch it supports; ragged, instrumented and TOPPRAsd
-  // launches stay on the one-warp-per-path kernel
-  if (!glen && !counters && scan_velacc_pair_supported(dof, interp, nseg, flags))
-    return launch_scan_velacc_pair(src, interp, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u,
-                                   status, fail_stage, (cudaStream_t)stream);
   return launch_scan_velacc(src, Wc, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u, status,
                             fail_stage, counters, glen, (cudaStream_t)stream);
 }
@@ -1273,9 +1233,8 @@ extern "C" int tb_lp2d_batch(const double *v, const double *a, const double *b, 
   }
   if (n > MAX_ROWS + 2) { set_error("tb_lp2d_batch: n=%d > %d rows", n, MAX_ROWS + 2); return TB_ERR_UNSUPPORTED; }
   cudaStream_t s = (cudaStream_t)stream;
-  const int blocks = (B + SCAN_WARPS - 1) / SCAN_WARPS;
 #define TB_LAUNCH_LP2D(RPL) \
-  lp2d_batch_kernel<RPL, SCAN_WARPS><<<blocks, SCAN_WARPS * 32, 0, s>>>(v, a, b, c, low, high, active_in, B, n, result, optval, optvar, active_out)
+  lp2d_batch_kernel<RPL><<<B, 32, 0, s>>>(v, a, b, c, low, high, active_in, B, n, result, optval, optvar, active_out)
   if (n <= 32) TB_LAUNCH_LP2D(1);
   else if (n <= 64) TB_LAUNCH_LP2D(2);
   else if (n <= 96) TB_LAUNCH_LP2D(3);
@@ -1292,8 +1251,6 @@ extern "C" int tb_lp1d_batch(const double *v, const double *a, const double *b, 
     set_error("tb_lp1d_batch: bad argument");
     return TB_ERR_ARG;
   }
-  const int blocks = (B + SCAN_WARPS - 1) / SCAN_WARPS;
-  lp1d_batch_kernel<<<blocks, SCAN_WARPS * 32, 0, (cudaStream_t)stream>>>(v, a, b, low, high, B, n, result, optval, optvar,
-                                                                         active_out);
+  lp1d_batch_kernel<<<B, 32, 0, (cudaStream_t)stream>>>(v, a, b, low, high, B, n, result, optval, optvar, active_out);
   return check_launch("tb_lp1d_batch");
 }

@@ -1,5 +1,5 @@
-// tb_scan_common.cuh — helpers shared by the scan kernels (tb_scan.cu: one warp per path; tb_scan_pair.cu: two paths per
-// warp): Seidel's row order (cy_seidel_solverwrapper.pyx:252-264), the shortcut thresholds, Python's min/max.
+// tb_scan_common.cuh — helpers shared by the scan kernels (tb_scan.cu: one warp per path; tb_scan_fwd.cu: one thread per
+// path): Seidel's row order (cy_seidel_solverwrapper.pyx:252-264), the shortcut thresholds, Python's min/max.
 #pragma once
 #include <limits.h>
 
@@ -51,20 +51,10 @@ struct VelAccSrc {
   int breaks_shared, nseg, dof, lim_shared;
 };
 
-
-// launcher of the two-paths-per-warp build (tb_scan_pair.cu); returns TB_ERR_UNSUPPORTED when the problem does not fit
-int launch_scan_velacc_pair(const VelAccSrc &src, int interp, const double *grid, int grid_shared, int B, int G,
-                            const double *sd_start, const double *sd_end, const double *sd_end_hi, int flags, double *K,
-                            double *sd, double *u, int *status, int *fail_stage, cudaStream_t stream);
-bool scan_velacc_pair_supported(int dof, int interp, int nseg, int flags);
-
 // forward pass with one thread per path (tb_scan_fwd.cu), for large batches: reads K / status / fail_stage of a
-// TB_SCAN_BACKWARD_ONLY launch
-#ifndef TB_SCAN_FWD_THREADS_MIN_DEFAULT
-// smallest batch (paths) that takes the thread-per-path forward pass.  H100 80GB (400 W), 7-DOF, 200 gridpoints, fused
-// scan: 16384 paths 5.17 vs 5.36 ms (warp form), 24576: 7.33 vs 7.95 ms, 32768: 9.40 vs 10.96 ms
-#define TB_SCAN_FWD_THREADS_MIN_DEFAULT 16384
-#endif
+// TB_SCAN_BACKWARD_ONLY launch.  FWD_THREADS_MIN: smallest batch (paths) that takes it.  H100 80GB (400 W), 7-DOF,
+// 200 gridpoints, fused scan: 16384 paths 5.17 vs 5.36 ms (warp form), 24576: 7.33 vs 7.95 ms, 32768: 9.40 vs 10.96 ms
+constexpr int FWD_THREADS_MIN = 16384;
 bool forward_threads_supported(int dof, int B);
 int launch_forward_threads(const VelAccSrc &src, int interp, const double *grid, int grid_shared, int B, int G,
                            const double *sd_start, const double *K, double *sd, double *u, int *status, int *fail_stage,

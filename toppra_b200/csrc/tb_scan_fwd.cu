@@ -15,8 +15,6 @@
 // Exactness: the rows are K1's arithmetic (scipy evaluate_poly1 on the derivative coefficients, interpolation lift); the
 // values at s_{i+1} of stage i are carried into stage i+1 (the warp kernel recomputes the same numbers); the negated copies
 // use exact IEEE negation: (-b) x + c = -(b x) + c and -bxc / (-a) = bxc / a; min / max over the rows is order-independent.
-#include <stdlib.h>
-
 #include "tb_scan_common.cuh"
 
 namespace tb {
@@ -166,11 +164,7 @@ forward_threads_kernel(const VelAccSrc src, const int interp, const double *__re
 
 }  // namespace
 
-bool forward_threads_supported(int dof, int B) {
-  static const char *env = getenv("TB_SCAN_FWD_THREADS_MIN");   // batch size from which the thread-per-path form is used
-  const long min_b = env ? atol(env) : TB_SCAN_FWD_THREADS_MIN_DEFAULT;
-  return dof >= 1 && dof <= 8 && min_b > 0 && (long)B >= min_b;
-}
+bool forward_threads_supported(int dof, int B) { return dof >= 1 && dof <= 8 && B >= FWD_THREADS_MIN; }
 
 int launch_forward_threads(const VelAccSrc &src, int interp, const double *grid, int grid_shared, int B, int G,
                            const double *sd_start, const double *K, double *sd, double *u, int *status, int *fail_stage,
