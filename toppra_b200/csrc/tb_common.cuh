@@ -4,6 +4,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../../include/toppra_b200.h"
 
 namespace tb {
@@ -23,7 +25,45 @@ constexpr double CVXPY_MAXX = 10000.0;
 
 constexpr int MAX_ROWS = 126;   // R <= 126 -> nC = R + 2 <= 128 = 4 rows per lane
 
+// Calls f(std::integral_constant<int, RPL>{}) with the LP rows per lane of a one-warp kernel for nC rows: RPL = 1..4,
+// lane `lane` holds rows lane + 32 * s, s < RPL.  nC <= MAX_ROWS + 2 (checked by the caller).
+template <class F>
+auto with_rows_per_lane(const int nC, F &&f) {
+  if (nC <= 32) return f(std::integral_constant<int, 1>{});
+  if (nC <= 64) return f(std::integral_constant<int, 2>{});
+  if (nC <= 96) return f(std::integral_constant<int, 3>{});
+  return f(std::integral_constant<int, 4>{});
+}
+
 constexpr unsigned FULL = 0xffffffffu;
+
+// Warp-wide min / max of doubles (no NaNs) with two 32-bit redux.sync each instead of five shuffle rounds.
+// Order-preserving map double -> (khi, klo): flip all bits of negative numbers, the sign bit of the others; then
+// reduce the high words, and the low words among the lanes that tie on the high word.
+__device__ __forceinline__ double warp_min(double v) {
+  const int hi = __double2hiint(v), lo = __double2loint(v);
+  const int m = hi >> 31;  // 0 or -1
+  const unsigned khi = (unsigned)(hi ^ (m | (int)0x80000000)), klo = (unsigned)(lo ^ m);
+  const unsigned mh = __reduce_min_sync(FULL, khi);
+  const unsigned ml = __reduce_min_sync(FULL, khi == mh ? klo : 0xffffffffu);
+  const int m2 = ((int)~mh) >> 31;  // -1 if the winner is negative
+  return __hiloint2double((int)(mh ^ (unsigned)(m2 | (int)0x80000000)), (int)(ml ^ (unsigned)m2));
+}
+__device__ __forceinline__ double warp_max(double v) {
+  const int hi = __double2hiint(v), lo = __double2loint(v);
+  const int m = hi >> 31;
+  const unsigned khi = (unsigned)(hi ^ (m | (int)0x80000000)), klo = (unsigned)(lo ^ m);
+  const unsigned mh = __reduce_max_sync(FULL, khi);
+  const unsigned ml = __reduce_max_sync(FULL, khi == mh ? klo : 0u);
+  const int m2 = ((int)~mh) >> 31;
+  return __hiloint2double((int)(mh ^ (unsigned)(m2 | (int)0x80000000)), (int)(ml ^ (unsigned)m2));
+}
+
+// Path (or LP) of a one-warp CTA of feasible_kernel, reachable_kernel, lp2d_batch_kernel and scan_robust_kernel:
+// blockIdx.x.  The term threadIdx.x >> 5 is 0, but it keeps the index per-thread for the compiler: as a uniform value,
+// ptxas moves the per-path addressing to the uniform datapath, and the machine code of these kernels changes
+// (reachable_kernel<4> then spills 20-32 bytes).
+__device__ __forceinline__ long warp_path() { return (long)blockIdx.x + (int)(threadIdx.x >> 5); }
 
 __device__ __forceinline__ int find_interval(const double *__restrict__ x, const int nseg, const double s) {
   // scipy _ppoly.pyx find_interval: x[j] <= s < x[j+1]; s == x[-1] -> last interval; out of range -> end intervals

@@ -29,17 +29,6 @@ namespace {
 constexpr double ECOS_INFTY = 1000.0;   // toppra/constants.py:47
 constexpr double ECOS_MAXX = 10000.0;   // toppra/constants.py:46
 
-__device__ __forceinline__ double rwarp_min(double v) {
-  const int hi = __double2hiint(v), lo = __double2loint(v);
-  const int m = hi >> 31;
-  const unsigned khi = (unsigned)(hi ^ (m | (int)0x80000000)), klo = (unsigned)(lo ^ m);
-  const unsigned mh = __reduce_min_sync(FULL, khi);
-  const unsigned ml = __reduce_min_sync(FULL, khi == mh ? klo : 0xffffffffu);
-  const int m2 = ((int)~mh) >> 31;
-  return __hiloint2double((int)(mh ^ (unsigned)(m2 | (int)0x80000000)), (int)(ml ^ (unsigned)m2));
-}
-__device__ __forceinline__ double rwarp_max(double v) { return -rwarp_min(-v); }
-
 // Bounds on u implied by one row at a fixed x.  lo/hi are only tightened; bad = the row excludes every u.
 __device__ __forceinline__ void row_u_bounds(const bool conic, const double a, const double b, const double c,
                                              const double ru, const double rx, const double rc, const double x,
@@ -93,8 +82,8 @@ __device__ __forceinline__ double u_interval(const double x, const double (&a)[R
   bool bad = false;
 #pragma unroll
   for (int s = 0; s < RPL; ++s) row_u_bounds(cmask[s] != 0, a[s], b[s], c[s], ru, rx, rc, x, lo, hi, bad);
-  const double ulo = rwarp_max(lo);
-  uhi = rwarp_min(hi);
+  const double ulo = -warp_min(-lo);
+  uhi = warp_min(hi);
   if (__any_sync(FULL, bad)) return -__longlong_as_double(0x7ff0000000000000LL);
   return uhi - ulo;
 }
@@ -190,16 +179,17 @@ __device__ __forceinline__ void rload_rows(const double *__restrict__ rec, const
   }
 }
 
-template <int RPL, int WARPS>
-__global__ void __launch_bounds__(WARPS * 32, (RPL == 1) ? 28 / WARPS : 1)
+// One warp per CTA, like the record scan: a finished path frees its slot at once.
+template <int RPL>
+__global__ void __launch_bounds__(32, (RPL == 1) ? 28 : 1)
 scan_robust_kernel(const double *__restrict__ records, const int W, const int R, const int conic0, const int conicn,
                    const double ru, const double rx, const double rc, const double *__restrict__ grid,
                    const int grid_shared, const int B, const int G, const double *__restrict__ sd_start,
                    const double *__restrict__ sd_end, const int flags, double *__restrict__ Kout,
                    double *__restrict__ sdout, double *__restrict__ uout, int *__restrict__ status,
                    int *__restrict__ fail_stage, int *__restrict__ counters) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long path = (long)blockIdx.x * WARPS + warp;
+  const int lane = threadIdx.x & 31;
+  const long path = warp_path();
   if (path >= B) return;
   const int N = G - 1, nC = R + 2;
   const double *rec_path = records + (size_t)path * G * W;
@@ -336,19 +326,6 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
   }
 }
 
-constexpr int ROBUST_WARPS = 1;  // like K2: a finished path frees its slot at once
-
-template <int RPL>
-int launch_robust(const double *records, int W, int R, int conic0, int conicn, const double *ell, const double *grid,
-                  int grid_shared, int B, int G, const double *sd_start, const double *sd_end, int flags, double *K,
-                  double *sd, double *u, int *status, int *fail_stage, int *counters, cudaStream_t stream) {
-  const int blocks = (B + ROBUST_WARPS - 1) / ROBUST_WARPS;
-  scan_robust_kernel<RPL, ROBUST_WARPS><<<blocks, ROBUST_WARPS * 32, 0, stream>>>(
-      records, W, R, conic0, conicn, ell[0], ell[1], ell[2], grid, grid_shared, B, G, sd_start, sd_end, flags, K, sd, u,
-      status, fail_stage, counters);
-  return check_launch("tb_scan_robust");
-}
-
 }  // namespace
 }  // namespace tb
 
@@ -367,12 +344,11 @@ extern "C" int tb_scan_robust(const double *records, int W, int R, int conic_row
   if (W < 3 * R + 2) { set_error("tb_scan_robust: record stride W=%d < 3R+2", W); return TB_ERR_ALIGN; }
   if (conic_row0 < 0 || conic_rows < 0 || conic_row0 + conic_rows > R) { set_error("tb_scan_robust: bad conic row range"); return TB_ERR_ARG; }
   if (ellipsoid_host3[0] < 0 || ellipsoid_host3[1] < 0 || ellipsoid_host3[2] < 0) { set_error("tb_scan_robust: negative ellipsoid axis"); return TB_ERR_ARG; }
-  cudaStream_t s = (cudaStream_t)stream;
-  const int nC = R + 2;
-#define TB_ROBUST(RPL) launch_robust<RPL>(records, W, R, conic_row0, conic_rows, ellipsoid_host3, grid, grid_shared, B, G, sd_start, sd_end, flags, K, sd, u, status, fail_stage, counters, s)
-  if (nC <= 32) return TB_ROBUST(1);
-  if (nC <= 64) return TB_ROBUST(2);
-  if (nC <= 96) return TB_ROBUST(3);
-  return TB_ROBUST(4);
-#undef TB_ROBUST
+  const double ru = ellipsoid_host3[0], rx = ellipsoid_host3[1], rc = ellipsoid_host3[2];
+  with_rows_per_lane(R + 2, [&](auto rpl) {
+    scan_robust_kernel<rpl.value><<<B, 32, 0, (cudaStream_t)stream>>>(records, W, R, conic_row0, conic_rows, ru, rx, rc,
+                                                                      grid, grid_shared, B, G, sd_start, sd_end, flags,
+                                                                      K, sd, u, status, fail_stage, counters);
+  });
+  return check_launch("tb_scan_robust");
 }

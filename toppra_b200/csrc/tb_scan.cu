@@ -56,28 +56,6 @@ __device__ __forceinline__ void mbar_wait_s(const uint32_t addr, unsigned parity
   } while (!ok);
 }
 
-// Warp-wide min / max of doubles (no NaNs) with two 32-bit redux.sync each instead of five shuffle rounds.
-// Order-preserving map double -> (khi, klo): flip all bits of negative numbers, the sign bit of the others; then
-// reduce the high words, and the low words among the lanes that tie on the high word.
-__device__ __forceinline__ double warp_min(double v) {
-  const int hi = __double2hiint(v), lo = __double2loint(v);
-  const int m = hi >> 31;  // 0 or -1
-  const unsigned khi = (unsigned)(hi ^ (m | (int)0x80000000)), klo = (unsigned)(lo ^ m);
-  const unsigned mh = __reduce_min_sync(FULL, khi);
-  const unsigned ml = __reduce_min_sync(FULL, khi == mh ? klo : 0xffffffffu);
-  const int m2 = ((int)~mh) >> 31;  // -1 if the winner is negative
-  return __hiloint2double((int)(mh ^ (unsigned)(m2 | (int)0x80000000)), (int)(ml ^ (unsigned)m2));
-}
-__device__ __forceinline__ double warp_max(double v) {
-  const int hi = __double2hiint(v), lo = __double2loint(v);
-  const int m = hi >> 31;
-  const unsigned khi = (unsigned)(hi ^ (m | (int)0x80000000)), klo = (unsigned)(lo ^ m);
-  const unsigned mh = __reduce_max_sync(FULL, khi);
-  const unsigned ml = __reduce_max_sync(FULL, khi == mh ? klo : 0u);
-  const int m2 = ((int)~mh) >> 31;
-  return __hiloint2double((int)(mh ^ (unsigned)(m2 | (int)0x80000000)), (int)(ml ^ (unsigned)m2));
-}
-
 constexpr int SCAN_NBUF = 4;  // record buffers per warp (NBUF-1 stages of look-ahead)
 
 // One projected constraint of the 1-D sub-problem (pyx:326-347): its limit on t as an upper bound `thi` (denom >
@@ -752,33 +730,24 @@ scan_kernel(const double *__restrict__ records, const int W, const int R, const 
   }
 }
 
-// Path (or LP) of a one-warp CTA of feasible_kernel, reachable_kernel and lp2d_batch_kernel: blockIdx.x.  The term
-// threadIdx.x >> 5 is 0, but it keeps the index per-thread for the compiler: as a uniform value, ptxas moves the
-// per-path addressing to the uniform datapath, and the machine code of all three kernels changes (reachable_kernel<4>
-// then spills 20-32 bytes).
-__device__ __forceinline__ long warp_path() { return (long)blockIdx.x + (int)(threadIdx.x >> 5); }
-
 // compute_feasible_sets, reachability_algorithm.py:131-164: X[i] = [min x, max x] over stage i alone
-// (x in [-1e4, 1e4], x_next in [-1e4, 1e4]); warm-start slots chained over i like the reference.
+// (x in [-1e4, 1e4], x_next in [-1e4, 1e4]); warm-start slots up/dn chained over i like the reference.
+// ub: the records carry a u-bound pair (TB_SCAN_UBOUND).  The caller owns the row arrays, the warm-start slots and
+// n_resolve: declared here, the row arrays double the spills of reachable_kernel<4, *>.  The record address is formed
+// here from (records, path) rather than passed in as the path's base pointer: that way ptxas keeps
+// feasible_kernel<3> at 112 registers instead of 114.
 template <int RPL>
-__global__ void __launch_bounds__(32)
-feasible_kernel(const double *__restrict__ records, const int W, const int R, const double *__restrict__ grid,
-                const int grid_shared, const int B, const int G, const int ub, double *__restrict__ Xout) {
-  const int lane = threadIdx.x & 31;
-  const long path = warp_path();
-  if (path >= B) return;
-  const int N = G - 1, nC = R + 2;
-  const double *rec_path = records + (size_t)path * G * W;
-  const double *gp = grid + (grid_shared ? 0 : (size_t)path * G);
-  double *Xp = Xout + (size_t)path * G * 2;
-  double a[RPL], b[RPL], c[RPL];
-  int up0 = 0, up1 = 0, dn0 = 0, dn1 = 0, n_resolve = 0;
+__device__ __forceinline__ void feasible_pass(const double *records, const long path, const int G, const int W,
+                                              const int R, const int nC, const double *gp, const int N, const bool ub,
+                                              const int lane, double *Xp, double (&a)[RPL], double (&b)[RPL],
+                                              double (&c)[RPL],
+                                              int &up0, int &up1, int &dn0, int &dn1, int &n_resolve) {
   const double nan_d = __longlong_as_double(0x7ff8000000000000LL);
   for (int i = 0; i <= N; ++i) {
-    const double *rec = rec_path + (size_t)i * W;
+    const double *rec = records + (size_t)path * G * W + (size_t)i * W;
     load_rows<RPL>(rec, R, nC, lane, a, b, c);
     const double xlo = fmax(rec[3 * R], -CVXPY_MAXX), xhi = fmin(rec[3 * R + 1], CVXPY_MAXX);  // pyx:598-601
-    const double ulo = ub ? rec[3 * R + 2] : VAR_MIN, uhi = ub ? rec[3 * R + 3] : VAR_MAX;   // TB_SCAN_UBOUND records
+    const double ulo = ub ? rec[3 * R + 2] : VAR_MIN, uhi = ub ? rec[3 * R + 3] : VAR_MAX;
     if (i < N) {
       const double delta = gp[i + 1] - gp[i];
       set_xnext_rows<RPL>(lane, delta, -CVXPY_MAXX, CVXPY_MAXX, a, b, c);
@@ -794,6 +763,38 @@ feasible_kernel(const double *__restrict__ records, const int W, const int R, co
     if (x0 < 0) x0 = 0;  // reachability_algorithm.py:160-162
     if (lane == 0) { Xp[2 * i] = x0; Xp[2 * i + 1] = x1; }
   }
+}
+
+template <int RPL>
+__global__ void __launch_bounds__(32)
+feasible_kernel(const double *__restrict__ records, const int W, const int R, const double *__restrict__ grid,
+                const int grid_shared, const int B, const int G, const int ub, double *__restrict__ Xout) {
+  const int lane = threadIdx.x & 31;
+  const long path = warp_path();
+  if (path >= B) return;
+  const int N = G - 1, nC = R + 2;
+  const double *gp = grid + (grid_shared ? 0 : (size_t)path * G);
+  double *Xp = Xout + (size_t)path * G * 2;
+  double a[RPL], b[RPL], c[RPL];
+  int up0 = 0, up1 = 0, dn0 = 0, dn1 = 0, n_resolve = 0;
+  feasible_pass<RPL>(records, path, G, W, R, nC, gp, N, ub != 0, lane, Xp, a, b, c, up0, up1, dn0, dn1, n_resolve);
+}
+
+// End of cy_solve_lp1d with the active index (pyx:93-144): the lanes' bounds my_hi / my_lo, each with the first of the
+// lane's rows that set it (hi_idx / lo_idx, INT_MAX = none: strict improvement only), reduced over the warp.  Sequential
+// semantics: the first row (lowest index) that reaches the final value wins; -1 = low, -2 = high if no row improved
+// the bound.  Returns false if infeasible (cur_min > cur_max); else the optimum of max v0 * t and its active index.
+__device__ __forceinline__ bool lp1d_active_reduce(const double v0, const double my_hi, const int hi_idx,
+                                                   const double my_lo, const int lo_idx, double &out, int &active) {
+  const double cur_max = warp_min(my_hi), cur_min = warp_max(my_lo);
+  int hk = (hi_idx != INT_MAX && my_hi == cur_max) ? hi_idx : INT_MAX;
+  int lk = (lo_idx != INT_MAX && my_lo == cur_min) ? lo_idx : INT_MAX;
+  hk = __reduce_min_sync(FULL, hk);
+  lk = __reduce_min_sync(FULL, lk);
+  if (cur_min > cur_max) return false;
+  if (fabs(v0) < LP_TINY || v0 < 0) { out = cur_min; active = (lk == INT_MAX) ? -1 : lk; }
+  else { out = cur_max; active = (hk == INT_MAX) ? -2 : hk; }
+  return true;
 }
 
 // cy_solve_lp1d (pyx:93-144) over the rows a*u + (b*x + c) <= 0 of one stage, WITH the active index the reference stores
@@ -819,15 +820,7 @@ __device__ __forceinline__ bool lp1d_fixed_x_active_warp(const double v0, const 
       if (t > my_lo) { my_lo = t; lo_idx = r; }
     }
   }
-  const double cur_max = warp_min(my_hi), cur_min = warp_max(my_lo);
-  int hk = (hi_idx != INT_MAX && my_hi == cur_max) ? hi_idx : INT_MAX;
-  int lk = (lo_idx != INT_MAX && my_lo == cur_min) ? lo_idx : INT_MAX;
-  hk = __reduce_min_sync(FULL, hk);
-  lk = __reduce_min_sync(FULL, lk);
-  if (cur_min > cur_max) return false;
-  if (fabs(v0) < LP_TINY || v0 < 0) { out_u = cur_min; active = (lk == INT_MAX) ? -1 : lk; }
-  else { out_u = cur_max; active = (hk == INT_MAX) ? -2 : hk; }
-  return true;
+  return lp1d_active_reduce(v0, my_hi, hi_idx, my_lo, lo_idx, out_u, active);
 }
 
 // compute_reachable_sets (reachability_algorithm.py:378-431), one warp per path, ONE launch: the feasible-set pass
@@ -854,21 +847,7 @@ reachable_kernel(const double *__restrict__ records, const int W, const int R, c
   double a[RPL], b[RPL], c[RPL];
   int up0 = 0, up1 = 0, dn0 = 0, dn1 = 0, n_resolve = 0;
   const double nan_d = __longlong_as_double(0x7ff8000000000000LL);
-  // ---- feasible sets (as feasible_kernel) ----
-  for (int i = 0; i <= N; ++i) {
-    const double *rec = rec_path + (size_t)i * W;
-    load_rows<RPL>(rec, R, nC, lane, a, b, c);
-    const double xlo = fmax(rec[3 * R], -CVXPY_MAXX), xhi = fmin(rec[3 * R + 1], CVXPY_MAXX);
-    const double ulo = UB ? rec[3 * R + 2] : VAR_MIN, uhi = UB ? rec[3 * R + 3] : VAR_MAX;
-    if (i < N) set_xnext_rows<RPL>(lane, gp[i + 1] - gp[i], -CVXPY_MAXX, CVXPY_MAXX, a, b, c);
-    double uu, xx;
-    const bool ok0 = lp2d_warp<RPL>(-1e-9, -1.0, a, b, c, nC, ulo, uhi, xlo, xhi, up0, up1, uu, xx, lane, n_resolve);
-    double x0 = ok0 ? xx : nan_d;
-    const bool ok1 = lp2d_warp<RPL>(1e-9, 1.0, a, b, c, nC, ulo, uhi, xlo, xhi, dn0, dn1, uu, xx, lane, n_resolve);
-    const double x1 = ok1 ? xx : nan_d;
-    if (x0 < 0) x0 = 0;
-    if (lane == 0) { Xp[2 * i] = x0; Xp[2 * i + 1] = x1; }
-  }
+  feasible_pass<RPL>(records, path, G, W, R, nC, gp, N, UB, lane, Xp, a, b, c, up0, up1, dn0, dn1, n_resolve);
   __syncwarp();
   // ---- reachable sets ----
   const double s0 = sdmin ? sdmin[path] : 0.0, s1 = sdmax ? sdmax[path] : s0;
@@ -959,7 +938,7 @@ __global__ void lp1d_batch_kernel(const double *__restrict__ v, const double *__
   const long p = (long)blockIdx.x * (blockDim.x >> 5) + warp;
   if (p >= B) return;
   double my_hi = high[p], my_lo = low[p];
-  int hi_idx = INT_MAX, lo_idx = INT_MAX;  // first row index attaining the bound (strict improvement only)
+  int hi_idx = INT_MAX, lo_idx = INT_MAX;
   for (int r = lane; r < n; r += 32) {
     const double ar = a[p * n + r], br = b[p * n + r];
     if (ar > LP_TINY) {
@@ -970,22 +949,16 @@ __global__ void lp1d_batch_kernel(const double *__restrict__ v, const double *__
       if (cx > my_lo) { my_lo = cx; lo_idx = r; }
     }
   }
-  const double cur_max = warp_min(my_hi), cur_min = warp_max(my_lo);
-  // sequential semantics: the first row (lowest index) that reaches the final value wins; -2/-1 if none improved
-  int hk = (hi_idx != INT_MAX && my_hi == cur_max) ? hi_idx : INT_MAX;
-  int lk = (lo_idx != INT_MAX && my_lo == cur_min) ? lo_idx : INT_MAX;
-  hk = __reduce_min_sync(FULL, hk);
-  lk = __reduce_min_sync(FULL, lk);
+  const double v0 = v[p * 2];
+  double x = 0.0;
+  int active = 0;
+  const bool ok = lp1d_active_reduce(v0, my_hi, hi_idx, my_lo, lo_idx, x, active);
   if (lane == 0) {
     const double nan_d = __longlong_as_double(0x7ff8000000000000LL);
-    const double v0 = v[p * 2], v1 = v[p * 2 + 1];
-    if (cur_min > cur_max) {
-      result[p] = 0; optval[p] = nan_d; optvar[p] = nan_d; active_out[p] = 0;
-    } else if (fabs(v0) < LP_TINY || v0 < 0) {
-      result[p] = 1; optvar[p] = cur_min; optval[p] = v0 * cur_min + v1; active_out[p] = (lk == INT_MAX) ? -1 : lk;
-    } else {
-      result[p] = 1; optvar[p] = cur_max; optval[p] = v0 * cur_max + v1; active_out[p] = (hk == INT_MAX) ? -2 : hk;
-    }
+    result[p] = ok ? 1 : 0;
+    optvar[p] = ok ? x : nan_d;
+    optval[p] = ok ? (v0 * x + v[p * 2 + 1]) : nan_d;
+    active_out[p] = ok ? active : 0;
   }
 }
 
@@ -1127,12 +1100,10 @@ extern "C" int tb_scan_ragged(const double *records, int W, int R, const double 
   if (glen && grid_shared) { set_error("tb_scan: ragged batches (glen) need per-path grids [B][G]"); return TB_ERR_ARG; }
   const bool backward_only = (flags & TB_SCAN_BACKWARD_ONLY) != 0;
   if (!K || !status || (!backward_only && (!sd || (G > 1 && !u)))) { set_error("tb_scan: null output"); return TB_ERR_ARG; }
-  cudaStream_t s = (cudaStream_t)stream;
-  const int nC = R + 2;
-  if (nC <= 32) return launch_scan<1>(records, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u, status, fail_stage, counters, glen, s);
-  if (nC <= 64) return launch_scan<2>(records, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u, status, fail_stage, counters, glen, s);
-  if (nC <= 96) return launch_scan<3>(records, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u, status, fail_stage, counters, glen, s);
-  return launch_scan<4>(records, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u, status, fail_stage, counters, glen, s);
+  return with_rows_per_lane(R + 2, [&](auto rpl) {
+    return launch_scan<rpl.value>(records, W, R, grid, grid_shared, B, G, sd_start, sd_end, sd_end_hi, flags, K, sd, u,
+                                  status, fail_stage, counters, glen, (cudaStream_t)stream);
+  });
 }
 
 extern "C" int tb_scan_ex(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
@@ -1194,12 +1165,9 @@ extern "C" int tb_feasible_sets_ex(const double *records, int W, int R, const do
   if (!X) { set_error("tb_feasible_sets: null output"); return TB_ERR_ARG; }
   const int ub = (flags & TB_SCAN_UBOUND) ? 1 : 0;
   if (ub && W < 3 * R + 4) { set_error("tb_feasible_sets: TB_SCAN_UBOUND needs W >= 3R+4"); return TB_ERR_ARG; }
-  cudaStream_t s = (cudaStream_t)stream;
-  const int nC = R + 2;
-  if (nC <= 32) return launch_feasible<1>(records, W, R, grid, grid_shared, B, G, ub, X, s);
-  if (nC <= 64) return launch_feasible<2>(records, W, R, grid, grid_shared, B, G, ub, X, s);
-  if (nC <= 96) return launch_feasible<3>(records, W, R, grid, grid_shared, B, G, ub, X, s);
-  return launch_feasible<4>(records, W, R, grid, grid_shared, B, G, ub, X, s);
+  return with_rows_per_lane(R + 2, [&](auto rpl) {
+    return launch_feasible<rpl.value>(records, W, R, grid, grid_shared, B, G, ub, X, (cudaStream_t)stream);
+  });
 }
 
 extern "C" int tb_feasible_sets(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
@@ -1215,12 +1183,10 @@ extern "C" int tb_reachable_sets(const double *records, int W, int R, const doub
   if (rc) return rc;
   if (!X || !L) { set_error("tb_reachable_sets: null output"); return TB_ERR_ARG; }
   if ((flags & TB_SCAN_UBOUND) && W < 3 * R + 4) { set_error("tb_reachable_sets: TB_SCAN_UBOUND needs W >= 3R+4"); return TB_ERR_ARG; }
-  cudaStream_t s = (cudaStream_t)stream;
-  const int nC = R + 2;
-  if (nC <= 32) return launch_reachable<1>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, flags, X, L, fail_stage, s);
-  if (nC <= 64) return launch_reachable<2>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, flags, X, L, fail_stage, s);
-  if (nC <= 96) return launch_reachable<3>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, flags, X, L, fail_stage, s);
-  return launch_reachable<4>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, flags, X, L, fail_stage, s);
+  return with_rows_per_lane(R + 2, [&](auto rpl) {
+    return launch_reachable<rpl.value>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, flags, X, L, fail_stage,
+                                       (cudaStream_t)stream);
+  });
 }
 
 extern "C" int tb_lp2d_batch(const double *v, const double *a, const double *b, const double *c, const double *low,
@@ -1232,14 +1198,10 @@ extern "C" int tb_lp2d_batch(const double *v, const double *a, const double *b, 
     return TB_ERR_ARG;
   }
   if (n > MAX_ROWS + 2) { set_error("tb_lp2d_batch: n=%d > %d rows", n, MAX_ROWS + 2); return TB_ERR_UNSUPPORTED; }
-  cudaStream_t s = (cudaStream_t)stream;
-#define TB_LAUNCH_LP2D(RPL) \
-  lp2d_batch_kernel<RPL><<<B, 32, 0, s>>>(v, a, b, c, low, high, active_in, B, n, result, optval, optvar, active_out)
-  if (n <= 32) TB_LAUNCH_LP2D(1);
-  else if (n <= 64) TB_LAUNCH_LP2D(2);
-  else if (n <= 96) TB_LAUNCH_LP2D(3);
-  else TB_LAUNCH_LP2D(4);
-#undef TB_LAUNCH_LP2D
+  with_rows_per_lane(n, [&](auto rpl) {
+    lp2d_batch_kernel<rpl.value><<<B, 32, 0, (cudaStream_t)stream>>>(v, a, b, c, low, high, active_in, B, n, result,
+                                                                     optval, optvar, active_out);
+  });
   return check_launch("tb_lp2d_batch");
 }
 

@@ -242,7 +242,37 @@ def scan(records, R, grid, sd_start=None, sd_end=None, sd_end_hi=None, backward_
     check_grid(grid, B, G)
     for t, what in ((sd_start, "sd_start"), (sd_end, "sd_end"), (sd_end_hi, "sd_end_hi")):
         check_path_vector(t, B, what)
-    if forward_from is not None:  # forward pass alone on the K / status of an earlier backward-only launch
+    out, u_arg = _scan_outputs(B, G, dev, backward_only, counters, forward_from)
+    check_glen(glen, B, grid)
+    ub = has_ubound(records, R)
+    flags = _scan_flags(backward_only, sd_forward, forward_from, fast_lower and not ub, ub)
+    with torch.cuda.device(dev):
+        rc = _lib.load().tb_scan_ragged(_lib.ptr(records), W, int(R), _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G,
+                                        _lib.ptr(glen), _lib.ptr(sd_start), _lib.ptr(sd_end), _lib.ptr(sd_end_hi), flags,
+                                        _lib.ptr(out["K"]), _lib.ptr(out["sd"]), _lib.ptr(u_arg), _lib.ptr(out["status"]),
+                                        _lib.ptr(out["fail_stage"]), _lib.ptr(out.get("counters")), _lib.stream_ptr())
+    _lib.check(rc, "tb_scan")
+    return out
+
+
+SCAN_FLAGS = dict(backward_only=1, sd_fast=4, sd_slow=12, forward_only=16, fast_lower=32, ubound=64)
+
+
+def _scan_flags(backward_only, sd_forward, forward_from, fast_lower, ubound=False):
+    """TB_SCAN_* flags word of a scan launch; forward_from (an earlier backward-only result) means forward only."""
+    return ((SCAN_FLAGS["backward_only"] if backward_only else 0)
+            | {None: 0, "fast": SCAN_FLAGS["sd_fast"], "slow": SCAN_FLAGS["sd_slow"]}[sd_forward]
+            | (SCAN_FLAGS["forward_only"] if forward_from is not None else 0)
+            | (SCAN_FLAGS["fast_lower"] if fast_lower else 0)
+            | (SCAN_FLAGS["ubound"] if ubound else 0))
+
+
+def _scan_outputs(B, G, dev, backward_only, counters, forward_from=None):
+    """Output dict of a scan: K [B,G,2], sd [B,G], u [B,G-1], status / fail_stage [B] int32[, counters [B,4] zeroed].
+    forward_from: reuse K / status / fail_stage of an earlier backward-only launch.  sd and u are None when
+    backward_only.  Also returns the tensor to pass as u: a one-element stand-in when G = 1 leaves u empty."""
+    torch = torch_mod()
+    if forward_from is not None:
         K, status, fail_stage = forward_from["K"], forward_from["status"], forward_from["fail_stage"]
     else:
         K = torch.empty((B, G, 2), dtype=torch.float64, device=dev)
@@ -250,27 +280,11 @@ def scan(records, R, grid, sd_start=None, sd_end=None, sd_end_hi=None, backward_
         fail_stage = torch.empty((B,), dtype=torch.int32, device=dev)
     sd = None if backward_only else torch.empty((B, G), dtype=torch.float64, device=dev)
     u = None if backward_only else torch.empty((B, max(G - 1, 0)), dtype=torch.float64, device=dev)
-    cnt = torch.zeros((B, 4), dtype=torch.int32, device=dev) if counters else None
     u_arg = u if (u is None or u.numel() > 0) else torch.empty((1,), dtype=torch.float64, device=dev)
-    check_glen(glen, B, grid)
-    ub = has_ubound(records, R)
-    with torch.cuda.device(dev):
-        rc = _lib.load().tb_scan_ragged(_lib.ptr(records), W, int(R), _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G,
-                                    _lib.ptr(glen), _lib.ptr(sd_start), _lib.ptr(sd_end), _lib.ptr(sd_end_hi),
-                                    (1 if backward_only else 0) | ({None: 0, "fast": 4, "slow": 12}[sd_forward])
-                                    | (16 if forward_from is not None else 0) | (32 if (fast_lower and not ub) else 0)
-                                    | (64 if ub else 0),
-                                    _lib.ptr(K), _lib.ptr(sd),
-                                    _lib.ptr(u_arg),
-                                    _lib.ptr(status), _lib.ptr(fail_stage), _lib.ptr(cnt), _lib.stream_ptr())
-    _lib.check(rc, "tb_scan")
     out = dict(K=K, sd=sd, u=u, status=status, fail_stage=fail_stage)
     if counters:
-        out["counters"] = cnt
-    return out
-
-
-SCAN_FLAGS = dict(backward_only=1, sd_fast=4, sd_slow=12, forward_only=16, fast_lower=32, ubound=64)
+        out["counters"] = torch.zeros((B, 4), dtype=torch.int32, device=dev)
+    return out, u_arg
 
 
 def check_glen(glen, B, grid):
@@ -332,30 +346,17 @@ def scan_velacc(ppoly, breaks, grid, alim, interp, xbound, sd_start=None, sd_end
         raise ValueError("xbound must have shape (B, G, 2)")
     for t, what in ((sd_start, "sd_start"), (sd_end, "sd_end"), (sd_end_hi, "sd_end_hi")):
         check_path_vector(t, B, what)
-    if forward_from is not None:
-        K, status, fail_stage = forward_from["K"], forward_from["status"], forward_from["fail_stage"]
-    else:
-        K = torch.empty((B, G, 2), dtype=torch.float64, device=dev)
-        status = torch.empty((B,), dtype=torch.int32, device=dev)
-        fail_stage = torch.empty((B,), dtype=torch.int32, device=dev)
-    sd = None if backward_only else torch.empty((B, G), dtype=torch.float64, device=dev)
-    u = None if backward_only else torch.empty((B, max(G - 1, 0)), dtype=torch.float64, device=dev)
-    cnt = torch.zeros((B, 4), dtype=torch.int32, device=dev) if counters else None
-    u_arg = u if (u is None or u.numel() > 0) else torch.empty((1,), dtype=torch.float64, device=dev)
-    flags = ((1 if backward_only else 0) | ({None: 0, "fast": 4, "slow": 12}[sd_forward])
-             | (16 if forward_from is not None else 0) | (32 if fast_lower else 0))
+    out, u_arg = _scan_outputs(B, G, dev, backward_only, counters, forward_from)
+    flags = _scan_flags(backward_only, sd_forward, forward_from, fast_lower)
     check_glen(glen, B, grid)
     with torch.cuda.device(dev):
         rc = _lib.load().tb_scan_velacc_ragged(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, nseg, dof,
                                         _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G, _lib.ptr(glen), _lib.ptr(alim),
                                         1 if alim.dim() == 2 else 0, 1 if interp else 0, _lib.ptr(xbound),
-                                        _lib.ptr(sd_start), _lib.ptr(sd_end), _lib.ptr(sd_end_hi), flags, _lib.ptr(K),
-                                        _lib.ptr(sd), _lib.ptr(u_arg), _lib.ptr(status), _lib.ptr(fail_stage),
-                                        _lib.ptr(cnt), _lib.stream_ptr())
+                                        _lib.ptr(sd_start), _lib.ptr(sd_end), _lib.ptr(sd_end_hi), flags,
+                                        _lib.ptr(out["K"]), _lib.ptr(out["sd"]), _lib.ptr(u_arg), _lib.ptr(out["status"]),
+                                        _lib.ptr(out["fail_stage"]), _lib.ptr(out.get("counters")), _lib.stream_ptr())
     _lib.check(rc, "tb_scan_velacc")
-    out = dict(K=K, sd=sd, u=u, status=status, fail_stage=fail_stage)
-    if counters:
-        out["counters"] = cnt
     return out
 
 
@@ -366,12 +367,7 @@ def scan_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, sd_start=No
     B, G, W = records.shape
     dev = records.device
     backward_only = backward_only or feasible_sets
-    K = torch.empty((B, G, 2), dtype=torch.float64, device=dev)
-    sd = None if backward_only else torch.empty((B, G), dtype=torch.float64, device=dev)
-    u = None if backward_only else torch.empty((B, max(G - 1, 1)), dtype=torch.float64, device=dev)
-    status = torch.empty((B,), dtype=torch.int32, device=dev)
-    fail_stage = torch.empty((B,), dtype=torch.int32, device=dev)
-    cnt = torch.zeros((B, 4), dtype=torch.int32, device=dev) if counters else None
+    out, u_arg = _scan_outputs(B, G, dev, backward_only, counters)
     ell = np.ascontiguousarray(ellipsoid, dtype=np.float64)
     assert ell.shape == (3,)
     with torch.cuda.device(dev):
@@ -379,12 +375,9 @@ def scan_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, sd_start=No
                                         ctypes.c_void_p(ell.ctypes.data), _lib.ptr(grid), 1 if grid.dim() == 1 else 0,
                                         B, G, _lib.ptr(sd_start), _lib.ptr(sd_end),
                                         2 if feasible_sets else (1 if backward_only else 0),
-                                        _lib.ptr(K), _lib.ptr(sd), _lib.ptr(u), _lib.ptr(status), _lib.ptr(fail_stage),
-                                        _lib.ptr(cnt), _lib.stream_ptr())
+                                        _lib.ptr(out["K"]), _lib.ptr(out["sd"]), _lib.ptr(u_arg), _lib.ptr(out["status"]),
+                                        _lib.ptr(out["fail_stage"]), _lib.ptr(out.get("counters")), _lib.stream_ptr())
     _lib.check(rc, "tb_scan_robust")
-    out = dict(K=K, sd=sd, u=None if u is None else u[:, :max(G - 1, 0)], status=status, fail_stage=fail_stage)
-    if counters:
-        out["counters"] = cnt
     return out
 
 
@@ -395,7 +388,8 @@ def feasible_sets(records, R, grid):
     X = torch.empty((B, G, 2), dtype=torch.float64, device=records.device)
     with torch.cuda.device(records.device):
         rc = _lib.load().tb_feasible_sets_ex(_lib.ptr(records), W, int(R), _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B,
-                                             G, 64 if has_ubound(records, R) else 0, _lib.ptr(X), _lib.stream_ptr())
+                                             G, SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0, _lib.ptr(X),
+                                             _lib.stream_ptr())
     _lib.check(rc, "tb_feasible_sets")
     return X
 
@@ -414,8 +408,9 @@ def reachable_sets(records, R, grid, sdmin=None, sdmax=None):
     fs = torch.empty((B,), dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
         rc = _lib.load().tb_reachable_sets(_lib.ptr(records), W, int(R), _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G,
-                                           _lib.ptr(sdmin), _lib.ptr(sdmax), 64 if has_ubound(records, R) else 0,
-                                           _lib.ptr(X), _lib.ptr(L), _lib.ptr(fs), _lib.stream_ptr())
+                                           _lib.ptr(sdmin), _lib.ptr(sdmax),
+                                           SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0, _lib.ptr(X), _lib.ptr(L),
+                                           _lib.ptr(fs), _lib.stream_ptr())
     _lib.check(rc, "tb_reachable_sets")
     return dict(X=X, L=L, fail_stage=fs)
 
