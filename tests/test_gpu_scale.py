@@ -38,6 +38,10 @@ def test_cfg2_full_batch_vs_oracle(ta):
     assert np.array_equal(h["K"], o["K"]) and np.array_equal(h["sd"], o["sd"]) and np.array_equal(h["sdd"], o["u"])
     cnt = res.counters.cpu().numpy()
     assert (cnt[:, 0] == 2 * (G - 1)).all() and (cnt[:, 1] == G - 1).all()   # 398 2-D + 199 1-D LPs per path
+    # without counters the launch takes the specialised build that bench.py times, not the run-time-flag build
+    p = inst.compute_parameterization(0.0, 0.0).to_host()
+    assert np.array_equal(p["status"], o["status"])
+    assert np.array_equal(p["K"], o["K"]) and np.array_equal(p["sd"], o["sd"]) and np.array_equal(p["sdd"], o["u"])
 
 
 def test_velocity_active_batch_vs_oracle(ta):

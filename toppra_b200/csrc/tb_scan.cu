@@ -361,6 +361,21 @@ __device__ __forceinline__ bool lp1d_fixed_x_warp(const double v0, const double 
   return true;
 }
 
+// The rows lp1d_fixed_x_warp skips (|a| <= LP_TINY, as cy_solve_lp1d does) hold at (u, x).  The fast min-x shortcut
+// needs this: the 2-D LP it stands in for keeps those rows, and a flat row such as x >= 0.5 or x <= -1 moves or
+// removes the optimum at x = xlo although the 1-D LP there is feasible.
+template <int RPL>
+__device__ __forceinline__ bool flat_rows_hold(const double u, const double x, const double (&a)[RPL],
+                                               const double (&b)[RPL], const double (&c)[RPL]) {
+  bool bad = false;
+#pragma unroll
+  for (int s = 0; s < RPL; ++s) {
+    const bool flat = !(a[s] > LP_TINY) && !(a[s] < -LP_TINY);
+    bad |= flat && (a[s] * u + (b[s] * x + c[s]) > 0.0);
+  }
+  return !__any_sync(FULL, bad);
+}
+
 // Load this lane's rows of one stage record (shared memory) into registers.  LP row r: r = 0,1 are the
 // x_next rows (filled by the caller), r >= 2 is static row r-2; padding rows are (0,0,-1).
 template <int RPL>
@@ -591,7 +606,8 @@ scan_kernel(const double *__restrict__ records, const int W, const int R, const 
     bool ok_lo;
     double x_lower;
     double ufeas;
-    if (fast_lower && xlo <= xhi && lp1d_fixed_x_warp<RPL>(1.0, xlo, a, b, c, ulo, uhi, ufeas)) {
+    if (fast_lower && xlo <= xhi && lp1d_fixed_x_warp<RPL>(1.0, xlo, a, b, c, ulo, uhi, ufeas) &&
+        flat_rows_hold<RPL>(ufeas, xlo, a, b, c)) {
       // TB_SCAN_FAST_LOWER: some u is feasible at x = xlo, so min x IS xlo.  The reference reaches the same vertex
       // through ~4 projected re-solves and returns xlo plus rounding noise of its projection arithmetic
       // (|noise| <= ~1e-16, 5 % of the stages): this shortcut is exact for the LP, not bit-identical to that noise.
