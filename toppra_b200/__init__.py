@@ -7,8 +7,9 @@ CPU fallback (importing works anywhere, computing needs the GPU and the built li
 import logging
 
 from . import constants, exceptions
-from .interpolator import (AbstractGeometricPath, BatchSplineInterpolator, PolynomialPath, PPolyPath,
-                           SplineInterpolator, UnivariateSplineInterpolator, propose_gridpoints)
+from .interpolator import (AbstractGeometricPath, BatchPiecewisePolyPath, BatchSplineInterpolator, PiecewisePolyPath,
+                           PolynomialPath, PPolyPath, SplineInterpolator, UnivariateSplineInterpolator,
+                           propose_gridpoints)
 from .simplepath import SimplePath
 from .parametrizer import (BatchParametrizeConstAccel, BatchParametrizeSpline, ParametrizeConstAccel,
                            ParametrizeSpline)
@@ -22,6 +23,6 @@ __version__ = "0.1.0"
 
 logging.getLogger("toppra_b200").addHandler(logging.NullHandler())
 
-__all__ = ["AbstractGeometricPath", "BatchSplineInterpolator", "PPolyPath", "PolynomialPath", "SimplePath", "SplineInterpolator", "UnivariateSplineInterpolator", "propose_gridpoints",
+__all__ = ["AbstractGeometricPath", "BatchSplineInterpolator", "BatchPiecewisePolyPath", "PiecewisePolyPath", "PPolyPath", "PolynomialPath", "SimplePath", "SplineInterpolator", "UnivariateSplineInterpolator", "propose_gridpoints",
            "ParametrizeConstAccel", "ParametrizeSpline", "BatchParametrizeConstAccel", "BatchParametrizeSpline", "constraint", "solverwrapper", "algorithm", "BatchResult",
            "BatchTOPPRA", "BatchTOPPRAsd", "solve_batch", "constants", "exceptions", "setup_logging"]

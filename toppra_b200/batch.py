@@ -129,7 +129,7 @@ class BatchTOPPRA(object):
     ----------
     constraint_list: list of toppra_b200.constraint objects (limits shared by all paths, or batched
         (B, dof, 2) limits).
-    path: BatchSplineInterpolator
+    path: BatchSplineInterpolator (or BatchPiecewisePolyPath)
     gridpoints: (G,) shared by all paths, or (B, G); must start/end at the path interval.
     """
 
@@ -212,11 +212,12 @@ class BatchTOPPRA(object):
         kinds = [type(c) for c in constraint_list]
         self.fused = (fused is not False and sorted(k.__name__ for k in kinds) in
                       (["JointAccelerationConstraint"], ["JointAccelerationConstraint", "JointVelocityConstraint"])
+                      and engine.is_cubic(path.d_ppoly)
                       and engine.velacc_fused_supported(path.nseg, path.dof,
                                                         constraint_list[kinds.index(JointAccelerationConstraint)].interpolation))
         if fused and not self.fused:
-            raise ValueError("fused=True needs a [JointVelocityConstraint,] JointAccelerationConstraint problem that fits "
-                             "one LP row per lane (see tb_scan_velacc)")
+            raise ValueError("fused=True needs a [JointVelocityConstraint,] JointAccelerationConstraint problem on a "
+                             "piecewise-cubic path that fits one LP row per lane (see tb_scan_velacc)")
         self.xbound = None
 
     @property

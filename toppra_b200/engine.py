@@ -6,7 +6,7 @@ import ctypes
 
 import numpy as np
 
-from . import _lib
+from . import _lib, _lib_poly
 
 BC_KINDS = {"not-a-knot": 0, "clamped": 1, "natural": 2, "periodic": 3}
 
@@ -88,13 +88,32 @@ def spline_fit(ss, wp, bc=((0, None), (0, None))):
     return ppoly
 
 
+def is_cubic(ppoly):
+    """Paths with 4 coefficients per piece take libtoppra_b200's kernels; 1..8 otherwise take libtoppra_b200_poly's
+    (the order-k path: evaluate, build records from the samples, record scan)."""
+    return ppoly.shape[1] == 4
+
+
+def require_cubic(ppoly, what):
+    if not is_cubic(ppoly):
+        raise NotImplementedError("%s needs piecewise-cubic paths; this path has order %d (%d coefficients per piece)"
+                                  % (what, ppoly.shape[1], ppoly.shape[1]))
+
+
 def ppoly_eval(ppoly, breaks, s, order):
-    """ppoly [B,4,nseg,dof], breaks [nseg+1] or [B,nseg+1], s [G] or [B,G] -> [B,G,dof]."""
+    """ppoly [B,k,nseg,dof], breaks [nseg+1] or [B,nseg+1], s [G] or [B,G] -> [B,G,dof]."""
     torch = torch_mod()
-    lib = _lib.load()
-    B, _, nseg, dof = ppoly.shape
+    B, kc, nseg, dof = ppoly.shape
     G = s.shape[-1]
     out = torch.empty((B, G, dof), dtype=torch.float64, device=ppoly.device)
+    if not is_cubic(ppoly):
+        with torch.cuda.device(ppoly.device):
+            rc = _lib_poly.load().tbp_ppoly_eval(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, B, kc,
+                                                 nseg, dof, _lib.ptr(s), 1 if s.dim() == 1 else 0, G, int(order),
+                                                 _lib.ptr(out), _lib.stream_ptr())
+        _lib.check(rc, "tbp_ppoly_eval")
+        return out
+    lib = _lib.load()
     with torch.cuda.device(ppoly.device):
         rc = lib.tb_ppoly_eval(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, B, nseg, dof,
                                _lib.ptr(s), 1 if s.dim() == 1 else 0, G, int(order), _lib.ptr(out), _lib.stream_ptr())
@@ -153,7 +172,8 @@ def check_path_vector(t, B, what):
 
 
 def coeff_velacc(ppoly, breaks, grid, vlim, alim, interp, records, R_total, row0=0, write_xbound=1):
-    """K1.  vlim/alim: [dof,2] or [B,dof,2] device tensors (either may be None, not both)."""
+    """K1.  vlim/alim: [dof,2] or [B,dof,2] device tensors (either may be None, not both).  Order-k paths: q' and q''
+    at the gridpoints (tbp_ppoly_eval), then the records from those samples (rows_velacc_sampled)."""
     torch = torch_mod()
     B, _, nseg, dof = ppoly.shape
     G = grid.shape[-1]
@@ -164,6 +184,10 @@ def coeff_velacc(ppoly, breaks, grid, vlim, alim, interp, records, R_total, row0
             raise ValueError("limits must have shape (dof, 2) or (B, dof, 2) with B = %d, dof = %d; got %s"
                              % (B, dof, tuple(t.shape)))
     check_grid_shapes(B, breaks, nseg + 1, grid, G)
+    if not is_cubic(ppoly):
+        qd, qdd = ppoly_eval(ppoly, breaks, grid, 1), ppoly_eval(ppoly, breaks, grid, 2)
+        rows_velacc_sampled(qd, qdd, grid, vlim, alim, interp, records, R_total, row0, write_xbound)
+        return
     shared = all(t.dim() == 2 for t in lims)
     if not shared:
         vlim = None if vlim is None else (vlim if vlim.dim() == 3 else vlim.expand(B, dof, 2).contiguous())
@@ -176,6 +200,33 @@ def coeff_velacc(ppoly, breaks, grid, vlim, alim, interp, records, R_total, row0
     _lib.check(rc, "tb_coeff_velacc")
 
 
+def rows_velacc_sampled(qd, qdd, grid, vlim, alim, interp, records, R_total, row0=0, write_xbound=1):
+    """K1's records from sampled path derivatives qd = q'(grid), qdd = q''(grid), both [B, G, dof]
+    (tbp_rows_velacc_sampled).  Every other argument as coeff_velacc."""
+    torch = torch_mod()
+    B, G, dof = qd.shape
+    W = records.shape[-1]
+    check_shape(qdd, (B, G, dof), "qdd")
+    check_grid(grid, B, G)
+    if tuple(records.shape[:2]) != (B, G):
+        raise ValueError("records must have shape (%d, %d, W); got %s" % (B, G, tuple(records.shape)))
+    lims = [t for t in (vlim, alim) if t is not None]
+    for t in lims:
+        if t.dim() not in (2, 3) or tuple(t.shape[-2:]) != (dof, 2) or (t.dim() == 3 and t.shape[0] != B):
+            raise ValueError("limits must have shape (dof, 2) or (B, dof, 2) with B = %d, dof = %d; got %s"
+                             % (B, dof, tuple(t.shape)))
+    shared = all(t.dim() == 2 for t in lims)
+    if not shared:
+        vlim = None if vlim is None else (vlim if vlim.dim() == 3 else vlim.expand(B, dof, 2).contiguous())
+        alim = None if alim is None else (alim if alim.dim() == 3 else alim.expand(B, dof, 2).contiguous())
+    with torch.cuda.device(records.device):
+        rc = _lib_poly.load().tbp_rows_velacc_sampled(_lib.ptr(qd), _lib.ptr(qdd), B, dof, _lib.ptr(grid),
+                                                      1 if grid.dim() == 1 else 0, G, _lib.ptr(vlim), _lib.ptr(alim),
+                                                      1 if shared else 0, 1 if interp else 0, _lib.ptr(records), W,
+                                                      int(R_total), int(row0), int(write_xbound), _lib.stream_ptr())
+    _lib.check(rc, "tbp_rows_velacc_sampled")
+
+
 DEVICE_MODELS = {"coupled_cosine": 0, "pendulums": 1}  # TB_INVDYN_* of include/toppra_b200.h
 
 
@@ -184,6 +235,7 @@ def coeff_second_order(model, params, ppoly, breaks, grid, taulim, friction, int
     evaluated on the GPU from the spline, written straight into `records`.  taulim [dof,2] or [B,dof,2] (device),
     friction [dof] device tensor or None.  Returns the number of rows written."""
     torch = torch_mod()
+    require_cubic(ppoly, "SecondOrderConstraint with a device model (tb_coeff_second_order)")
     B, _, nseg, dof = ppoly.shape
     G = grid.shape[-1]
     W = records.shape[-1]
@@ -305,6 +357,7 @@ def velacc_fused_supported(nseg, dof, interp):
 def xbound_velocity(ppoly, breaks, grid, vlim, out=None):
     """Velocity bound alone: xbound [B, G, 2] clipped to the solver box (+-1e8 when vlim is None) = K1 with no rows."""
     torch = torch_mod()
+    require_cubic(ppoly, "xbound_velocity (the fused scan's velocity bound)")
     B = ppoly.shape[0]
     xb = torch.empty((B, grid.shape[-1], 2), dtype=torch.float64, device=ppoly.device) if out is None else out
     if vlim is None:
@@ -317,6 +370,7 @@ def xbound_velocity(ppoly, breaks, grid, vlim, out=None):
 def xbound_constant(ppoly, breaks, grid, vlim, records, R_total, write_xbound):
     """JointVelocityConstraint alone into the xbound slots of `records` (tb_xbound_velocity, thread per gridpoint)."""
     torch = torch_mod()
+    require_cubic(ppoly, "xbound_constant")
     B, _, nseg, dof = ppoly.shape
     G = grid.shape[-1]
     W = records.shape[-1]
@@ -336,6 +390,7 @@ def scan_velacc(ppoly, breaks, grid, alim, interp, xbound, sd_start=None, sd_end
     """K2 fused with K1 for JointVelocity + JointAcceleration (tb_scan_velacc): rows are built inside the scan from
     the spline; `xbound` [B, G, 2] from xbound_velocity().  Same outputs as scan()."""
     torch = torch_mod()
+    require_cubic(ppoly, "scan_velacc (the fused vel+acc scan)")
     B, _, nseg, dof = ppoly.shape
     G = grid.shape[-1]
     dev = ppoly.device
@@ -420,13 +475,22 @@ def propose_gridpoints(ppoly, breaks, max_err_threshold=1e-4, max_iteration=100,
     """propose_gridpoints for B paths (tb_propose_gridpoints).  Returns (grid [B, max_points] padded with the path end,
     glen [B] int32, status [B] int32: 0 ok, 1 = no good grid within max_iteration passes, < 0 = max_points exceeded)."""
     torch = torch_mod()
-    B, _, nseg, dof = ppoly.shape
+    B, kc, nseg, dof = ppoly.shape
     dev = ppoly.device
     check_grid_shapes(B, breaks, nseg + 1, breaks, nseg + 1)
     grid = torch.empty((B, int(max_points)), dtype=torch.float64, device=dev)
     scratch = torch.empty_like(grid)
     glen = torch.empty((B,), dtype=torch.int32, device=dev)
     status = torch.empty((B,), dtype=torch.int32, device=dev)
+    if not is_cubic(ppoly):
+        with torch.cuda.device(dev):
+            rc = _lib_poly.load().tbp_propose_gridpoints(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, B,
+                                                         kc, nseg, dof, float(max_err_threshold), int(max_iteration),
+                                                         float(max_seg_length), int(min_nb_points), int(max_points),
+                                                         _lib.ptr(grid), _lib.ptr(scratch), _lib.ptr(glen),
+                                                         _lib.ptr(status), _lib.stream_ptr())
+        _lib.check(rc, "tbp_propose_gridpoints")
+        return grid, glen, status
     with torch.cuda.device(dev):
         rc = _lib.load().tb_propose_gridpoints(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, B, nseg,
                                                dof, float(max_err_threshold), int(max_iteration), float(max_seg_length),
@@ -573,10 +637,19 @@ def time_grid(sd, grid):
 def constaccel_eval(ppoly, breaks, grid, sd, t_grid, us, ts, order):
     """K3: q / qd / qdd at times ts ([M] shared or [B,M]) -> [B,M,dof]."""
     torch = torch_mod()
-    B, _, nseg, dof = ppoly.shape
+    B, kc, nseg, dof = ppoly.shape
     G = sd.shape[1]
     M = ts.shape[-1]
     out = torch.empty((B, M, dof), dtype=torch.float64, device=sd.device)
+    if not is_cubic(ppoly):
+        with torch.cuda.device(sd.device):
+            rc = _lib_poly.load().tbp_constaccel_eval(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, kc,
+                                                      nseg, dof, _lib.ptr(grid), 1 if grid.dim() == 1 else 0,
+                                                      _lib.ptr(sd), _lib.ptr(t_grid), _lib.ptr(us), B, G, _lib.ptr(ts),
+                                                      1 if ts.dim() == 1 else 0, M, int(order), _lib.ptr(out),
+                                                      _lib.stream_ptr())
+        _lib.check(rc, "tbp_constaccel_eval")
+        return out
     with torch.cuda.device(sd.device):
         rc = _lib.load().tb_constaccel_eval(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, nseg, dof,
                                             _lib.ptr(grid), 1 if grid.dim() == 1 else 0, _lib.ptr(sd), _lib.ptr(t_grid),
@@ -595,9 +668,28 @@ def xbound_varying(ppoly, breaks, grid, vlim_grid, records, R_total, write_xboun
     check_grid_shapes(B, breaks, nseg + 1, grid, G)
     if tuple(vlim_grid.shape[-3:]) != (G, dof, 2) or vlim_grid.dim() not in (3, 4) or (vlim_grid.dim() == 4 and vlim_grid.shape[0] != B):
         raise ValueError("varying velocity limits must have shape (G, dof, 2) or (B, G, dof, 2); got %s" % (tuple(vlim_grid.shape),))
+    if not is_cubic(ppoly):
+        xbound_varying_sampled(ppoly_eval(ppoly, breaks, grid, 1), vlim_grid, records, R_total, write_xbound)
+        return
     with torch.cuda.device(records.device):
         rc = _lib.load().tb_xbound_varying(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, B, nseg, dof,
                                            _lib.ptr(grid), 1 if grid.dim() == 1 else 0, G, _lib.ptr(vlim_grid),
                                            1 if vlim_grid.dim() == 3 else 0, _lib.ptr(records), W, int(R_total),
                                            int(write_xbound), _lib.stream_ptr())
     _lib.check(rc, "tb_xbound_varying")
+
+
+def xbound_varying_sampled(qd, vlim_grid, records, R_total, write_xbound):
+    """xbound_varying from sampled qd = q'(grid) [B, G, dof] (tbp_xbound_varying_sampled)."""
+    torch = torch_mod()
+    B, G, dof = qd.shape
+    W = records.shape[-1]
+    if tuple(vlim_grid.shape[-3:]) != (G, dof, 2) or vlim_grid.dim() not in (3, 4) or (vlim_grid.dim() == 4 and vlim_grid.shape[0] != B):
+        raise ValueError("varying velocity limits must have shape (G, dof, 2) or (B, G, dof, 2); got %s" % (tuple(vlim_grid.shape),))
+    if tuple(records.shape[:2]) != (B, G):
+        raise ValueError("records must have shape (%d, %d, W); got %s" % (B, G, tuple(records.shape)))
+    with torch.cuda.device(records.device):
+        rc = _lib_poly.load().tbp_xbound_varying_sampled(_lib.ptr(qd), B, dof, G, _lib.ptr(vlim_grid),
+                                                         1 if vlim_grid.dim() == 3 else 0, _lib.ptr(records), W,
+                                                         int(R_total), int(write_xbound), _lib.stream_ptr())
+    _lib.check(rc, "tbp_xbound_varying_sampled")

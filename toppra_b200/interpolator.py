@@ -8,7 +8,7 @@ from typing import Union
 
 import numpy as np
 
-from . import engine
+from . import _lib_poly, engine
 from .utils import deprecated
 
 logger = logging.getLogger(__name__)
@@ -22,8 +22,9 @@ def propose_gridpoints(path, max_err_threshold=1e-4, max_iteration=100, max_seg_
     `min_nb_points` points.  Runs on the GPU (csrc/tb_frows.cu: tb_propose_gridpoints); this is the B = 1 case of
     `BatchSplineInterpolator.propose_gridpoints`.  Returns the list of gridpoints like the reference."""
     if not hasattr(path, "as_batch"):
-        raise TypeError("toppra_b200.propose_gridpoints needs a path with a piecewise-cubic device form "
-                        "(SplineInterpolator, PPolyPath, SimplePath, PolynomialPath); got %s" % type(path).__name__)
+        raise TypeError("toppra_b200.propose_gridpoints needs a path with a piecewise-polynomial device form "
+                        "(SplineInterpolator, PPolyPath, PiecewisePolyPath, SimplePath, PolynomialPath); got %s"
+                        % type(path).__name__)
     grid, glen = path.as_batch().propose_gridpoints(max_err_threshold, max_iteration, max_seg_length, min_nb_points,
                                                     max_points)
     return grid[0, :int(glen[0])].cpu().numpy().tolist()
@@ -155,6 +156,11 @@ class BatchSplineInterpolator(object):
         if c.shape[1] < 4:
             pad = torch.zeros((c.shape[0], 4 - c.shape[1]) + tuple(c.shape[2:]), dtype=c.dtype, device=c.device)
             c = torch.cat((pad, c), dim=1).contiguous()
+        self._set_pieces(breaks, c)
+        return self
+
+    def _set_pieces(self, breaks, c):
+        """Device form of pieces c [B, k, nseg, dof] (CUDA fp64) over `breaks`; checks the breaks."""
         self.B, _, nseg, self._dof = c.shape
         self.n = nseg + 1
         self.d_ss = engine.as_device(breaks, self.device)
@@ -167,7 +173,6 @@ class BatchSplineInterpolator(object):
         self.ss_host = engine.host_view(breaks)
         self.d_ppoly = c
         self.d_wp = engine.ppoly_eval(self.d_ppoly, self.d_ss, self.d_ss, 0)  # positions at the breaks
-        return self
 
     @property
     def dof(self):
@@ -220,6 +225,41 @@ class BatchSplineInterpolator(object):
         view.d_ss = self.d_ss if self.d_ss.dim() == 1 else self.d_ss[lo:hi]
         view.ss_host = None if self.ss_host is None else (self.ss_host if self.ss_host.ndim == 1 else self.ss_host[lo:hi])
         view.d_ppoly = self.d_ppoly[lo:hi]
+        return view
+
+
+class BatchPiecewisePolyPath(BatchSplineInterpolator):
+    """B paths given as piecewise polynomials with up to 8 coefficients per piece (degree <= 7) in scipy's PPoly layout.
+
+    breaks: (nseg + 1,) shared or (B, nseg + 1), strictly increasing.
+    coeffs: (B, k, nseg, dof), 1 <= k <= 8, highest power first, local power basis
+            sum_j c[j] (s - breaks[i]) ** (k - 1 - j) like `scipy.interpolate.PPoly.c`.
+    device: torch device (default: that of a CUDA `coeffs`, else the current CUDA device)
+
+    Derivatives are those of scipy's derivative objects, `PPoly(c, x).derivative()` and `.derivative().derivative()`,
+    bit for bit.  k <= 4 is zero-padded to the cubic form exactly like `BatchSplineInterpolator.from_ppoly` and runs on
+    the cubic kernels; 5 <= k <= 8 runs on libtoppra_b200_poly.so (evaluate q', q'' at the gridpoints, build the stage
+    records from them, then the record scan).  `BatchTOPPRA` / `BatchTOPPRAsd` accept both; the fused vel+acc scan is
+    cubic only.  `order` is k."""
+
+    def __init__(self, breaks, coeffs, device=None):
+        torch = engine.torch_mod()
+        self.device = engine.default_device(device if device is not None else
+                                            (coeffs.device if isinstance(coeffs, torch.Tensor) else None))
+        c = engine.as_device(coeffs, self.device)
+        if c.dim() != 4 or not 1 <= c.shape[1] <= _lib_poly.MAX_COEFFS:
+            raise ValueError("coeffs must have shape (B, k, nseg, dof) with 1 <= k <= %d; got %s"
+                             % (_lib_poly.MAX_COEFFS, tuple(c.shape)))
+        self.order = int(c.shape[1])
+        if self.order <= 4:
+            self.__dict__.update(BatchSplineInterpolator.from_ppoly(breaks, c, device=self.device).__dict__)
+            return
+        self._set_pieces(breaks, c)
+
+    def chunk(self, lo, hi):
+        view = object.__new__(BatchPiecewisePolyPath)
+        view.__dict__.update(BatchSplineInterpolator.chunk(self, lo, hi).__dict__)
+        view.order = self.order
         return view
 
 
@@ -321,7 +361,11 @@ class PPolyPath(AbstractGeometricPath):
             c = c[:, :, None]
         if c.ndim != 3:
             raise ValueError("PPoly coefficients must have shape (k, nseg) or (k, nseg, dof)")
-        self._batch = BatchSplineInterpolator.from_ppoly(self._x, c[None], device=device)
+        self._batch = self._device_form(self._x, c[None], device)
+
+    @staticmethod
+    def _device_form(x, c, device):
+        return BatchSplineInterpolator.from_ppoly(x, c, device=device)
 
     def __call__(self, path_positions, order=0):
         if order not in (0, 1, 2):
@@ -352,6 +396,34 @@ class PPolyPath(AbstractGeometricPath):
 
     def as_batch(self):
         return self._batch
+
+
+class PiecewisePolyPath(PPolyPath):
+    """A single path given as a piecewise polynomial with up to 8 coefficients per piece (degree <= 7) in scipy's PPoly
+    layout — the reference's C++ `PiecewisePolyPath` in Python form.  Same surface as `PPolyPath`; `ppoly` is an object
+    with `.c` (k, nseg[, dof]) and `.x` (nseg + 1,), or the pair (c, x).  Values and derivatives equal scipy's
+    `PPoly(c, x)`, `.derivative()` and `.derivative().derivative()` bit for bit, so `TOPPRA(constraints, path)` gives
+    the reference's result for a path object with that convention.
+
+    Quintic paths from scipy::
+
+        from scipy.interpolate import BPoly, PPoly, make_interp_spline
+        path = PiecewisePolyPath(PPoly.from_spline(make_interp_spline(ss, qs, k=5)))
+        # quintic Hermite through positions, velocities and accelerations; yi[i] = [q_i, qd_i, qdd_i] per joint
+        path = PiecewisePolyPath(PPoly.from_bernstein_basis(BPoly.from_derivatives(ss, yi)))
+
+    `PPoly.from_spline` keeps the B-spline's full knot vector, whose outer pieces have zero length; pass
+    `(pp.c[:, k:-k], pp.x[k:-k])` (k = 5 here) to keep the pieces inside the interval, where the breaks increase
+    strictly."""
+
+    @staticmethod
+    def _device_form(x, c, device):
+        return BatchPiecewisePolyPath(x, c, device=device)
+
+    @property
+    def order(self):
+        """Coefficients per piece (degree + 1)."""
+        return self._batch.order
 
 
 class PolynomialPath(PPolyPath):

@@ -67,8 +67,8 @@ class B200SolverWrapper(SolverWrapper):
         from ..batch import build_records, conic_info
         super(B200SolverWrapper, self).__init__(constraint_list, path, path_discretization)
         if not hasattr(path, "as_batch"):
-            raise TypeError("toppra_b200 needs a path with a piecewise-cubic device form (SplineInterpolator, PPolyPath, "
-                            "SimplePath, PolynomialPath up to degree 3); got %s" % type(path).__name__)
+            raise TypeError("toppra_b200 needs a path with a piecewise-polynomial device form (SplineInterpolator, PPolyPath, "
+                            "PiecewisePolyPath, SimplePath, PolynomialPath up to degree 3); got %s" % type(path).__name__)
         bpath = path.as_batch()
         grid = np.ascontiguousarray(self.path_discretization, dtype=np.float64)
         self.ctx = RecordContext(bpath, engine.as_device(grid, bpath.device), grid, path)
