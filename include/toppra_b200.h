@@ -230,6 +230,27 @@ int tb_scan_velacc_ragged(const double *ppoly, const double *breaks, int breaks_
                           int lim_shared, int interp, const double *xbound, const double *sd_start, const double *sd_end,
                           const double *sd_end_hi, int flags, double *K, double *sd, double *u, int *status,
                           int *fail_stage, int *counters, void *stream);
+/* The other per-path solves on ragged batches, with the same glen convention (nullable; glen with grid_shared = 1 is
+ * TB_ERR_ARG).  Each path reads only its own glen[p] gridpoints and records; every output entry at or past its own end
+ * is NaN (X, L, K: rows >= glen[p]; sd: >= glen[p]; u / sdd: >= glen[p] - 1).  Everything else as the entry without the
+ * suffix:
+ *   tb_feasible_sets_ragged   = tb_feasible_sets_ex;
+ *   tb_reachable_sets_ragged  = tb_reachable_sets (L is 0 up to glen[p] after a failed stage, as there);
+ *   tb_scan_robust_ragged     = tb_scan_robust (also with TB_SCAN_FEASIBLE_SETS);
+ *   tb_sd_bisect_ragged       = tb_sd_bisect: the durations sum each path's own glen[p] - 1 stages. */
+int tb_feasible_sets_ragged(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
+                            const int *glen, int flags, double *X, void *stream);
+int tb_reachable_sets_ragged(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
+                             const int *glen, const double *sdmin, const double *sdmax, int flags, double *X, double *L,
+                             int *fail_stage, void *stream);
+int tb_scan_robust_ragged(const double *records, int W, int R, int conic_row0, int conic_rows,
+                          const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
+                          const int *glen, const double *sd_start, const double *sd_end, int flags, double *K,
+                          double *sd, double *u, int *status, int *fail_stage, int *counters, void *stream);
+int tb_sd_bisect_ragged(const double *x_fast, const double *u_fast, const double *x_slow, const double *u_slow,
+                        const double *grid, int grid_shared, int B, int G, const int *glen,
+                        const double *desired_duration, double atol, int max_iter, const int *status_in, double *sd,
+                        double *sdd, double *info, int *status, void *stream);
 
 /* K2 fused with K1 for the JointVelocity + JointAcceleration problem (the headline case): no stage records at all.
  * Every lane of the path's warp builds its own LP row in the stage prologue from the spline (same arithmetic as

@@ -21,17 +21,21 @@ def conic_info(ctx, constraints):
     return None
 
 
+def ragged(glen):
+    """Keyword arguments that make an engine call ragged: none on a common grid length, so those calls stay as they are."""
+    return {} if glen is None else {"glen": glen}
+
+
 def scan_any(records, R, grid, conic, sd_start=None, sd_end=None, sd_end_hi=None, backward_only=False,
              counters=False, fast_lower=False, glen=None):
     """K2 for purely linear problems, K2r when a robust constraint is present."""
     if conic is None:
         return engine.scan(records, R, grid, sd_start, sd_end, sd_end_hi, backward_only, counters,
                            fast_lower=fast_lower, glen=glen)
-    if glen is not None:
-        raise NotImplementedError("robust problems on ragged grids")
     if sd_end_hi is not None:
         raise NotImplementedError("robust problems: compute_controllable_sets needs sdmin == sdmax")
-    return engine.scan_robust(records, R, conic[0], conic[1], conic[2], grid, sd_start, sd_end, backward_only, counters)
+    return engine.scan_robust(records, R, conic[0], conic[1], conic[2], grid, sd_start, sd_end, backward_only, counters,
+                              **ragged(glen))
 
 
 def build_records(ctx, constraints, out=None):
@@ -261,13 +265,11 @@ class BatchTOPPRA(object):
         if self.conic is None:
             return engine.scan(self.records, self.R, self.d_grid, s0, s1, sd_end_hi, fast_lower=not self.exact,
                                glen=self.glen, **kw)
-        if self.glen is not None:
-            raise NotImplementedError("robust problems on ragged grids")
         if sd_end_hi is not None:
             raise NotImplementedError("robust problems: compute_controllable_sets needs sdmin == sdmax")
         kw.pop("forward_from", None)
         return engine.scan_robust(self.records, self.R, self.conic[0], self.conic[1], self.conic[2], self.d_grid, s0, s1,
-                                  kw.get("backward_only", False), kw.get("counters", False))
+                                  kw.get("backward_only", False), kw.get("counters", False), **ragged(self.glen))
 
     def _vel_tensor(self, v):
         if v is None:
@@ -367,29 +369,23 @@ class BatchTOPPRA(object):
         """Paths per chunk so that the record buffer stays within max_record_bytes."""
         if self.fused:
             return self.B  # no stage records
+        return self.record_chunk_size()
+
+    def record_chunk_size(self):
+        """Paths per chunk of the methods that always read stage records (feasible and reachable sets), fused or not."""
         rows = sum(c.num_rows(self.ctx) for c in self.constraints)
         per_path = 8 * engine.record_doubles(rows) * self.G
         return max(1, min(self.B, self.max_record_bytes // per_path))
 
-    def compute_parameterization(self, sd_start=0.0, sd_end=0.0, counters=False):
-        """Backward + forward pass for all paths (K1 + K2).  Returns a BatchResult (device tensors).
-        Large batches run in chunks of `chunk_size()` paths (K1 -> K2 per chunk, one record buffer)."""
+    def _chunked(self, nchunk, shapes, solve):
+        """Solve the batch in chunks of `nchunk` paths through ONE record buffer.  Per chunk [lo, hi): its records are built
+        (K1) into the buffer, then solve(lo, hi, records, grid, glen) returns a dict of that chunk's results, which are
+        written into full-batch tensors.  shapes: {key: (shape, dtype)} of those tensors."""
         torch = engine.torch_mod()
-        s0, s1 = self._vel_tensor(sd_start), self._vel_tensor(sd_end)
-        nchunk = self.chunk_size()
-        if nchunk >= self.B:
-            return BatchResult(self._scan(s0, s1, counters=counters))
-        B, G, dev = self.B, self.G, self.device
-        out = dict(K=torch.empty((B, G, 2), dtype=torch.float64, device=dev),
-                   sd=torch.empty((B, G), dtype=torch.float64, device=dev),
-                   u=torch.empty((B, G - 1), dtype=torch.float64, device=dev),
-                   status=torch.empty((B,), dtype=torch.int32, device=dev),
-                   fail_stage=torch.empty((B,), dtype=torch.int32, device=dev))
-        if counters:
-            out["counters"] = torch.empty((B, 4), dtype=torch.int32, device=dev)
+        out = {key: torch.empty(shape, dtype=dt, device=self.device) for key, (shape, dt) in shapes.items()}
         buf = None
-        for lo in range(0, B, nchunk):
-            hi = min(B, lo + nchunk)
+        for lo in range(0, self.B, nchunk):
+            hi = min(self.B, lo + nchunk)
             grid = self.d_grid if self.d_grid.dim() == 1 else self.d_grid[lo:hi]
             glen = None if self.glen is None else self.glen[lo:hi].contiguous()   # ragged grids: the chunk's lengths
             ctx = RecordContext(self.path.chunk(lo, hi), grid, self._grid_host, None, lo, hi)
@@ -398,11 +394,37 @@ class BatchTOPPRA(object):
                 rec = buf
             else:
                 rec, _ = build_records(ctx, self.constraints, out=buf)
-            part = scan_any(rec, self.R, grid, self.conic, None if s0 is None else s0[lo:hi],
-                            None if s1 is None else s1[lo:hi], counters=counters, fast_lower=not self.exact, glen=glen)
+            part = solve(lo, hi, rec, grid, glen)
             for key in out:
                 out[key][lo:hi] = part[key]
-        return BatchResult(out)
+        return out
+
+    def _shapes(self, *keys):
+        """{key: (shape, dtype)} of full-batch results."""
+        torch = engine.torch_mod()
+        B, G = self.B, self.G
+        table = {"K": ((B, G, 2), torch.float64), "X": ((B, G, 2), torch.float64), "L": ((B, G, 2), torch.float64),
+                 "sd": ((B, G), torch.float64), "u": ((B, G - 1), torch.float64), "info": ((B, 4), torch.float64),
+                 "status": ((B,), torch.int32), "fail_stage": ((B,), torch.int32), "counters": ((B, 4), torch.int32)}
+        return {key: table[key] for key in keys}
+
+    def _records(self):
+        """The whole batch's stage records, built once (also for problems whose scan is fused)."""
+        if self.records is None:
+            self.records, self.R = build_records(self.ctx, self.constraints)
+        return self.records
+
+    def compute_parameterization(self, sd_start=0.0, sd_end=0.0, counters=False):
+        """Backward + forward pass for all paths (K1 + K2).  Returns a BatchResult (device tensors).
+        Large batches run in chunks of `chunk_size()` paths (K1 -> K2 per chunk, one record buffer)."""
+        s0, s1 = self._vel_tensor(sd_start), self._vel_tensor(sd_end)
+        nchunk = self.chunk_size()
+        if nchunk >= self.B:
+            return BatchResult(self._scan(s0, s1, counters=counters))
+        keys = ("K", "sd", "u", "status", "fail_stage") + (("counters",) if counters else ())
+        return BatchResult(self._chunked(nchunk, self._shapes(*keys), lambda lo, hi, rec, grid, glen: scan_any(
+            rec, self.R, grid, self.conic, _rows(s0, lo, hi), _rows(s1, lo, hi), counters=counters,
+            fast_lower=not self.exact, glen=glen)))
 
     def compute_controllable_sets(self, sdmin, sdmax):
         """K[B,G,2] with K[N] = [sdmin^2, sdmax^2] (reference reachability_algorithm.py:166-202) and status."""
@@ -410,33 +432,47 @@ class BatchTOPPRA(object):
         hi = np.ascontiguousarray(np.broadcast_to(np.asarray(sdmax, dtype=np.float64), (self.B,)))
         assert np.all(lo <= hi) and np.all(0 <= lo)
         same = bool(np.all(lo == hi))
-        out = self._scan(None, engine.as_device(lo, self.device), None if same else engine.as_device(hi, self.device),
-                         backward_only=True)
+        s1, s1_hi = engine.as_device(lo, self.device), None if same else engine.as_device(hi, self.device)
+        nchunk = self.chunk_size()
+        if nchunk >= self.B:
+            out = self._scan(None, s1, s1_hi, backward_only=True)
+        else:
+            out = self._chunked(nchunk, self._shapes("K", "status"), lambda a, b, rec, grid, glen: scan_any(
+                rec, self.R, grid, self.conic, None, s1[a:b], _rows(s1_hi, a, b), backward_only=True,
+                fast_lower=not self.exact, glen=glen))
         return out["K"], out["status"]
 
     def compute_reachable_sets(self, sdmin, sdmax):
         """Reachable sets L [B, G, 2] of every path (reference compute_reachable_sets, reachability_algorithm.py:378-431)
-        in one launch of tb_reachable_sets (feasible-set pass + forward recursion).  Returns (L, X, fail_stage)."""
-        if self.conic is not None or self.glen is not None:
-            raise NotImplementedError("compute_reachable_sets: linear problems on a common grid length only")
+        in one launch of tb_reachable_sets (feasible-set pass + forward recursion) per record chunk.
+        Returns (L, X, fail_stage)."""
+        if self.conic is not None:
+            raise NotImplementedError("compute_reachable_sets: linear problems only")
         lo = np.ascontiguousarray(np.broadcast_to(np.asarray(sdmin, dtype=np.float64), (self.B,)))
         hi = np.ascontiguousarray(np.broadcast_to(np.asarray(sdmax, dtype=np.float64), (self.B,)))
         assert np.all(lo <= hi) and np.all(0 <= lo)
-        if self.records is None:
-            self.records, self.R = build_records(self.ctx, self.constraints)
-        out = engine.reachable_sets(self.records, self.R, self.d_grid, engine.as_device(lo, self.device),
-                                    engine.as_device(hi, self.device))
+        lo, hi = engine.as_device(lo, self.device), engine.as_device(hi, self.device)
+        nchunk = self.record_chunk_size()
+        if nchunk >= self.B:
+            out = engine.reachable_sets(self._records(), self.R, self.d_grid, lo, hi, **ragged(self.glen))
+        else:
+            out = self._chunked(nchunk, self._shapes("L", "X", "fail_stage"), lambda a, b, rec, grid, glen:
+                                engine.reachable_sets(rec, self.R, grid, lo[a:b], hi[a:b], **ragged(glen)))
         return out["L"], out["X"], out["fail_stage"]
 
     def compute_feasible_sets(self):
-        if self.glen is not None:
-            raise NotImplementedError("compute_feasible_sets on ragged grids")
-        if self.records is None:  # feasible sets read stage records (also for problems whose scan is fused)
-            self.records, self.R = build_records(self.ctx, self.constraints)
-        if self.conic is not None:
-            return engine.scan_robust(self.records, self.R, self.conic[0], self.conic[1], self.conic[2], self.d_grid,
-                                      feasible_sets=True)["K"]
-        return engine.feasible_sets(self.records, self.R, self.d_grid)
+        """Feasible sets X [B, G, 2] of every path (reference compute_feasible_sets, reachability_algorithm.py:131-164),
+        per record chunk."""
+        def solve(lo, hi, rec, grid, glen):
+            if self.conic is not None:
+                return engine.scan_robust(rec, self.R, self.conic[0], self.conic[1], self.conic[2], grid,
+                                          feasible_sets=True, **ragged(glen))
+            return dict(K=engine.feasible_sets(rec, self.R, grid, **ragged(glen)))
+
+        nchunk = self.record_chunk_size()
+        if nchunk >= self.B:
+            return solve(0, self.B, self._records(), self.d_grid, self.glen)["K"]
+        return self._chunked(nchunk, self._shapes("K"), solve)["K"]
 
 
 class BatchTOPPRAsd(BatchTOPPRA):
@@ -449,17 +485,37 @@ class BatchTOPPRAsd(BatchTOPPRA):
         self.desired_duration = desired_duration
 
     def compute_parameterization(self, sd_start=0.0, sd_end=0.0, atol=1e-5):
-        if self.conic is not None or self.glen is not None or self.chunk_size() < self.B:
-            raise NotImplementedError("BatchTOPPRAsd: linear problems on a common grid length in one chunk only")
+        if self.conic is not None:
+            raise NotImplementedError("BatchTOPPRAsd: linear problems only")
         s0, s1 = self._vel_tensor(sd_start), self._vel_tensor(sd_end)
         want = np.ascontiguousarray(np.broadcast_to(np.asarray(self.desired_duration, dtype=np.float64), (self.B,)))
-        fast = self._scan(s0, s1, sd_forward="fast")
-        slow = self._scan(s0, s1, sd_forward="slow")
-        out = engine.sd_bisect(fast["sd"], fast["u"], slow["sd"], slow["u"], self.d_grid,
-                               engine.as_device(want, self.device), atol, status_in=fast["status"])
-        res = BatchResult(dict(K=fast["K"], sd=out["sd"], u=out["u"], status=out["status"], fail_stage=fast["fail_stage"]))
+        want = engine.as_device(want, self.device)
+
+        def solve(lo, hi, rec, grid, glen):
+            a, b = _rows(s0, lo, hi), _rows(s1, lo, hi)
+            if rec is None:   # the whole batch on this problem's own row source
+                fast, slow = self._scan(a, b, sd_forward="fast"), self._scan(a, b, sd_forward="slow")
+            else:
+                fast, slow = (engine.scan(rec, self.R, grid, a, b, sd_forward=mode, fast_lower=not self.exact,
+                                          **ragged(glen)) for mode in ("fast", "slow"))
+            out = engine.sd_bisect(fast["sd"], fast["u"], slow["sd"], slow["u"], grid, want[lo:hi], atol,
+                                   status_in=fast["status"], **ragged(glen))
+            return dict(K=fast["K"], sd=out["sd"], u=out["u"], status=out["status"], fail_stage=fast["fail_stage"],
+                        info=out["info"])
+
+        nchunk = self.chunk_size()
+        if nchunk >= self.B:
+            out = solve(0, self.B, None, self.d_grid, self.glen)
+        else:
+            out = self._chunked(nchunk, self._shapes("K", "sd", "u", "status", "fail_stage", "info"), solve)
+        res = BatchResult(out)
         res.alpha, res.duration_fast, res.duration_slow = out["info"][:, 0], out["info"][:, 1], out["info"][:, 2]
         return res
+
+
+def _rows(t, lo, hi):
+    """Rows [lo, hi) of a per-path tensor, or None."""
+    return None if t is None else t[lo:hi]
 
 
 def solve_batch(ss_waypoints, waypoints, gridpoints, vlim, alim, sd_start=0.0, sd_end=0.0,

@@ -63,10 +63,12 @@ sd_bisect_kernel(const double *__restrict__ x_fast, const double *__restrict__ u
                  const double *__restrict__ u_slow, const double *__restrict__ grid, const int grid_shared, const int B,
                  const int G, const double *__restrict__ desired, const double atol, const int max_iter,
                  const int *__restrict__ status_in, double *__restrict__ sd, double *__restrict__ sdd,
-                 double *__restrict__ info, int *__restrict__ status) {
+                 double *__restrict__ info, int *__restrict__ status, const int *__restrict__ glen) {
   extern __shared__ double sm[];
   const int p = blockIdx.x, lane = threadIdx.x;
   if (p >= B) return;
+  // ragged batches: this path's own gridpoints; strides stay G, entries past them are NaN
+  const int Gp = glen ? min(max(glen[p], 1), G) : G;
   double *sds = sm, *term = sm + G;
   const double *xf = x_fast + (size_t)p * G, *xs = x_slow + (size_t)p * G;
   const double *uf = u_fast + (size_t)p * (G - 1), *us = u_slow + (size_t)p * (G - 1);
@@ -81,8 +83,8 @@ sd_bisect_kernel(const double *__restrict__ x_fast, const double *__restrict__ u
     return;
   }
   const double want = desired[p];
-  const double d_fast = blend_duration(xf, xs, g, G, 1.0, false, sds, term, lane);
-  const double d_slow = blend_duration(xs, xs, g, G, 0.0, false, sds, term, lane);
+  const double d_fast = blend_duration(xf, xs, g, Gp, 1.0, false, sds, term, lane);
+  const double d_slow = blend_duration(xs, xs, g, Gp, 0.0, false, sds, term, lane);
   double alpha;
   int iters = 0;
   if (d_fast > want) {
@@ -95,18 +97,20 @@ sd_bisect_kernel(const double *__restrict__ x_fast, const double *__restrict__ u
     while (diff > atol && iters < max_iter) {
       ++iters;
       alpha = 0.5 * (a_low + a_high);
-      const double d_alpha = blend_duration(xf, xs, g, G, alpha, true, sds, term, lane);
+      const double d_alpha = blend_duration(xf, xs, g, Gp, alpha, true, sds, term, lane);
       if (d_alpha < want) { a_low = alpha; diff = want - d_alpha; }
       else { a_high = alpha; diff = d_alpha - want; }
     }
   }
   bool bad = false;
-  for (int j = lane; j < G; j += 32) {
+  for (int j = lane; j < Gp; j += 32) {
     const double v = sqrt(alpha * xf[j] + (1 - alpha) * xs[j]);
     sdp[j] = v;
     bad = bad || (v != v);
   }
-  for (int j = lane; j < G - 1; j += 32) up[j] = alpha * uf[j] + (1 - alpha) * us[j];
+  for (int j = lane; j < Gp - 1; j += 32) up[j] = alpha * uf[j] + (1 - alpha) * us[j];
+  for (int j = Gp + lane; j < G; j += 32) sdp[j] = nan_d;
+  for (int j = Gp - 1 + lane; j < G - 1; j += 32) up[j] = nan_d;
   bad = __any_sync(FULL, bad);
   if (lane == 0) {
     status[p] = bad ? TB_STATUS_ERR_UNKNOWN : TB_STATUS_OK;
@@ -163,16 +167,18 @@ extern "C" int tb_propose_gridpoints(const double *ppoly, const double *breaks, 
   return check_launch("tb_propose_gridpoints");
 }
 
-extern "C" int tb_sd_bisect(const double *x_fast, const double *u_fast, const double *x_slow, const double *u_slow,
-                            const double *grid, int grid_shared, int B, int G, const double *desired_duration, double atol,
-                            int max_iter, const int *status_in, double *sd, double *sdd, double *info, int *status,
-                            void *stream) {
+extern "C" int tb_sd_bisect_ragged(const double *x_fast, const double *u_fast, const double *x_slow,
+                                   const double *u_slow, const double *grid, int grid_shared, int B, int G,
+                                   const int *glen, const double *desired_duration, double atol, int max_iter,
+                                   const int *status_in, double *sd, double *sdd, double *info, int *status,
+                                   void *stream) {
   using namespace tb;
   if (!x_fast || !u_fast || !x_slow || !u_slow || !grid || !desired_duration || !sd || !sdd || !info || !status || B <= 0 ||
       G < 2) {
     set_error("tb_sd_bisect: bad argument");
     return TB_ERR_ARG;
   }
+  if (glen && grid_shared) { set_error("tb_sd_bisect: ragged batches (glen) need per-path grids [B][G]"); return TB_ERR_ARG; }
   const size_t smem = (size_t)2 * G * sizeof(double);
   if (smem > 200 * 1024) { set_error("tb_sd_bisect: G=%d too large", G); return TB_ERR_UNSUPPORTED; }
   if (smem > 48 * 1024) {
@@ -181,8 +187,16 @@ extern "C" int tb_sd_bisect(const double *x_fast, const double *u_fast, const do
   }
   sd_bisect_kernel<<<B, 32, smem, (cudaStream_t)stream>>>(x_fast, u_fast, x_slow, u_slow, grid, grid_shared, B, G,
                                                          desired_duration, atol, max_iter > 0 ? max_iter : 200, status_in,
-                                                         sd, sdd, info, status);
+                                                         sd, sdd, info, status, glen);
   return check_launch("tb_sd_bisect");
+}
+
+extern "C" int tb_sd_bisect(const double *x_fast, const double *u_fast, const double *x_slow, const double *u_slow,
+                            const double *grid, int grid_shared, int B, int G, const double *desired_duration, double atol,
+                            int max_iter, const int *status_in, double *sd, double *sdd, double *info, int *status,
+                            void *stream) {
+  return tb_sd_bisect_ragged(x_fast, u_fast, x_slow, u_slow, grid, grid_shared, B, G, nullptr, desired_duration, atol,
+                             max_iter, status_in, sd, sdd, info, status, stream);
 }
 
 extern "C" int tb_spline_time_stamps(const double *sd, const double *grid, int grid_shared, const int *glen, int B, int G,

@@ -187,11 +187,20 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
                    const int grid_shared, const int B, const int G, const double *__restrict__ sd_start,
                    const double *__restrict__ sd_end, const int flags, double *__restrict__ Kout,
                    double *__restrict__ sdout, double *__restrict__ uout, int *__restrict__ status,
-                   int *__restrict__ fail_stage, int *__restrict__ counters) {
+                   int *__restrict__ fail_stage, int *__restrict__ counters, const int *__restrict__ glen) {
   const int lane = threadIdx.x & 31;
   const long path = warp_path();
   if (path >= B) return;
-  const int N = G - 1, nC = R + 2;
+  // glen (optional): ragged batches, as in scan_kernel; K / sd / u past this path's gridpoints are NaN
+  const int Gp = glen ? min(max(glen[path], 1), G) : G;
+  const int nC = R + 2;
+  // The stage count lives in shared memory (one warp per CTA) and is re-read where it is used.  Held in a register
+  // across the passes it raises the RPL 1 build's spills under its 72-register cap (-Xptxas -v: 192/368 bytes of spill
+  // stores/loads with a compile-time G - 1, 264/608 with a register-held count, 152/224 like this).
+  volatile __shared__ int s_n;
+  if (lane == 0) s_n = Gp - 1;
+  __syncwarp();
+  const volatile int &N = s_n;
   const double *rec_path = records + (size_t)path * G * W;
   const double *gp = grid + (grid_shared ? 0 : (size_t)path * G);
   double *Kp = Kout + (size_t)path * G * 2;
@@ -199,6 +208,13 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
   double *sdp = backward_only ? nullptr : sdout + (size_t)path * G;
   double *up = backward_only ? nullptr : uout + (size_t)path * (G > 1 ? G - 1 : 0);
   const double nan_d = __longlong_as_double(0x7ff8000000000000LL);
+  // the padding is written up front: no pass below touches it, and the registers that hold Gp and the output pointers
+  // are free here (written at the end, it adds spill traffic to the RPL 1 build)
+  for (int j = 2 * Gp + lane; j < 2 * G; j += 32) Kp[j] = nan_d;
+  if (!(flags & 3)) {
+    for (int j = Gp + lane; j < G; j += 32) sdp[j] = nan_d;
+    for (int j = N + lane; j < G - 1; j += 32) up[j] = nan_d;
+  }
   double a[RPL], b[RPL], c[RPL];
   unsigned cmask[RPL];
   int n_eval = 0, n_retry = 0;
@@ -266,7 +282,7 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
     return;
   }
   if (st != TB_STATUS_OK) {
-    for (int j = lane; j < G; j += 32) sdp[j] = nan_d;
+    for (int j = lane; j < Gp; j += 32) sdp[j] = nan_d;
     for (int j = lane; j < N; j += 32) up[j] = nan_d;
   } else {
     double x = x_start;
@@ -297,7 +313,7 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
         st = TB_STATUS_ERR_UNKNOWN;
         fstage = i;
         if (lane == 0) sdp[i] = x;
-        for (int j = i + 1 + lane; j < G; j += 32) sdp[j] = nan_d;
+        for (int j = i + 1 + lane; j < Gp; j += 32) sdp[j] = nan_d;
         for (int j = i + lane; j < N; j += 32) up[j] = 0.0;
         break;
       }
@@ -312,7 +328,7 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
       x = x_next;
     }
     __syncwarp();
-    for (int j = lane; j < G; j += 32) sdp[j] = sqrt(sdp[j]);
+    for (int j = lane; j < Gp; j += 32) sdp[j] = sqrt(sdp[j]);
   }
   if (lane == 0) {
     status[path] = st;
@@ -329,15 +345,16 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
 }  // namespace
 }  // namespace tb
 
-extern "C" int tb_scan_robust(const double *records, int W, int R, int conic_row0, int conic_rows,
-                              const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
-                              const double *sd_start, const double *sd_end, int flags, double *K, double *sd, double *u,
-                              int *status, int *fail_stage, int *counters, void *stream) {
+extern "C" int tb_scan_robust_ragged(const double *records, int W, int R, int conic_row0, int conic_rows,
+                                     const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
+                                     const int *glen, const double *sd_start, const double *sd_end, int flags, double *K,
+                                     double *sd, double *u, int *status, int *fail_stage, int *counters, void *stream) {
   using namespace tb;
   if (!records || !grid || !ellipsoid_host3 || !K || !status || B <= 0 || G <= 0 || R < 0) {
     set_error("tb_scan_robust: bad argument");
     return TB_ERR_ARG;
   }
+  if (glen && grid_shared) { set_error("tb_scan_robust: ragged batches (glen) need per-path grids [B][G]"); return TB_ERR_ARG; }
   const bool backward_only = (flags & (TB_SCAN_BACKWARD_ONLY | TB_SCAN_FEASIBLE_SETS)) != 0;
   if (!backward_only && (!sd || (G > 1 && !u))) { set_error("tb_scan_robust: null output"); return TB_ERR_ARG; }
   if (R > MAX_ROWS) { set_error("tb_scan_robust: R=%d > %d rows", R, MAX_ROWS); return TB_ERR_UNSUPPORTED; }
@@ -348,7 +365,15 @@ extern "C" int tb_scan_robust(const double *records, int W, int R, int conic_row
   with_rows_per_lane(R + 2, [&](auto rpl) {
     scan_robust_kernel<rpl.value><<<B, 32, 0, (cudaStream_t)stream>>>(records, W, R, conic_row0, conic_rows, ru, rx, rc,
                                                                       grid, grid_shared, B, G, sd_start, sd_end, flags,
-                                                                      K, sd, u, status, fail_stage, counters);
+                                                                      K, sd, u, status, fail_stage, counters, glen);
   });
   return check_launch("tb_scan_robust");
+}
+
+extern "C" int tb_scan_robust(const double *records, int W, int R, int conic_row0, int conic_rows,
+                              const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
+                              const double *sd_start, const double *sd_end, int flags, double *K, double *sd, double *u,
+                              int *status, int *fail_stage, int *counters, void *stream) {
+  return tb_scan_robust_ragged(records, W, R, conic_row0, conic_rows, ellipsoid_host3, grid, grid_shared, B, G, nullptr,
+                               sd_start, sd_end, flags, K, sd, u, status, fail_stage, counters, stream);
 }

@@ -784,15 +784,19 @@ __device__ __forceinline__ void feasible_pass(const double *records, const long 
 template <int RPL>
 __global__ void __launch_bounds__(32)
 feasible_kernel(const double *__restrict__ records, const int W, const int R, const double *__restrict__ grid,
-                const int grid_shared, const int B, const int G, const int ub, double *__restrict__ Xout) {
+                const int grid_shared, const int B, const int G, const int ub, double *__restrict__ Xout,
+                const int *__restrict__ glen) {
   const int lane = threadIdx.x & 31;
   const long path = warp_path();
   if (path >= B) return;
-  const int N = G - 1, nC = R + 2;
+  // glen (optional): ragged batches, as in scan_kernel; X past this path's gridpoints is NaN
+  const int Gp = glen ? min(max(glen[path], 1), G) : G;
+  const int N = Gp - 1, nC = R + 2;
   const double *gp = grid + (grid_shared ? 0 : (size_t)path * G);
   double *Xp = Xout + (size_t)path * G * 2;
   double a[RPL], b[RPL], c[RPL];
   int up0 = 0, up1 = 0, dn0 = 0, dn1 = 0, n_resolve = 0;
+  for (int j = 2 * Gp + lane; j < 2 * G; j += 32) Xp[j] = __longlong_as_double(0x7ff8000000000000LL);
   feasible_pass<RPL>(records, path, G, W, R, nC, gp, N, ub != 0, lane, Xp, a, b, c, up0, up1, dn0, dn1, n_resolve);
 }
 
@@ -851,11 +855,13 @@ __global__ void __launch_bounds__(32)
 reachable_kernel(const double *__restrict__ records, const int W, const int R, const double *__restrict__ grid,
                  const int grid_shared, const int B, const int G, const double *__restrict__ sdmin,
                  const double *__restrict__ sdmax, double *__restrict__ Xout, double *__restrict__ Lout,
-                 int *__restrict__ fail_stage) {
+                 int *__restrict__ fail_stage, const int *__restrict__ glen) {
   const int lane = threadIdx.x & 31;
   const long path = warp_path();
   if (path >= B) return;
-  const int N = G - 1, nC = R + 2;
+  // glen (optional): ragged batches, as in scan_kernel; X and L past this path's gridpoints are NaN
+  const int Gp = glen ? min(max(glen[path], 1), G) : G;
+  const int N = Gp - 1, nC = R + 2;
   const double *rec_path = records + (size_t)path * G * W;
   const double *gp = grid + (grid_shared ? 0 : (size_t)path * G);
   double *Xp = Xout + (size_t)path * G * 2;
@@ -863,12 +869,13 @@ reachable_kernel(const double *__restrict__ records, const int W, const int R, c
   double a[RPL], b[RPL], c[RPL];
   int up0 = 0, up1 = 0, dn0 = 0, dn1 = 0, n_resolve = 0;
   const double nan_d = __longlong_as_double(0x7ff8000000000000LL);
+  for (int j = 2 * Gp + lane; j < 2 * G; j += 32) { Xp[j] = nan_d; Lp[j] = nan_d; }   // no pass below writes these
   feasible_pass<RPL>(records, path, G, W, R, nC, gp, N, UB, lane, Xp, a, b, c, up0, up1, dn0, dn1, n_resolve);
   __syncwarp();
   // ---- reachable sets ----
   const double s0 = sdmin ? sdmin[path] : 0.0, s1 = sdmax ? sdmax[path] : s0;
   double l0 = s0 * s0, l1 = s1 * s1;
-  for (int j = 2 * lane; j < 2 * G; j += 64) { Lp[j] = 0.0; Lp[j + 1] = 0.0; }   // np.zeros((N + 1, 2))
+  for (int j = 2 * lane; j < 2 * Gp; j += 64) { Lp[j] = 0.0; Lp[j + 1] = 0.0; }   // np.zeros((N + 1, 2))
   __syncwarp();
   if (lane == 0) { Lp[0] = l0; Lp[1] = l1; }
   int fs = -1;
@@ -1077,19 +1084,21 @@ int launch_scan_velacc(const VelAccSrc &src, int W, int R, const double *grid, i
 
 template <int RPL>
 int launch_feasible(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
-                    int ub, double *X, cudaStream_t stream) {
-  feasible_kernel<RPL><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, ub, X);
+                    const int *glen, int ub, double *X, cudaStream_t stream) {
+  feasible_kernel<RPL><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, ub, X, glen);
   return check_launch("tb_feasible_sets");
 }
 
 template <int RPL>
 int launch_reachable(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
-                     const double *sdmin, const double *sdmax, int flags, double *X, double *L, int *fail_stage,
-                     cudaStream_t stream) {
+                     const int *glen, const double *sdmin, const double *sdmax, int flags, double *X, double *L,
+                     int *fail_stage, cudaStream_t stream) {
   if (flags & TB_SCAN_UBOUND)
-    reachable_kernel<RPL, true><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, X, L, fail_stage);
+    reachable_kernel<RPL, true><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, X, L,
+                                                      fail_stage, glen);
   else
-    reachable_kernel<RPL, false><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, X, L, fail_stage);
+    reachable_kernel<RPL, false><<<B, 32, 0, stream>>>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, X, L,
+                                                       fail_stage, glen);
   return check_launch("tb_reachable_sets");
 }
 
@@ -1173,17 +1182,23 @@ extern "C" int tb_scan(const double *records, int W, int R, const double *grid, 
                     nullptr, stream);
 }
 
-extern "C" int tb_feasible_sets_ex(const double *records, int W, int R, const double *grid, int grid_shared, int B,
-                                   int G, int flags, double *X, void *stream) {
+extern "C" int tb_feasible_sets_ragged(const double *records, int W, int R, const double *grid, int grid_shared, int B,
+                                       int G, const int *glen, int flags, double *X, void *stream) {
   using namespace tb;
   int rc = check_scan_args("tb_feasible_sets", records, W, R, grid, B, G);
   if (rc) return rc;
   if (!X) { set_error("tb_feasible_sets: null output"); return TB_ERR_ARG; }
+  if (glen && grid_shared) { set_error("tb_feasible_sets: ragged batches (glen) need per-path grids [B][G]"); return TB_ERR_ARG; }
   const int ub = (flags & TB_SCAN_UBOUND) ? 1 : 0;
   if (ub && W < 3 * R + 4) { set_error("tb_feasible_sets: TB_SCAN_UBOUND needs W >= 3R+4"); return TB_ERR_ARG; }
   return with_rows_per_lane(R + 2, [&](auto rpl) {
-    return launch_feasible<rpl.value>(records, W, R, grid, grid_shared, B, G, ub, X, (cudaStream_t)stream);
+    return launch_feasible<rpl.value>(records, W, R, grid, grid_shared, B, G, glen, ub, X, (cudaStream_t)stream);
   });
+}
+
+extern "C" int tb_feasible_sets_ex(const double *records, int W, int R, const double *grid, int grid_shared, int B,
+                                   int G, int flags, double *X, void *stream) {
+  return tb_feasible_sets_ragged(records, W, R, grid, grid_shared, B, G, nullptr, flags, X, stream);
 }
 
 extern "C" int tb_feasible_sets(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
@@ -1191,18 +1206,26 @@ extern "C" int tb_feasible_sets(const double *records, int W, int R, const doubl
   return tb_feasible_sets_ex(records, W, R, grid, grid_shared, B, G, 0, X, stream);
 }
 
-extern "C" int tb_reachable_sets(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
-                                 const double *sdmin, const double *sdmax, int flags, double *X, double *L,
-                                 int *fail_stage, void *stream) {
+extern "C" int tb_reachable_sets_ragged(const double *records, int W, int R, const double *grid, int grid_shared,
+                                        int B, int G, const int *glen, const double *sdmin, const double *sdmax,
+                                        int flags, double *X, double *L, int *fail_stage, void *stream) {
   using namespace tb;
   int rc = check_scan_args("tb_reachable_sets", records, W, R, grid, B, G);
   if (rc) return rc;
   if (!X || !L) { set_error("tb_reachable_sets: null output"); return TB_ERR_ARG; }
+  if (glen && grid_shared) { set_error("tb_reachable_sets: ragged batches (glen) need per-path grids [B][G]"); return TB_ERR_ARG; }
   if ((flags & TB_SCAN_UBOUND) && W < 3 * R + 4) { set_error("tb_reachable_sets: TB_SCAN_UBOUND needs W >= 3R+4"); return TB_ERR_ARG; }
   return with_rows_per_lane(R + 2, [&](auto rpl) {
-    return launch_reachable<rpl.value>(records, W, R, grid, grid_shared, B, G, sdmin, sdmax, flags, X, L, fail_stage,
-                                       (cudaStream_t)stream);
+    return launch_reachable<rpl.value>(records, W, R, grid, grid_shared, B, G, glen, sdmin, sdmax, flags, X, L,
+                                       fail_stage, (cudaStream_t)stream);
   });
+}
+
+extern "C" int tb_reachable_sets(const double *records, int W, int R, const double *grid, int grid_shared, int B, int G,
+                                 const double *sdmin, const double *sdmax, int flags, double *X, double *L,
+                                 int *fail_stage, void *stream) {
+  return tb_reachable_sets_ragged(records, W, R, grid, grid_shared, B, G, nullptr, sdmin, sdmax, flags, X, L, fail_stage,
+                                  stream);
 }
 
 extern "C" int tb_lp2d_batch(const double *v, const double *a, const double *b, const double *c, const double *low,

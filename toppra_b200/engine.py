@@ -416,8 +416,9 @@ def scan_velacc(ppoly, breaks, grid, alim, interp, xbound, sd_start=None, sd_end
 
 
 def scan_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, sd_start=None, sd_end=None, backward_only=False,
-                counters=False, feasible_sets=False):
-    """K2r: like scan() with rows [conic_row0, conic_row0+conic_rows) robustified by the ellipsoid (ru, rx, rc)."""
+                counters=False, feasible_sets=False, glen=None):
+    """K2r: like scan() with rows [conic_row0, conic_row0+conic_rows) robustified by the ellipsoid (ru, rx, rc).
+    glen: optional int32 [B] gridpoints per path (ragged batch, tb_scan_robust_ragged)."""
     torch = torch_mod()
     B, G, W = records.shape
     dev = records.device
@@ -425,47 +426,68 @@ def scan_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, sd_start=No
     out, u_arg = _scan_outputs(B, G, dev, backward_only, counters)
     ell = np.ascontiguousarray(ellipsoid, dtype=np.float64)
     assert ell.shape == (3,)
+    lib = _lib.load()
+    args = (_lib.ptr(records), W, int(R), int(conic_row0), int(conic_rows), ctypes.c_void_p(ell.ctypes.data),
+            _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G)
+    rest = (_lib.ptr(sd_start), _lib.ptr(sd_end), 2 if feasible_sets else (1 if backward_only else 0),
+            _lib.ptr(out["K"]), _lib.ptr(out["sd"]), _lib.ptr(u_arg), _lib.ptr(out["status"]),
+            _lib.ptr(out["fail_stage"]), _lib.ptr(out.get("counters")), _lib.stream_ptr())
+    if glen is not None:
+        check_grid(grid, B, G)
+        check_glen(glen, B, grid)
+        with torch.cuda.device(dev):
+            rc = lib.tb_scan_robust_ragged(*args, _lib.ptr(glen), *rest)
+        _lib.check(rc, "tb_scan_robust_ragged")
+        return out
     with torch.cuda.device(dev):
-        rc = _lib.load().tb_scan_robust(_lib.ptr(records), W, int(R), int(conic_row0), int(conic_rows),
-                                        ctypes.c_void_p(ell.ctypes.data), _lib.ptr(grid), 1 if grid.dim() == 1 else 0,
-                                        B, G, _lib.ptr(sd_start), _lib.ptr(sd_end),
-                                        2 if feasible_sets else (1 if backward_only else 0),
-                                        _lib.ptr(out["K"]), _lib.ptr(out["sd"]), _lib.ptr(u_arg), _lib.ptr(out["status"]),
-                                        _lib.ptr(out["fail_stage"]), _lib.ptr(out.get("counters")), _lib.stream_ptr())
+        rc = lib.tb_scan_robust(*args, *rest)
     _lib.check(rc, "tb_scan_robust")
     return out
 
 
-def feasible_sets(records, R, grid):
+def feasible_sets(records, R, grid, glen=None):
+    """compute_feasible_sets for B paths: X [B,G,2].  glen: optional int32 [B] gridpoints per path (ragged batch,
+    tb_feasible_sets_ragged; X past a path's own gridpoints is NaN)."""
     torch = torch_mod()
     B, G, W = records.shape
     check_grid(grid, B, G)
+    check_glen(glen, B, grid)
     X = torch.empty((B, G, 2), dtype=torch.float64, device=records.device)
+    lib = _lib.load()
+    args = (_lib.ptr(records), W, int(R), _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G)
+    flags = SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0
     with torch.cuda.device(records.device):
-        rc = _lib.load().tb_feasible_sets_ex(_lib.ptr(records), W, int(R), _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B,
-                                             G, SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0, _lib.ptr(X),
-                                             _lib.stream_ptr())
+        if glen is None:
+            rc = lib.tb_feasible_sets_ex(*args, flags, _lib.ptr(X), _lib.stream_ptr())
+        else:
+            rc = lib.tb_feasible_sets_ragged(*args, _lib.ptr(glen), flags, _lib.ptr(X), _lib.stream_ptr())
     _lib.check(rc, "tb_feasible_sets")
     return X
 
 
-def reachable_sets(records, R, grid, sdmin=None, sdmax=None):
+def reachable_sets(records, R, grid, sdmin=None, sdmax=None, glen=None):
     """compute_reachable_sets for B paths in one launch (tb_reachable_sets).  sdmin / sdmax: [B] tensors or None.
-    Returns dict(X [B,G,2] feasible sets, L [B,G,2] reachable sets, fail_stage [B] int32)."""
+    Returns dict(X [B,G,2] feasible sets, L [B,G,2] reachable sets, fail_stage [B] int32).  glen: optional int32 [B]
+    gridpoints per path (ragged batch, tb_reachable_sets_ragged; X and L past a path's own gridpoints are NaN)."""
     torch = torch_mod()
     B, G, W = records.shape
     dev = records.device
     check_grid(grid, B, G)
+    check_glen(glen, B, grid)
     for t, what in ((sdmin, "sdmin"), (sdmax, "sdmax")):
         check_path_vector(t, B, what)
     X = torch.empty((B, G, 2), dtype=torch.float64, device=dev)
     L = torch.empty((B, G, 2), dtype=torch.float64, device=dev)
     fs = torch.empty((B,), dtype=torch.int32, device=dev)
+    lib = _lib.load()
+    args = (_lib.ptr(records), W, int(R), _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G)
+    rest = (_lib.ptr(sdmin), _lib.ptr(sdmax), SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0, _lib.ptr(X),
+            _lib.ptr(L), _lib.ptr(fs), _lib.stream_ptr())
     with torch.cuda.device(dev):
-        rc = _lib.load().tb_reachable_sets(_lib.ptr(records), W, int(R), _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G,
-                                           _lib.ptr(sdmin), _lib.ptr(sdmax),
-                                           SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0, _lib.ptr(X), _lib.ptr(L),
-                                           _lib.ptr(fs), _lib.stream_ptr())
+        if glen is None:
+            rc = lib.tb_reachable_sets(*args, *rest)
+        else:
+            rc = lib.tb_reachable_sets_ragged(*args, _lib.ptr(glen), *rest)
     _lib.check(rc, "tb_reachable_sets")
     return dict(X=X, L=L, fail_stage=fs)
 
@@ -500,13 +522,14 @@ def propose_gridpoints(ppoly, breaks, max_err_threshold=1e-4, max_iteration=100,
     return grid, glen, status
 
 
-def sd_bisect(x_fast, u_fast, x_slow, u_slow, grid, desired, atol=1e-5, status_in=None, max_iter=200):
+def sd_bisect(x_fast, u_fast, x_slow, u_slow, grid, desired, atol=1e-5, status_in=None, max_iter=200, glen=None):
     """TOPPRAsd blend (tb_sd_bisect).  Returns dict(sd [B,G], u [B,G-1], info [B,4] = (alpha, fastest, slowest duration,
-    bisection steps), status [B])."""
+    bisection steps), status [B]).  glen: optional int32 [B] gridpoints per path (ragged batch, tb_sd_bisect_ragged)."""
     torch = torch_mod()
     B, G = x_fast.shape
     dev = x_fast.device
     check_grid(grid, B, G)
+    check_glen(glen, B, grid)
     check_path_vector(desired, B, "desired_duration")
     check_shape(x_slow, (B, G), "x_slow")
     for t, what in ((u_fast, "u_fast"), (u_slow, "u_slow")):
@@ -517,11 +540,16 @@ def sd_bisect(x_fast, u_fast, x_slow, u_slow, grid, desired, atol=1e-5, status_i
     u = torch.empty((B, G - 1), dtype=torch.float64, device=dev)
     info = torch.empty((B, 4), dtype=torch.float64, device=dev)
     status = torch.empty((B,), dtype=torch.int32, device=dev)
+    lib = _lib.load()
+    args = (_lib.ptr(x_fast), _lib.ptr(u_fast), _lib.ptr(x_slow), _lib.ptr(u_slow), _lib.ptr(grid),
+            1 if grid.dim() == 1 else 0, B, G)
+    rest = (_lib.ptr(desired), float(atol), int(max_iter), _lib.ptr(status_in), _lib.ptr(sd), _lib.ptr(u), _lib.ptr(info),
+            _lib.ptr(status), _lib.stream_ptr())
     with torch.cuda.device(dev):
-        rc = _lib.load().tb_sd_bisect(_lib.ptr(x_fast), _lib.ptr(u_fast), _lib.ptr(x_slow), _lib.ptr(u_slow),
-                                      _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G, _lib.ptr(desired), float(atol),
-                                      int(max_iter), _lib.ptr(status_in), _lib.ptr(sd), _lib.ptr(u), _lib.ptr(info),
-                                      _lib.ptr(status), _lib.stream_ptr())
+        if glen is None:
+            rc = lib.tb_sd_bisect(*args, *rest)
+        else:
+            rc = lib.tb_sd_bisect_ragged(*args, _lib.ptr(glen), *rest)
     _lib.check(rc, "tb_sd_bisect")
     return dict(sd=sd, u=u, info=info, status=status)
 
