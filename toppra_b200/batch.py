@@ -479,21 +479,24 @@ class BatchTOPPRAsd(BatchTOPPRA):
     """TOPPRAsd (reference desired_duration_algorithm.py:20-234) for B paths: every path gets the convex combination of
     its fastest and slowest parameterisation whose duration is `desired_duration` (scalar or [B]); unachievable
     durations return the fastest / slowest one.  Three launches: two scans (TB_SCAN_SD_FORWARD [| TB_SCAN_SD_SLOW]) and
-    the per-path bisection tb_sd_bisect (csrc/tb_frows.cu)."""
+    the per-path bisection tb_sd_bisect (csrc/tb_frows.cu).  Problems with a robust (conic) constraint run the conic
+    backward pass once (tb_scan_robust, backward only), both forward passes in one launch of tbr_sd_forward_robust
+    (csrc/tb_conic.cu), then tb_sd_bisect."""
 
     def set_desired_duration(self, desired_duration):
         self.desired_duration = desired_duration
 
     def compute_parameterization(self, sd_start=0.0, sd_end=0.0, atol=1e-5):
-        if self.conic is not None:
-            raise NotImplementedError("BatchTOPPRAsd: linear problems only")
         s0, s1 = self._vel_tensor(sd_start), self._vel_tensor(sd_end)
         want = np.ascontiguousarray(np.broadcast_to(np.asarray(self.desired_duration, dtype=np.float64), (self.B,)))
         want = engine.as_device(want, self.device)
 
         def solve(lo, hi, rec, grid, glen):
             a, b = _rows(s0, lo, hi), _rows(s1, lo, hi)
-            if rec is None:   # the whole batch on this problem's own row source
+            if self.conic is not None:
+                fast, slow = sd_passes_robust(self._records() if rec is None else rec, self.R, self.conic, grid, a, b,
+                                              glen)
+            elif rec is None:   # the whole batch on this problem's own row source
                 fast, slow = self._scan(a, b, sd_forward="fast"), self._scan(a, b, sd_forward="slow")
             else:
                 fast, slow = (engine.scan(rec, self.R, grid, a, b, sd_forward=mode, fast_lower=not self.exact,
@@ -516,6 +519,18 @@ class BatchTOPPRAsd(BatchTOPPRA):
 def _rows(t, lo, hi):
     """Rows [lo, hi) of a per-path tensor, or None."""
     return None if t is None else t[lo:hi]
+
+
+def sd_passes_robust(records, R, conic, grid, sd_start, sd_end, glen=None):
+    """TOPPRAsd's fastest and slowest pass of robust problems: the conic backward pass once (tb_scan_robust, backward
+    only), then both forward passes in one tbr_sd_forward_robust launch.  Returns (fast, slow) in the form of
+    engine.scan(..., sd_forward=...): K, sd (= x = sd^2), u, status, fail_stage (K / status / fail_stage in `fast`)."""
+    back = engine.scan_robust(records, R, conic[0], conic[1], conic[2], grid, None, sd_end, backward_only=True,
+                              **ragged(glen))
+    fwd = engine.sd_forward_robust(records, R, conic[0], conic[1], conic[2], grid, back["K"], back["status"], sd_start,
+                                   **ragged(glen))
+    fast = dict(K=back["K"], sd=fwd["x_fast"], u=fwd["u_fast"], status=fwd["status"], fail_stage=fwd["fail_stage"])
+    return fast, dict(sd=fwd["x_slow"], u=fwd["u_slow"])
 
 
 def solve_batch(ss_waypoints, waypoints, gridpoints, vlim, alim, sd_start=0.0, sd_end=0.0,

@@ -6,7 +6,7 @@ import ctypes
 
 import numpy as np
 
-from . import _lib, _lib_poly
+from . import _lib, _lib_poly, _lib_robust
 
 BC_KINDS = {"not-a-knot": 0, "clamped": 1, "natural": 2, "periodic": 3}
 
@@ -443,6 +443,62 @@ def scan_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, sd_start=No
         rc = lib.tb_scan_robust(*args, *rest)
     _lib.check(rc, "tb_scan_robust")
     return out
+
+
+def sd_forward_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, K, status_in, sd_start=None, glen=None):
+    """The fastest and the slowest TOPPRAsd forward pass of robust problems in one launch (tbr_sd_forward_robust), on K
+    and status of a backward-only scan_robust over the same records.  Returns dict(x_fast, x_slow [B,G] = sd^2,
+    u_fast, u_slow [B,G-1], status [B], fail_stage [B] int32 of the fastest pass).  glen: optional int32 [B] gridpoints
+    per path (ragged batch)."""
+    torch = torch_mod()
+    B, G, W = records.shape
+    dev = records.device
+    check_grid(grid, B, G)
+    check_glen(glen, B, grid)
+    check_path_vector(sd_start, B, "sd_start")
+    check_shape(K, (B, G, 2), "K")
+    if status_in.dtype != torch.int32 or tuple(status_in.shape) != (B,):
+        raise ValueError("status_in must be an int32 tensor of shape (%d,)" % B)
+    ell = np.ascontiguousarray(ellipsoid, dtype=np.float64)
+    assert ell.shape == (3,)
+    out = {key: torch.empty((B, G), dtype=torch.float64, device=dev) for key in ("x_fast", "x_slow")}
+    out.update({key: torch.empty((B, max(G - 1, 0)), dtype=torch.float64, device=dev) for key in ("u_fast", "u_slow")})
+    out["status"] = torch.empty((B,), dtype=torch.int32, device=dev)
+    out["fail_stage"] = torch.empty((B,), dtype=torch.int32, device=dev)
+    u_fast, u_slow = (out[k] if G > 1 else None for k in ("u_fast", "u_slow"))
+    with torch.cuda.device(dev):
+        rc = _lib_robust.load().tbr_sd_forward_robust(
+            _lib.ptr(records), W, int(R), int(conic_row0), int(conic_rows), ctypes.c_void_p(ell.ctypes.data),
+            _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G, _lib.ptr(glen), _lib.ptr(K), _lib.ptr(status_in),
+            _lib.ptr(sd_start), _lib.ptr(out["x_fast"]), _lib.ptr(u_fast), _lib.ptr(out["x_slow"]), _lib.ptr(u_slow),
+            _lib.ptr(out["status"]), _lib.ptr(out["fail_stage"]), _lib.stream_ptr())
+    _lib.check(rc, "tbr_sd_forward_robust")
+    return out
+
+
+def socp_stage_batch(g, a, b, c, conic_row0, conic_rows, ellipsoid, xbox, xnext=None):
+    """Batched robust stage problems on device (tbr_socp_stage_batch): min g0 u + g1 x over the rows a, b, c [B, n]
+    (robust on [conic_row0, conic_row0 + conic_rows)), xbox [B, 2] and the optional x_next rows xnext [B, 3] =
+    (delta, lo, hi) (NaN delta = none).  Inputs numpy or tensors.  Returns numpy optvar [B, 2] = (u, x), NaN if
+    infeasible."""
+    torch = torch_mod()
+    dev = default_device()
+    g = as_device(g, dev).reshape(-1, 2)
+    B = g.shape[0]
+    a, b, c = (as_device(t, dev).reshape(B, -1) for t in (a, b, c))
+    n = a.shape[1]
+    xbox = as_device(xbox, dev).reshape(B, 2)
+    xnext = None if xnext is None else as_device(xnext, dev).reshape(B, 3)
+    ell = np.ascontiguousarray(ellipsoid, dtype=np.float64)
+    assert ell.shape == (3,)
+    optvar = torch.empty((B, 2), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib_robust.load().tbr_socp_stage_batch(
+            _lib.ptr(g), _lib.ptr(a) if n else None, _lib.ptr(b) if n else None, _lib.ptr(c) if n else None, n,
+            int(conic_row0), int(conic_rows), ctypes.c_void_p(ell.ctypes.data), _lib.ptr(xbox), _lib.ptr(xnext), B,
+            _lib.ptr(optvar), _lib.stream_ptr())
+    _lib.check(rc, "tbr_socp_stage_batch")
+    return optvar.cpu().numpy()
 
 
 def feasible_sets(records, R, grid, glen=None):

@@ -10,6 +10,7 @@ seidelWrapper.__init__) and exposes
 import numpy as np
 
 from .. import engine
+from ..constants import ECOS_INFTY, ECOS_MAXX
 from ..constraint import RecordContext
 
 
@@ -117,9 +118,12 @@ class B200SolverWrapper(SolverWrapper):
     def solve_stagewise_optim(self, i, H, g, x_min, x_max, x_next_min, x_next_max):
         """One stage LP, reference semantics (cy_seidel_solverwrapper.pyx:549-697): min g.[u,x] subject to the
         stage-i rows, x_min <= x <= x_max, x_next_min <= x + 2 delta_i u <= x_next_max (NaN = bound absent).
-        Returns [u, x] or [nan, nan] when infeasible.  One small launch per call (tb_lp1d_batch / tb_lp2d_batch)."""
+        Returns [u, x] or [nan, nan] when infeasible.  One small launch per call (tb_lp1d_batch / tb_lp2d_batch).
+        Problems with a robust (conic) constraint: the second-order-cone program of ecosWrapper.solve_stagewise_optim
+        (ecos_solverwrapper.py:90-207), one tbr_socp_stage_batch launch."""
         assert 0 <= i <= self.N
-        self._no_conic("solve_stagewise_optim")
+        if self.conic is not None:
+            return self._solve_stage_conic(i, H, g, x_min, x_max, x_next_min, x_next_max)
         if self._rows_host is None:
             self._rows_host = self.rows()
         rows = self._rows_host
@@ -151,6 +155,25 @@ class B200SolverWrapper(SolverWrapper):
         slot[:] = act[0]
         return optvar[0].copy()
 
+    def _solve_stage_conic(self, i, H, g, x_min, x_max, x_next_min, x_next_max):
+        """ecos_solverwrapper.py:90-207: absent x / x_next bounds are -/+ECOS_INFTY, the xbound rows give
+        x >= xbound_lo and x <= min(ECOS_MAXX, xbound_hi); no x_next rows at the last stage."""
+        assert H is None or np.allclose(H, np.zeros(2))
+        if self._rows_host is None:
+            self._rows_host = self.rows()
+        rows, R = self._rows_host, self.R
+        xlo = -ECOS_INFTY if np.isnan(x_min) else x_min
+        xhi = ECOS_INFTY if np.isnan(x_max) else x_max
+        xbox = [max(xlo, rows["low"][i][1]), min(xhi, min(ECOS_MAXX, rows["high"][i][1]))]
+        xnext = None
+        if i < self.N:
+            xnext = [[self.deltas[i], -ECOS_INFTY if np.isnan(x_next_min) else x_next_min,
+                      ECOS_INFTY if np.isnan(x_next_max) else x_next_max]]
+        g = np.asarray(g, dtype=np.float64)[:2]
+        return engine.socp_stage_batch(g[None], rows["a"][i][None, 2:2 + R], rows["b"][i][None, 2:2 + R],
+                                       rows["c"][i][None, 2:2 + R], self.conic[0], self.conic[1], self.conic[2],
+                                       np.array([xbox]), xnext)[0]
+
     # ---- whole-pass entry points ---------------------------------------------------------------------
     def _scalar(self, v):
         return engine.as_device(np.array([float(v)]), self.ctx.device)
@@ -171,11 +194,15 @@ class B200SolverWrapper(SolverWrapper):
         return res
 
     def parameterize_sd(self, sd_start, sd_end, desired_duration, atol=1e-5):
-        """TOPPRAsd on the device: two scans (fastest / slowest forward rules) + tb_sd_bisect; host arrays out."""
-        self._no_conic("TOPPRAsd")
+        """TOPPRAsd on the device: two scans (fastest / slowest forward rules) + tb_sd_bisect; host arrays out.  Robust
+        problems: one backward-only conic scan, both forward passes in one tbr_sd_forward_robust launch, tb_sd_bisect."""
+        from ..batch import sd_passes_robust
         s0, s1 = self._scalar(sd_start), self._scalar(sd_end)
-        fast = engine.scan(self.records, self.R, self.ctx.d_grid, s0, s1, sd_forward="fast")
-        slow = engine.scan(self.records, self.R, self.ctx.d_grid, s0, s1, sd_forward="slow")
+        if self.conic is not None:
+            fast, slow = sd_passes_robust(self.records, self.R, self.conic, self.ctx.d_grid, s0, s1)
+        else:
+            fast = engine.scan(self.records, self.R, self.ctx.d_grid, s0, s1, sd_forward="fast")
+            slow = engine.scan(self.records, self.R, self.ctx.d_grid, s0, s1, sd_forward="slow")
         out = engine.sd_bisect(fast["sd"], fast["u"], slow["sd"], slow["u"], self.ctx.d_grid,
                                self._scalar(desired_duration), atol, status_in=fast["status"])
         info = out["info"][0].cpu().numpy()
