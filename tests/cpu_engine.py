@@ -400,7 +400,9 @@ def reachable_sets(records, R, grid, sdmin=None, sdmax=None):
 
 def propose_gridpoints(ppoly, breaks, max_err_threshold=1e-4, max_iteration=100, max_seg_length=0.05, min_nb_points=100,
                        max_points=2048):
-    """interpolator.py:49-122 per path on the oracle's PPoly evaluation."""
+    """interpolator.py:49-122 per path on the oracle's PPoly evaluation.  Failures as in tb_propose_gridpoints: status 1
+    (the last allowed pass ran; the reference raises) skips the doubling, and status -2 (a pass or the doubling would
+    exceed max_points) returns the last list that fitted."""
     pp, br = _np(ppoly), _np(breaks)
     B = pp.shape[0]
     grid = np.zeros((B, max_points))
@@ -408,25 +410,30 @@ def propose_gridpoints(ppoly, breaks, max_err_threshold=1e-4, max_iteration=100,
     for b in range(B):
         x = _per_path(br, b)
         pts = [x[0], x[-1]]
-        it = 0
+        it, st, converged = 0, 0, False
         for it in range(max_iteration):
             arr = np.asarray(pts)
             mids, dist = 0.5 * (arr[:-1] + arr[1:]), arr[1:] - arr[:-1]
             qss = orc.ppoly_eval(pp[b], x, mids, 2)
             new = [mids[j] for j in range(len(mids))
                    if dist[j] > max_seg_length or np.max(np.abs(0.5 * qss[j] * dist[j] ** 2)) > max_err_threshold]
-            pts = sorted(pts + new)
-            if not new:
+            if len(pts) + len(new) > max_points:
+                st = -2
                 break
-        while len(pts) < min_nb_points:
+            if not new:
+                converged = True
+                break
+            pts = sorted(pts + new)
+        if st == 0 and (not converged or it == max_iteration - 1):
+            st = 1
+        while st == 0 and len(pts) < min_nb_points:
+            if 2 * len(pts) - 1 > max_points:
+                st = -2
+                break
             arr = np.asarray(pts)
             pts = sorted(pts + list(0.5 * (arr[:-1] + arr[1:])))
-        if it == max_iteration - 1:
-            status[b] = 1
-        n = min(len(pts), max_points)
-        if len(pts) > max_points:
-            status[b] = -2
-        grid[b, :n], grid[b, n:], glen[b] = pts[:n], pts[-1], n
+        n = len(pts)
+        grid[b, :n], grid[b, n:], glen[b], status[b] = pts, pts[-1], n, st
     return torch.from_numpy(grid), torch.from_numpy(glen), torch.from_numpy(status)
 
 

@@ -54,13 +54,15 @@ __global__ void constaccel_eval_kernel(const double *__restrict__ ppoly, const d
     }
     int i = lo - 1;
     if (i == G - 1) i = G - 2;
-    if (i < 0) i = 0;  // t before the start: extrapolate the first stage
+    // t before the start: the reference indexes with -1, i.e. the LAST entry of each array (knot time, speed and
+    // position at the end, the last stage's acceleration: parametrizer.py:115-128)
+    const int it = i < 0 ? G - 1 : i, iu = i < 0 ? G - 2 : i;
     const double *sg = grid + (grid_shared ? 0 : p * G);
-    const double dt = t - tg[i];
-    const double u = us[p * (G - 1) + i];
-    const double v0 = sd[p * G + i];
+    const double dt = t - tg[it];
+    const double u = us[p * (G - 1) + iu];
+    const double v0 = sd[p * G + it];
     const double v = v0 + dt * u;
-    const double s = sg[i] + dt * v0 + 0.5 * (dt * dt) * u;
+    const double s = sg[it] + dt * v0 + 0.5 * (dt * dt) * u;
     const double *x = breaks + (breaks_shared ? 0 : p * (nseg + 1));
     const double *c = ppoly + p * 4 * nseg * dof;
     const int seg = find_interval(x, nseg, s);
