@@ -1,0 +1,61 @@
+/*
+ * toppra_b200_dyn.h — C-ABI of libtoppra_b200_dyn.so: rigid-body inverse dynamics (recursive Newton-Euler) of a
+ * fixed-base kinematic tree on the GPU, the hot path of joint-torque constraints on real robots
+ * (toppra_b200.RigidBodyModel; the reference drives JointTorqueConstraint with pinocchio.rnea for the same purpose).
+ *
+ * Conventions are those of include/toppra_b200.h: device pointers (except model_host), caller-owned memory,
+ * asynchronous on `stream`, 0 / TB_ERR_* / cudaError_t returns, fp64 with -fmad=false.  This library links against
+ * libtoppra_b200.so and reports errors through its tb_last_error().
+ *
+ * Model: a fixed-base tree of nv <= TBD_MAX_BODIES moving bodies, one joint DOF per body, DOF index = body index,
+ * bodies in topological order (parent[k] < k, -1 = the base).  model_host is a HOST array of 3 + 27 nv doubles:
+ *
+ *   [0, 3)            gravity g in the base frame (e.g. 0, 0, -9.81); it enters the recursion as base acceleration -g
+ *   body k at 3 + 27 k:
+ *     +0              parent body index (-1 = base), an integer stored as a double
+ *     +1              joint type: TBD_REVOLUTE or TBD_PRISMATIC
+ *     +2  .. +4       joint axis (unit, joint frame = body frame)
+ *     +5  .. +13      E, row-major 3x3: rotation of the joint frame at q = 0 relative to the parent frame
+ *                     (maps body-frame coordinates to parent-frame coordinates)
+ *     +14 .. +16      r: origin of the joint frame in the parent frame
+ *     +17             mass m
+ *     +18 .. +20      centre of mass c in the body frame
+ *     +21 .. +26      rotational inertia about the centre of mass in the body frame: Ixx, Ixy, Ixz, Iyy, Iyz, Izz
+ *
+ * The body frame at q is the joint frame moved by the joint: rotated by q about the axis (revolute) or translated by
+ * q along it (prismatic).  The model travels to the kernel by value as a __grid_constant__ parameter (no device copy,
+ * no __constant__ symbol shared between streams).
+ */
+#ifndef TOPPRA_B200_DYN_H_
+#define TOPPRA_B200_DYN_H_
+
+#ifdef __cplusplus
+extern "C" {
+#endif
+
+#define TBD_VERSION 100
+#define TBD_MAX_BODIES 16
+#define TBD_BODY_DOUBLES 27
+#define TBD_REVOLUTE 0
+#define TBD_PRISMATIC 1
+
+int tbd_version(void);
+
+/* tau = ID(q, qd, qdd) for M points, one thread per point: Featherstone's spatial RNEA in body coordinates.
+ *   q, qd, qdd, tau [M][nv] row-major. */
+int tbd_rnea(const double *model_host, int nv, int M, const double *q, const double *qd, const double *qdd, double *tau,
+             void *stream);
+
+/* The three inverse-dynamics terms of SecondOrderConstraint (linear_second_order.py) in one launch; the joint transforms
+ * are computed once per point and shared by the three passes:
+ *   c = ID(q, 0, 0);  a = ID(q, 0, qs) - c;  b = ID(q, qs, qss) - c;  c = c + sign(qs) * friction  (friction != NULL)
+ * qs = q', qss = q'' of the path.  Bit-identical to three tbd_rnea launches followed by those element-wise operations.
+ *   q, qs, qss, a, b, c [M][nv]; friction (nullable) [nv]. */
+int tbd_torque_terms(const double *model_host, int nv, int M, const double *q, const double *qs, const double *qss,
+                     const double *friction, double *a, double *b, double *c, void *stream);
+
+#ifdef __cplusplus
+}
+#endif
+
+#endif /* TOPPRA_B200_DYN_H_ */

@@ -7,7 +7,10 @@
 `inv_dyn(q, qd, qdd)` is USER code on 1-D numpy arrays, called 3 x (N+1) times on the host exactly like the
 reference does; the rows F.a, F.b, F.c - g (and the interpolation lift, linear_constraint.py:84-192) are assembled on
 the GPU by the same kernel path as `SecondOrderConstraint.joint_torque_constraint` (csrc/tb_coeff.cu:
-tb_rows_canlinear), which produces the same numbers for the same model."""
+tb_rows_canlinear), which produces the same numbers for the same model.
+
+With a `toppra_b200.RigidBodyModel` as `inv_dyn` the device protocol takes the batched route of that delegate: one
+fused inverse-dynamics launch for the whole batch (libtoppra_b200_dyn.so), so BatchTOPPRA accepts the constraint."""
 import numpy as np
 
 from .constraint import DiscretizationType

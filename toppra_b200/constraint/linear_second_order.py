@@ -10,6 +10,9 @@ The three inverse-dynamics evaluations per gridpoint are USER code.  Two ways to
     assembled on the GPU (csrc/tb_coeff.cu: tb_rows_canlinear);
   * `batched=True`: `inv_dyn(q, qd, qdd)` on CUDA tensors of shape (M, dof) -> (M, m); three calls in total for
     the whole batch x grid, everything stays on the device (general fallback for arbitrary models);
+  * a `toppra_b200.RigidBodyModel` as `inv_dyn` (joint_torque_constraint, JointTorqueConstraint): the batched route
+    with the three terms from ONE fused rigid-body inverse-dynamics launch per batch (libtoppra_b200_dyn.so:
+    tbd_torque_terms), bit-identical to three `model(...)` calls plus the operations below;
   * `device_model=(name, params)` (joint_torque_constraint only): the inverse dynamics is one of the models compiled
     into the library (`engine.DEVICE_MODELS`, include/toppra_b200.h TB_INVDYN_*): ONE kernel evaluates q, q', q'' and
     the three inverse-dynamics terms per gridpoint and writes the torque rows straight into the stage records
@@ -19,6 +22,7 @@ import numpy as np
 from .constraint import DiscretizationType
 from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate
 from .. import engine
+from ..dynamics import RigidBodyModel
 
 
 class SecondOrderConstraint(LinearConstraint):
@@ -52,7 +56,7 @@ class SecondOrderConstraint(LinearConstraint):
         stacked_eyes = np.vstack((np.eye(dof), -np.eye(dof)))
         g_aug = np.concatenate((taulim[..., 1], -taulim[..., 0]), axis=-1)
         device_model = kwargs.pop("device_model", None)
-        batched = kwargs.get("batched", False) or device_model is not None
+        batched = kwargs.get("batched", False) or device_model is not None or isinstance(inv_dyn, RigidBodyModel)
         kwargs["batched"] = batched
         if taulim.ndim == 3 and not batched:
             raise ValueError("batched torque limits need batched=True or a device_model")
@@ -125,6 +129,9 @@ class SecondOrderConstraint(LinearConstraint):
             q = bp.eval_device(ctx.d_grid, 0).reshape(B * G, dof)
             qd = bp.eval_device(ctx.d_grid, 1).reshape(B * G, dof)
             qdd = bp.eval_device(ctx.d_grid, 2).reshape(B * G, dof)
+            if isinstance(self.inv_dyn, RigidBodyModel) and self._eye_form is not None:
+                a, b, c = self.inv_dyn.torque_terms(q, qd, qdd, self._eye_form[1])
+                return (a.reshape(B, G, dof), b.reshape(B, G, dof), c.reshape(B, G, dof))
             zero = torch.zeros_like(q)
             c = self.inv_dyn(q, zero, zero)
             a = self.inv_dyn(q, zero, qd) - c

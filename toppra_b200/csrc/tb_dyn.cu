@@ -1,0 +1,272 @@
+// tb_dyn.cu — libtoppra_b200_dyn.so: inverse dynamics of a fixed-base rigid-body tree (recursive Newton-Euler), the
+// hot path of joint-torque constraints on real robots.  C-ABI and model layout in include/toppra_b200_dyn.h.
+//
+//   rnea_kernel          tau = ID(q, qd, qdd), one thread per point;
+//   torque_terms_kernel  c = ID(q, 0, 0), a = ID(q, 0, q') - c, b = ID(q, q', q'') - c, c += sign(q') friction, one
+//                        thread per point; the joint transforms (and their sincos) are computed once per point.
+//
+// Both kernels run the same two device functions, joint_transforms and rnea_pass, so torque_terms_kernel is bit-identical
+// to three rnea_kernel launches followed by the element-wise operations of SecondOrderConstraint (-fmad=false).
+//
+// Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
+// X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
+//   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
+//             plus the joint's S qd, S qdd and crm(v) S qd;
+//             f_k = I a + v x* I v with I the spatial inertia of mass m, COM c and rotational inertia Ic about c;
+//   backward  tau_k = S^T f_k;  parent: n += R n_k + p x (R f_k),  f += R f_k.
+// The per-body state (12 doubles of motion, 6 of force, 12 of transform) lives in per-thread local arrays indexed by
+// body: the tree is walked with a runtime trip count and runtime parents, so the arrays are not register-promoted.
+// DESIGN.md ("Rigid-body inverse dynamics") lists the registers and stack of both builds.
+//
+// This library is linked against libtoppra_b200.so and uses its error slot (set_error / tb_last_error).  Each library
+// carries its own static CUDA runtime, so launch errors are read here (launch_status).
+#include <cmath>
+#include <cuda_runtime.h>
+
+#include "tb_common.cuh"
+#include "../../include/toppra_b200_dyn.h"
+
+namespace tb {
+namespace {
+
+constexpr int NB = TBD_MAX_BODIES;
+constexpr int THREADS = 128;
+
+// The whole model, passed by value (__grid_constant__): every thread reads the same parameter address (a broadcast).
+struct DynModel {
+  double body[NB][TBD_BODY_DOUBLES];
+  double g[3];
+};
+
+__device__ __forceinline__ void cross3(const double *a, const double *b, double *o) {
+  o[0] = a[1] * b[2] - a[2] * b[1];
+  o[1] = a[2] * b[0] - a[0] * b[2];
+  o[2] = a[0] * b[1] - a[1] * b[0];
+}
+
+// o = R x (R row-major 3x3)
+__device__ __forceinline__ void mul3(const double *R, const double *x, double *o) {
+  o[0] = R[0] * x[0] + R[1] * x[1] + R[2] * x[2];
+  o[1] = R[3] * x[0] + R[4] * x[1] + R[5] * x[2];
+  o[2] = R[6] * x[0] + R[7] * x[1] + R[8] * x[2];
+}
+
+// o = R^T x
+__device__ __forceinline__ void mul3t(const double *R, const double *x, double *o) {
+  o[0] = R[0] * x[0] + R[3] * x[1] + R[6] * x[2];
+  o[1] = R[1] * x[0] + R[4] * x[1] + R[7] * x[2];
+  o[2] = R[2] * x[0] + R[5] * x[1] + R[8] * x[2];
+}
+
+// o = I x with I = (Ixx, Ixy, Ixz, Iyy, Iyz, Izz)
+__device__ __forceinline__ void mul_inertia(const double *I, const double *x, double *o) {
+  o[0] = I[0] * x[0] + I[1] * x[1] + I[2] * x[2];
+  o[1] = I[1] * x[0] + I[3] * x[1] + I[4] * x[2];
+  o[2] = I[2] * x[0] + I[4] * x[1] + I[5] * x[2];
+}
+
+// X[k] = (R row-major [0, 9), p [9, 12)) of every body at configuration q (one point, nv entries).
+__device__ void joint_transforms(const DynModel &m, const int nv, const double *__restrict__ q, double (*X)[12]) {
+  for (int k = 0; k < nv; ++k) {
+    const double *bd = m.body[k];
+    const double *ax = bd + 2, *E = bd + 5, *r = bd + 14;
+    double *R = X[k], *p = X[k] + 9;
+    const double qk = q[k];
+    if (bd[1] == TBD_REVOLUTE) {
+      double s, c;
+      sincos(qk, &s, &c);
+      const double t = 1.0 - c;
+      const double J[9] = {t * ax[0] * ax[0] + c,         t * ax[0] * ax[1] - s * ax[2], t * ax[0] * ax[2] + s * ax[1],
+                           t * ax[0] * ax[1] + s * ax[2], t * ax[1] * ax[1] + c,         t * ax[1] * ax[2] - s * ax[0],
+                           t * ax[0] * ax[2] - s * ax[1], t * ax[1] * ax[2] + s * ax[0], t * ax[2] * ax[2] + c};
+      for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) R[3 * i + j] = E[3 * i] * J[j] + E[3 * i + 1] * J[3 + j] + E[3 * i + 2] * J[6 + j];
+      p[0] = r[0]; p[1] = r[1]; p[2] = r[2];
+    } else {
+      const double d[3] = {ax[0] * qk, ax[1] * qk, ax[2] * qk};
+      double Ed[3];
+      mul3(E, d, Ed);
+      for (int i = 0; i < 9; ++i) R[i] = E[i];
+      p[0] = r[0] + Ed[0]; p[1] = r[1] + Ed[1]; p[2] = r[2] + Ed[2];
+    }
+  }
+}
+
+// tau = ID(q, qd, qdd) on the transforms X of q.  st, f: scratch [nv][12], [nv][6].
+__device__ void rnea_pass(const DynModel &m, const int nv, const double (*X)[12], const double *qd, const double *qdd,
+                          double (*st)[12], double (*f)[6], double *tau) {
+  for (int k = 0; k < nv; ++k) {
+    const double *bd = m.body[k];
+    const int par = (int)bd[0];
+    const double *R = X[k], *p = X[k] + 9, *ax = bd + 2;
+    double wp[3], vp[3], dwp[3], dvp[3];
+    if (par < 0) {
+      for (int i = 0; i < 3; ++i) { wp[i] = 0.0; vp[i] = 0.0; dwp[i] = 0.0; dvp[i] = -m.g[i]; }
+    } else {
+      for (int i = 0; i < 3; ++i) { wp[i] = st[par][i]; vp[i] = st[par][3 + i]; dwp[i] = st[par][6 + i]; dvp[i] = st[par][9 + i]; }
+    }
+    double t[3], w[3], v[3], dw[3], dv[3];
+    cross3(wp, p, t);
+    t[0] = vp[0] + t[0]; t[1] = vp[1] + t[1]; t[2] = vp[2] + t[2];
+    mul3t(R, t, v);
+    mul3t(R, wp, w);
+    mul3t(R, dwp, dw);
+    cross3(dwp, p, t);
+    t[0] = dvp[0] + t[0]; t[1] = dvp[1] + t[1]; t[2] = dvp[2] + t[2];
+    mul3t(R, t, dv);
+    const double sq[3] = {ax[0] * qd[k], ax[1] * qd[k], ax[2] * qd[k]};
+    const double sqq[3] = {ax[0] * qdd[k], ax[1] * qdd[k], ax[2] * qdd[k]};
+    const bool revolute = bd[1] == TBD_REVOLUTE;
+    if (revolute) {
+      for (int i = 0; i < 3; ++i) w[i] = w[i] + sq[i];
+      double c1[3], c2[3];
+      cross3(w, sq, c1);
+      cross3(v, sq, c2);
+      for (int i = 0; i < 3; ++i) { dw[i] = dw[i] + sqq[i] + c1[i]; dv[i] = dv[i] + c2[i]; }
+    } else {
+      for (int i = 0; i < 3; ++i) v[i] = v[i] + sq[i];
+      double c1[3];
+      cross3(w, sq, c1);
+      for (int i = 0; i < 3; ++i) dv[i] = dv[i] + sqq[i] + c1[i];
+    }
+    for (int i = 0; i < 3; ++i) { st[k][i] = w[i]; st[k][3 + i] = v[i]; st[k][6 + i] = dw[i]; st[k][9 + i] = dv[i]; }
+    // f = I a + v x* I v about the body origin
+    const double mass = bd[17], *c = bd + 18, *Ic = bd + 21;
+    double hl[3], ha[3], fl[3], n[3], u[3];
+    cross3(w, c, u);
+    for (int i = 0; i < 3; ++i) hl[i] = mass * (v[i] + u[i]);
+    mul_inertia(Ic, w, ha);
+    cross3(c, hl, u);
+    for (int i = 0; i < 3; ++i) ha[i] = ha[i] + u[i];
+    cross3(dw, c, u);
+    for (int i = 0; i < 3; ++i) fl[i] = mass * (dv[i] + u[i]);
+    mul_inertia(Ic, dw, n);
+    cross3(c, fl, u);
+    for (int i = 0; i < 3; ++i) n[i] = n[i] + u[i];
+    double u2[3];
+    cross3(w, ha, u);
+    cross3(v, hl, u2);
+    for (int i = 0; i < 3; ++i) n[i] = n[i] + u[i] + u2[i];
+    cross3(w, hl, u);
+    for (int i = 0; i < 3; ++i) { fl[i] = fl[i] + u[i]; f[k][i] = n[i]; f[k][3 + i] = fl[i]; }
+  }
+  for (int k = nv - 1; k >= 0; --k) {
+    const double *bd = m.body[k];
+    const double *ax = bd + 2;
+    const double *fk = bd[1] == TBD_REVOLUTE ? f[k] : f[k] + 3;
+    tau[k] = ax[0] * fk[0] + ax[1] * fk[1] + ax[2] * fk[2];
+    const int par = (int)bd[0];
+    if (par >= 0) {
+      const double *R = X[k], *p = X[k] + 9;
+      double Rf[3], Rn[3], u[3];
+      mul3(R, f[k] + 3, Rf);
+      mul3(R, f[k], Rn);
+      cross3(p, Rf, u);
+      for (int i = 0; i < 3; ++i) { f[par][i] = f[par][i] + Rn[i] + u[i]; f[par][3 + i] = f[par][3 + i] + Rf[i]; }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(THREADS)
+rnea_kernel(const __grid_constant__ DynModel m, const int nv, const int M, const double *__restrict__ q,
+            const double *__restrict__ qd, const double *__restrict__ qdd, double *__restrict__ tau) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double X[NB][12], st[NB][12], f[NB][6], t[NB];
+  joint_transforms(m, nv, q + o, X);
+  rnea_pass(m, nv, X, qd + o, qdd + o, st, f, t);
+  for (int k = 0; k < nv; ++k) tau[o + k] = t[k];
+}
+
+__global__ void __launch_bounds__(THREADS)
+torque_terms_kernel(const __grid_constant__ DynModel m, const int nv, const int M, const double *__restrict__ q,
+                    const double *__restrict__ qs, const double *__restrict__ qss, const double *__restrict__ friction,
+                    double *__restrict__ a, double *__restrict__ b, double *__restrict__ c) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double X[NB][12], st[NB][12], f[NB][6], zero[NB], tc[NB], t[NB];
+  for (int k = 0; k < nv; ++k) zero[k] = 0.0;
+  joint_transforms(m, nv, q + o, X);
+  rnea_pass(m, nv, X, zero, zero, st, f, tc);
+  rnea_pass(m, nv, X, zero, qs + o, st, f, t);
+  for (int k = 0; k < nv; ++k) a[o + k] = t[k] - tc[k];
+  rnea_pass(m, nv, X, qs + o, qss + o, st, f, t);
+  for (int k = 0; k < nv; ++k) b[o + k] = t[k] - tc[k];
+  for (int k = 0; k < nv; ++k) {
+    double ck = tc[k];
+    if (friction) {
+      const double x = qs[o + k];
+      const double sgn = (double)((0.0 < x) - (x < 0.0));   // torch.sign: 0 at +-0 and NaN
+      ck = ck + sgn * friction[k];
+    }
+    c[o + k] = ck;
+  }
+}
+
+int launch_status(const char *what) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("%s: launch failed: %s", what, cudaGetErrorString(e));
+    return (int)e;
+  }
+  return 0;
+}
+
+// Validates the packed model and copies it into the by-value launch parameter: 0, or the TB_ERR_* code (message set).
+int load_model(const double *host, const int nv, const int M, DynModel *m, const char *what) {
+  if (M <= 0) { set_error("%s: M=%d must be positive", what, M); return TB_ERR_ARG; }
+  if (nv < 1 || nv > NB) { set_error("%s: nv=%d outside 1..%d", what, nv, NB); return TB_ERR_UNSUPPORTED; }
+  for (int i = 0; i < 3; ++i) m->g[i] = host[i];
+  for (int k = 0; k < NB; ++k)
+    for (int j = 0; j < TBD_BODY_DOUBLES; ++j) m->body[k][j] = k < nv ? host[3 + TBD_BODY_DOUBLES * k + j] : 0.0;
+  for (int k = 0; k < nv; ++k) {
+    const double *bd = m->body[k];
+    if (!(bd[0] >= -1.0 && bd[0] < (double)k && bd[0] == std::floor(bd[0]))) {
+      set_error("%s: body %d: parent %g must be an integer in [-1, %d)", what, k, bd[0], k);
+      return TB_ERR_ARG;
+    }
+    if (bd[1] != TBD_REVOLUTE && bd[1] != TBD_PRISMATIC) {
+      set_error("%s: body %d: unknown joint type %g", what, k, bd[1]);
+      return TB_ERR_ARG;
+    }
+    if (!std::isfinite(bd[17]) || bd[17] < 0.0) {
+      set_error("%s: body %d: mass %g must be finite and non-negative", what, k, bd[17]);
+      return TB_ERR_ARG;
+    }
+    if (bd[2] == 0.0 && bd[3] == 0.0 && bd[4] == 0.0) {
+      set_error("%s: body %d: zero joint axis", what, k);
+      return TB_ERR_ARG;
+    }
+  }
+  return 0;
+}
+
+unsigned blocks(const int M) { return (unsigned)((M + THREADS - 1) / THREADS); }
+
+}  // namespace
+}  // namespace tb
+
+extern "C" int tbd_version(void) { return TBD_VERSION; }
+
+extern "C" int tbd_rnea(const double *model_host, int nv, int M, const double *q, const double *qd, const double *qdd,
+                        double *tau, void *stream) {
+  using namespace tb;
+  if (!model_host || !q || !qd || !qdd || !tau) { set_error("tbd_rnea: null pointer"); return TB_ERR_ARG; }
+  DynModel m;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_rnea")) return rc;
+  rnea_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, nv, M, q, qd, qdd, tau);
+  return launch_status("tbd_rnea");
+}
+
+extern "C" int tbd_torque_terms(const double *model_host, int nv, int M, const double *q, const double *qs,
+                                const double *qss, const double *friction, double *a, double *b, double *c,
+                                void *stream) {
+  using namespace tb;
+  if (!model_host || !q || !qs || !qss || !a || !b || !c) { set_error("tbd_torque_terms: null pointer"); return TB_ERR_ARG; }
+  DynModel m;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_torque_terms")) return rc;
+  torque_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, nv, M, q, qs, qss, friction, a, b, c);
+  return launch_status("tbd_torque_terms");
+}

@@ -1,0 +1,253 @@
+"""Rigid-body models of fixed-base robots for joint-torque constraints: `RigidBodyModel` (per-body arrays or a URDF file)
+whose inverse dynamics run on the GPU (libtoppra_b200_dyn.so, Featherstone's recursive Newton-Euler algorithm).
+
+    model = RigidBodyModel.from_urdf("arm.urdf")
+    tau = model(q, qd, qdd)                                  # CUDA tensors (M, nv): one kernel launch
+    pc = JointTorqueConstraint(model, model.torque_limits(), friction)
+
+A `RigidBodyModel` is a valid `inv_dyn` for `JointTorqueConstraint` and `SecondOrderConstraint.joint_torque_constraint`;
+there it takes the device route: the three inverse-dynamics terms of every gridpoint of the batch come from ONE fused
+launch (`torque_terms`).  The packed layout the library takes is documented in include/toppra_b200_dyn.h."""
+import ctypes
+import xml.etree.ElementTree as ET
+
+import numpy as np
+
+from . import _lib, _lib_dyn
+
+MAX_BODIES = 16
+BODY_DOUBLES = 27
+REVOLUTE, PRISMATIC = 0, 1
+_JOINT_TYPES = {"revolute": REVOLUTE, "continuous": REVOLUTE, "prismatic": PRISMATIC}
+
+
+def rpy_matrix(rpy):
+    """URDF `origin rpy`: fixed-axis roll-pitch-yaw, R = Rz(y) Ry(p) Rx(r)."""
+    r, p, y = rpy
+    cr, sr, cp, sp, cy, sy = np.cos(r), np.sin(r), np.cos(p), np.sin(p), np.cos(y), np.sin(y)
+    Rx = np.array([[1, 0, 0], [0, cr, -sr], [0, sr, cr]])
+    Ry = np.array([[cp, 0, sp], [0, 1, 0], [-sp, 0, cp]])
+    Rz = np.array([[cy, -sy, 0], [sy, cy, 0], [0, 0, 1]])
+    return Rz @ Ry @ Rx
+
+
+def axis_rotation(axis, angle):
+    """Rotation by `angle` about the unit vector `axis` (Rodrigues)."""
+    a = np.asarray(axis, dtype=np.float64)
+    K = np.array([[0, -a[2], a[1]], [a[2], 0, -a[0]], [-a[1], a[0], 0]])
+    return np.eye(3) + np.sin(angle) * K + (1 - np.cos(angle)) * (K @ K)
+
+
+class RigidBodyModel(object):
+    """Fixed-base kinematic tree of nv <= 16 moving bodies, one joint DOF each (DOF index = body index), bodies in
+    topological order (parent[k] < k, -1 = base).
+
+    parent (nv,); joint_type (nv,) of "revolute" / "prismatic" (or 0 / 1); axis (nv, 3) in the joint frame;
+    E (nv, 3, 3), r (nv, 3): placement of the joint frame in the parent frame at q = 0 (E maps body to parent
+    coordinates); mass (nv,); com (nv, 3) in the body frame; inertia (nv, 6) = Ixx, Ixy, Ixz, Iyy, Iyz, Izz about the
+    centre of mass in the body frame; gravity (3,) in the base frame."""
+
+    def __init__(self, parent, joint_type, axis, E, r, mass, com, inertia, gravity=(0.0, 0.0, -9.81), joint_names=None,
+                 effort_limit=None, velocity_limit=None):
+        parent = np.asarray(parent, dtype=np.float64).reshape(-1)
+        nv = parent.shape[0]
+        if not 1 <= nv <= MAX_BODIES:
+            raise ValueError("RigidBodyModel: %d moving bodies, supported 1..%d" % (nv, MAX_BODIES))
+        jt = np.array([_JOINT_TYPES.get(t, t) if isinstance(t, str) else t for t in np.atleast_1d(joint_type)],
+                      dtype=np.float64)
+        axis = np.asarray(axis, dtype=np.float64).reshape(nv, 3)
+        norm = np.linalg.norm(axis, axis=1, keepdims=True)
+        axis = np.where(norm > 0, axis / np.where(norm > 0, norm, 1.0), axis)   # a zero axis is rejected by the library
+        packed = np.zeros(3 + BODY_DOUBLES * nv)
+        packed[:3] = np.asarray(gravity, dtype=np.float64).reshape(3)
+        body = packed[3:].reshape(nv, BODY_DOUBLES)
+        body[:, 0] = parent
+        body[:, 1] = jt.reshape(nv)
+        body[:, 2:5] = axis
+        body[:, 5:14] = np.asarray(E, dtype=np.float64).reshape(nv, 9)
+        body[:, 14:17] = np.asarray(r, dtype=np.float64).reshape(nv, 3)
+        body[:, 17] = np.asarray(mass, dtype=np.float64).reshape(nv)
+        body[:, 18:21] = np.asarray(com, dtype=np.float64).reshape(nv, 3)
+        body[:, 21:27] = np.asarray(inertia, dtype=np.float64).reshape(nv, 6)
+        self.packed = packed
+        self.nv = nv
+        self.joint_names = list(joint_names) if joint_names is not None else ["joint%d" % k for k in range(nv)]
+        inf = np.full(nv, np.inf)
+        self.effort_limit = inf.copy() if effort_limit is None else np.asarray(effort_limit, dtype=np.float64)
+        self.velocity_limit = inf.copy() if velocity_limit is None else np.asarray(velocity_limit, dtype=np.float64)
+
+    @property
+    def dof(self):
+        return self.nv
+
+    @property
+    def gravity(self):
+        return self.packed[:3].copy()
+
+    def body(self, k):
+        """The 27 packed doubles of body k (include/toppra_b200_dyn.h)."""
+        return self.packed[3 + BODY_DOUBLES * k:3 + BODY_DOUBLES * (k + 1)].copy()
+
+    def torque_limits(self):
+        """(nv, 2) [-effort, effort] per joint, the tau_lim of JointTorqueConstraint (+-inf where the URDF has none)."""
+        return np.stack([-self.effort_limit, self.effort_limit], axis=1)
+
+    # ---- evaluation on the GPU ----------------------------------------------------------------------------------
+    def _model_ptr(self):
+        return ctypes.c_void_p(self.packed.ctypes.data)
+
+    def _prepare(self, torch, *xs):
+        out = []
+        for x in xs:
+            if x.dim() != 2 or x.shape[1] != self.nv:
+                raise ValueError("RigidBodyModel: expected (M, %d) tensors, got %s" % (self.nv, tuple(x.shape)))
+            out.append(x.to(dtype=torch.float64).contiguous())
+        if any(x.shape != out[0].shape or x.device != out[0].device for x in out):
+            raise ValueError("RigidBodyModel: q, qd, qdd must share shape and device")
+        return out
+
+    def __call__(self, q, qd, qdd):
+        """Joint torques tau = M(q) qdd + h(q, qd) + g(q).  CUDA tensors (M, nv) -> (M, nv), one tbd_rnea launch on the
+        current stream; numpy (nv,) or (M, nv) -> numpy, through a device round trip."""
+        torch = _lib.require_cuda()
+        if isinstance(q, torch.Tensor) and q.is_cuda:
+            q, qd, qdd = self._prepare(torch, q, qd, qdd)
+            tau = torch.empty_like(q)
+            with torch.cuda.device(q.device):
+                _lib.check(_lib_dyn.load().tbd_rnea(self._model_ptr(), self.nv, q.shape[0], _lib.ptr(q), _lib.ptr(qd),
+                                                    _lib.ptr(qdd), _lib.ptr(tau), _lib.stream_ptr()), "tbd_rnea")
+            return tau
+        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd, qdd)]
+        single = arrs[0].ndim == 1
+        dev = [torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]
+        tau = self(*dev).cpu().numpy()
+        return tau[0] if single else tau
+
+    def torque_terms(self, q, qs, qss, friction=None):
+        """The terms of SecondOrderConstraint for CUDA tensors (M, nv), one tbd_torque_terms launch:
+        c = ID(q, 0, 0), a = ID(q, 0, qs) - c, b = ID(q, qs, qss) - c, c += sign(qs) * friction (friction (nv,) or
+        None).  Returns (a, b, c)."""
+        torch = _lib.require_cuda()
+        q, qs, qss = self._prepare(torch, q, qs, qss)
+        a, b, c = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
+        fric = None
+        if friction is not None and np.any(np.asarray(friction) != 0):
+            fric = torch.as_tensor(np.broadcast_to(np.asarray(friction, dtype=np.float64), (self.nv,)).copy(), device=q.device)
+        with torch.cuda.device(q.device):
+            _lib.check(_lib_dyn.load().tbd_torque_terms(self._model_ptr(), self.nv, q.shape[0], _lib.ptr(q), _lib.ptr(qs),
+                                                        _lib.ptr(qss), _lib.ptr(fric), _lib.ptr(a), _lib.ptr(b),
+                                                        _lib.ptr(c), _lib.stream_ptr()), "tbd_torque_terms")
+        return a, b, c
+
+    # ---- URDF ---------------------------------------------------------------------------------------------------
+    @classmethod
+    def from_urdf(cls, urdf, locked_joints=None, gravity=(0.0, 0.0, -9.81)):
+        """Build the model from a URDF file name or XML string (xml.etree only).
+
+        revolute / continuous joints become revolute bodies, prismatic ones prismatic; fixed joints and the joints named
+        in `locked_joints` (name -> position) fold their child link into the parent body (mass, centre of mass, inertia
+        by the parallel-axis theorem).  DOF order is depth-first with children in file order; `joint_names` lists it.
+        floating, planar and unlocked mimic joints, a missing or ambiguous root and more than 16 moving bodies raise
+        ValueError."""
+        text = urdf if urdf.lstrip().startswith("<") else open(urdf).read()
+        robot = ET.fromstring(text)
+        locked = dict(locked_joints or {})
+        links = {}
+        for el in robot.findall("link"):
+            links[el.get("name")] = el
+        joints, parent_of, children = [], {}, {name: [] for name in links}
+        for el in robot.findall("joint"):
+            name, jtype = el.get("name"), el.get("type")
+            par, chi = el.find("parent").get("link"), el.find("child").get("link")
+            if par not in links or chi not in links:
+                raise ValueError("URDF joint %r connects unknown links %r -> %r" % (name, par, chi))
+            if chi in parent_of:
+                raise ValueError("URDF link %r has two parent joints" % chi)
+            if jtype in ("floating", "planar"):
+                raise ValueError("URDF joint %r: %s joints are not supported (fixed base, one DOF per joint)"
+                                 % (name, jtype))
+            if jtype not in _JOINT_TYPES and jtype != "fixed":
+                raise ValueError("URDF joint %r: unknown type %r" % (name, jtype))
+            if el.find("mimic") is not None and name not in locked:
+                raise ValueError("URDF joint %r mimics another joint; lock it (locked_joints)" % name)
+            parent_of[chi] = name
+            joints.append(el)
+            children[par].append(el)
+        unknown = set(locked) - {j.get("name") for j in joints}
+        if unknown:
+            raise ValueError("locked_joints names unknown joints: %s" % sorted(unknown))
+        roots = [name for name in links if name not in parent_of]
+        if len(roots) != 1:
+            raise ValueError("URDF needs exactly one root link, found %s" % (roots or "none"))
+
+        bodies = []          # dicts of one moving body each, in DOF order
+        parts = {-1: []}     # body index -> [(mass, com, inertia about com)] in the body frame
+
+        def origin(el):
+            o = el.find("origin") if el is not None else None
+            xyz = np.array(o.get("xyz", "0 0 0").split(), dtype=np.float64) if o is not None else np.zeros(3)
+            rpy = np.array(o.get("rpy", "0 0 0").split(), dtype=np.float64) if o is not None else np.zeros(3)
+            return rpy_matrix(rpy), xyz
+
+        def add_inertial(body, link, R, p):
+            inert = links[link].find("inertial")
+            if inert is None:
+                return
+            Ri, pi = origin(inert)
+            m = float(inert.find("mass").get("value")) if inert.find("mass") is not None else 0.0
+            el = inert.find("inertia")
+            v = {k: float(el.get(k, 0.0)) if el is not None else 0.0
+                 for k in ("ixx", "ixy", "ixz", "iyy", "iyz", "izz")}
+            I = np.array([[v["ixx"], v["ixy"], v["ixz"]], [v["ixy"], v["iyy"], v["iyz"]], [v["ixz"], v["iyz"], v["izz"]]])
+            Rb = R @ Ri
+            parts[body].append((m, R @ pi + p, Rb @ I @ Rb.T))
+
+        def visit(link, body, R, p):
+            add_inertial(body, link, R, p)
+            for el in children[link]:
+                name, jtype = el.get("name"), el.get("type")
+                Ro, po = origin(el)
+                Rj, pj = R @ Ro, R @ po + p
+                ax_el = el.find("axis")
+                axis = np.array(ax_el.get("xyz").split(), dtype=np.float64) if ax_el is not None else np.array([1.0, 0.0, 0.0])
+                if np.linalg.norm(axis) == 0 and jtype != "fixed":
+                    raise ValueError("URDF joint %r has a zero axis" % name)
+                axis = axis / np.linalg.norm(axis) if jtype != "fixed" else axis
+                child = el.find("child").get("link")
+                if jtype == "fixed" or name in locked:
+                    if jtype != "fixed":
+                        pos = float(locked[name])
+                        if _JOINT_TYPES[jtype] == REVOLUTE:
+                            Rj = Rj @ axis_rotation(axis, pos)
+                        else:
+                            pj = pj + Rj @ (axis * pos)
+                    visit(child, body, Rj, pj)
+                    continue
+                if len(bodies) == MAX_BODIES:
+                    raise ValueError("URDF has more than %d moving joints" % MAX_BODIES)
+                lim = el.find("limit")
+                bodies.append(dict(parent=body, type=_JOINT_TYPES[jtype], axis=axis, E=Rj, r=pj, name=name,
+                                   effort=float(lim.get("effort", np.inf)) if lim is not None else np.inf,
+                                   velocity=float(lim.get("velocity", np.inf)) if lim is not None else np.inf))
+                k = len(bodies) - 1
+                parts[k] = []
+                visit(child, k, np.eye(3), np.zeros(3))
+
+        visit(roots[0], -1, np.eye(3), np.zeros(3))
+        if not bodies:
+            raise ValueError("URDF has no moving joint")
+        mass, com, inertia = [], [], []
+        for k in range(len(bodies)):
+            m = sum(pm for pm, _, _ in parts[k])
+            c = sum(pm * pc for pm, pc, _ in parts[k]) / m if m > 0 else np.zeros(3)
+            Ic = np.zeros((3, 3))
+            for pm, pc, pI in parts[k]:
+                d = pc - c
+                Ic = Ic + pI + pm * (np.dot(d, d) * np.eye(3) - np.outer(d, d))
+            mass.append(m)
+            com.append(c)
+            inertia.append([Ic[0, 0], Ic[0, 1], Ic[0, 2], Ic[1, 1], Ic[1, 2], Ic[2, 2]])
+        return cls([b["parent"] for b in bodies], [b["type"] for b in bodies], [b["axis"] for b in bodies],
+                   [b["E"] for b in bodies], [b["r"] for b in bodies], mass, com, inertia, gravity,
+                   joint_names=[b["name"] for b in bodies], effort_limit=[b["effort"] for b in bodies],
+                   velocity_limit=[b["velocity"] for b in bodies])
