@@ -25,6 +25,21 @@
  * The body frame at q is the joint frame moved by the joint: rotated by q about the axis (revolute) or translated by
  * q along it (prismatic).  The model travels to the kernel by value as a __grid_constant__ parameter (no device copy,
  * no __constant__ symbol shared between streams).
+ *
+ * Frame: a frame rigidly attached to one body (toppra_b200.RigidBodyFrame).  frame_host is a HOST array of
+ * TBD_FRAME_DOUBLES doubles:
+ *
+ *   +0              body index (-1 = the base), an integer stored as a double
+ *   +1  .. +9       R, row-major 3x3: orientation of the frame in the body frame (maps frame to body coordinates)
+ *   +10 .. +12      p: origin of the frame in the body frame
+ *   +13             reference frame of the velocity: TBD_WORLD, TBD_LOCAL or TBD_LOCAL_WORLD_ALIGNED
+ *
+ * A frame velocity is [linear(3); angular(3)] (pinocchio's Motion::toVector()).  With p_f, R_f the frame's world
+ * placement, dp_f the velocity of its origin and w the angular velocity in world coordinates:
+ *   TBD_LOCAL_WORLD_ALIGNED   (dp_f, w)
+ *   TBD_LOCAL                 (R_f^T dp_f, R_f^T w)
+ *   TBD_WORLD                 (dp_f - w x p_f, w): the spatial velocity at the world origin
+ * The reference-frame codes are pinocchio's ReferenceFrame values.
  */
 #ifndef TOPPRA_B200_DYN_H_
 #define TOPPRA_B200_DYN_H_
@@ -38,6 +53,10 @@ extern "C" {
 #define TBD_BODY_DOUBLES 27
 #define TBD_REVOLUTE 0
 #define TBD_PRISMATIC 1
+#define TBD_FRAME_DOUBLES 14
+#define TBD_WORLD 0
+#define TBD_LOCAL 1
+#define TBD_LOCAL_WORLD_ALIGNED 2
 
 int tbd_version(void);
 
@@ -53,6 +72,18 @@ int tbd_rnea(const double *model_host, int nv, int M, const double *q, const dou
  *   q, qs, qss, a, b, c [M][nv]; friction (nullable) [nv]. */
 int tbd_torque_terms(const double *model_host, int nv, int M, const double *q, const double *qs, const double *qss,
                      const double *friction, double *a, double *b, double *c, void *stream);
+
+/* v = the velocity of the frame frame_host at (q, qd) for M points, one thread per point.
+ *   q, qd [M][nv]; v [M][6].  TB_ERR_ARG for a frame body outside [-1, nv) or not an integer, an unknown reference
+ *   frame or a non-finite R or p. */
+int tbd_frame_velocity(const double *model_host, int nv, const double *frame_host, int M, const double *q,
+                       const double *qd, double *v, void *stream);
+
+/* The row of CartesianVelocityNorm: b = v^T (S v) with v the velocity of frame_host at (q, qs = q'), S v row by row,
+ * then v . (S v), each sum left to right.  Bit-identical to tbd_frame_velocity followed by that quadratic form.
+ *   S_host: HOST array of 36 doubles (6x6 row-major, finite); q, qs [M][nv]; b [M]. */
+int tbd_velocity_norm_terms(const double *model_host, int nv, const double *frame_host, const double *S_host, int M,
+                            const double *q, const double *qs, double *b, void *stream);
 
 #ifdef __cplusplus
 }

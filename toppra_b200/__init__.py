@@ -17,7 +17,7 @@ from . import constraint
 from . import solverwrapper
 from . import algorithm
 from .batch import BatchResult, BatchTOPPRA, BatchTOPPRAsd, solve_batch
-from .dynamics import RigidBodyModel
+from .dynamics import RigidBodyFrame, RigidBodyModel
 from .utils import setup_logging
 
 __version__ = "0.1.0"
@@ -26,4 +26,4 @@ logging.getLogger("toppra_b200").addHandler(logging.NullHandler())
 
 __all__ = ["AbstractGeometricPath", "BatchSplineInterpolator", "BatchPiecewisePolyPath", "PiecewisePolyPath", "PPolyPath", "PolynomialPath", "SimplePath", "SplineInterpolator", "UnivariateSplineInterpolator", "propose_gridpoints",
            "ParametrizeConstAccel", "ParametrizeSpline", "BatchParametrizeConstAccel", "BatchParametrizeSpline", "constraint", "solverwrapper", "algorithm", "BatchResult",
-           "BatchTOPPRA", "BatchTOPPRAsd", "solve_batch", "RigidBodyModel", "constants", "exceptions", "setup_logging"]
+           "BatchTOPPRA", "BatchTOPPRAsd", "solve_batch", "RigidBodyFrame", "RigidBodyModel", "constants", "exceptions", "setup_logging"]

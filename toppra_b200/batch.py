@@ -388,7 +388,7 @@ class BatchTOPPRA(object):
             hi = min(self.B, lo + nchunk)
             grid = self.d_grid if self.d_grid.dim() == 1 else self.d_grid[lo:hi]
             glen = None if self.glen is None else self.glen[lo:hi].contiguous()   # ragged grids: the chunk's lengths
-            ctx = RecordContext(self.path.chunk(lo, hi), grid, self._grid_host, None, lo, hi)
+            ctx = RecordContext(self.path.chunk(lo, hi), grid, self._grid_host, None, lo, hi, self.B)
             if buf is None:
                 buf, self.R = build_records(ctx, self.constraints)
                 rec = buf

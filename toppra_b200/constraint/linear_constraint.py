@@ -80,7 +80,7 @@ class LinearConstraint(Constraint):
 class RecordContext(object):
     """What a constraint needs to write its rows: the (batched) device path, the gridpoints on device and host."""
 
-    def __init__(self, bpath, d_grid, grid_host, path=None, lo=0, hi=None):
+    def __init__(self, bpath, d_grid, grid_host, path=None, lo=0, hi=None, total=None):
         self.bpath = bpath          # BatchSplineInterpolator (or a chunk view of one)
         self.d_grid = d_grid        # CUDA tensor [G] (shared) or [B, G]
         self.grid_host = grid_host  # numpy [G] (shared grids only) or None
@@ -90,6 +90,7 @@ class RecordContext(object):
         self.device = bpath.device
         self.lo = lo                # this context covers paths [lo, hi) of the full batch (chunked solves)
         self.hi = self.B if hi is None else hi
+        self.total = self.hi if total is None else total   # paths of the full batch (per-path limit arrays)
 
     def limits(self, t):
         """Per-path limit tensors [Bfull, dof, 2] are sliced to this chunk; shared ones pass through."""

@@ -8,6 +8,11 @@
 // Both kernels run the same two device functions, joint_transforms and rnea_pass, so torque_terms_kernel is bit-identical
 // to three rnea_kernel launches followed by the element-wise operations of SecondOrderConstraint (-fmad=false).
 //
+//   frame_velocity_kernel       v = the 6-D velocity of a frame at (q, qd), one thread per point;
+//   velocity_norm_terms_kernel  b = v^T S v at (q, q'), the row of CartesianVelocityNorm, one thread per point.
+// Both run frame_velocity, which walks only the frame's root-to-body chain with its state in registers (no local
+// arrays); the per-body placement is TB_BODY_TRANSFORM, shared with joint_transforms.
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -65,30 +70,39 @@ __device__ __forceinline__ void mul_inertia(const double *I, const double *x, do
   o[2] = I[2] * x[0] + I[4] * x[1] + I[5] * x[2];
 }
 
+// Placement (R row-major, p) of body bd in its parent frame at joint position qk: the joint frame (E, r) rotated by qk
+// about the axis (sincos, Rodrigues) or translated by qk along it.  Shared by joint_transforms and frame_velocity.  A
+// macro, not a function: as a separate function it changes the instruction schedule nvcc gives joint_transforms, and
+// rnea_kernel and torque_terms_kernel keep their machine code byte for byte this way.
+#define TB_BODY_TRANSFORM(bd, qk, R, p)                                                                                  \
+  do {                                                                                                                 \
+    const double *ax = (bd) + 2, *E = (bd) + 5, *r = (bd) + 14;                                                        \
+    if ((bd)[1] == TBD_REVOLUTE) {                                                                                     \
+      double s, c;                                                                                                     \
+      sincos((qk), &s, &c);                                                                                            \
+      const double t = 1.0 - c;                                                                                        \
+      const double J[9] = {t * ax[0] * ax[0] + c,         t * ax[0] * ax[1] - s * ax[2], t * ax[0] * ax[2] + s * ax[1], \
+                           t * ax[0] * ax[1] + s * ax[2], t * ax[1] * ax[1] + c,         t * ax[1] * ax[2] - s * ax[0], \
+                           t * ax[0] * ax[2] - s * ax[1], t * ax[1] * ax[2] + s * ax[0], t * ax[2] * ax[2] + c};        \
+      for (int i = 0; i < 3; ++i)                                                                                      \
+        for (int j = 0; j < 3; ++j) (R)[3 * i + j] = E[3 * i] * J[j] + E[3 * i + 1] * J[3 + j] + E[3 * i + 2] * J[6 + j]; \
+      (p)[0] = r[0]; (p)[1] = r[1]; (p)[2] = r[2];                                                                     \
+    } else {                                                                                                           \
+      const double d[3] = {ax[0] * (qk), ax[1] * (qk), ax[2] * (qk)};                                                  \
+      double Ed[3];                                                                                                    \
+      mul3(E, d, Ed);                                                                                                  \
+      for (int i = 0; i < 9; ++i) (R)[i] = E[i];                                                                       \
+      (p)[0] = r[0] + Ed[0]; (p)[1] = r[1] + Ed[1]; (p)[2] = r[2] + Ed[2];                                             \
+    }                                                                                                                  \
+  } while (0)
+
 // X[k] = (R row-major [0, 9), p [9, 12)) of every body at configuration q (one point, nv entries).
 __device__ void joint_transforms(const DynModel &m, const int nv, const double *__restrict__ q, double (*X)[12]) {
   for (int k = 0; k < nv; ++k) {
     const double *bd = m.body[k];
-    const double *ax = bd + 2, *E = bd + 5, *r = bd + 14;
     double *R = X[k], *p = X[k] + 9;
     const double qk = q[k];
-    if (bd[1] == TBD_REVOLUTE) {
-      double s, c;
-      sincos(qk, &s, &c);
-      const double t = 1.0 - c;
-      const double J[9] = {t * ax[0] * ax[0] + c,         t * ax[0] * ax[1] - s * ax[2], t * ax[0] * ax[2] + s * ax[1],
-                           t * ax[0] * ax[1] + s * ax[2], t * ax[1] * ax[1] + c,         t * ax[1] * ax[2] - s * ax[0],
-                           t * ax[0] * ax[2] - s * ax[1], t * ax[1] * ax[2] + s * ax[0], t * ax[2] * ax[2] + c};
-      for (int i = 0; i < 3; ++i)
-        for (int j = 0; j < 3; ++j) R[3 * i + j] = E[3 * i] * J[j] + E[3 * i + 1] * J[3 + j] + E[3 * i + 2] * J[6 + j];
-      p[0] = r[0]; p[1] = r[1]; p[2] = r[2];
-    } else {
-      const double d[3] = {ax[0] * qk, ax[1] * qk, ax[2] * qk};
-      double Ed[3];
-      mul3(E, d, Ed);
-      for (int i = 0; i < 9; ++i) R[i] = E[i];
-      p[0] = r[0] + Ed[0]; p[1] = r[1] + Ed[1]; p[2] = r[2] + Ed[2];
-    }
+    TB_BODY_TRANSFORM(bd, qk, R, p);
   }
 }
 
@@ -205,6 +219,93 @@ torque_terms_kernel(const __grid_constant__ DynModel m, const int nv, const int 
   }
 }
 
+// A frame rigidly attached to one body, passed by value next to the model: its placement (R, p) in the body frame, the
+// bodies from the root to that body (chain[0, n); n = 0 for a frame on the base), the reference frame of the result and,
+// for tbd_velocity_norm_terms, the 6x6 weight S.
+struct DynFrame {
+  double R[9], p[3], S[36];
+  int chain[NB];
+  int n, ref;
+};
+
+// v = [linear(3); angular(3)] velocity of frame f at (q, qd), in f's reference frame.  Walks f's chain from the root
+// with the world placement (Rw, pw), the angular velocity w and the body-origin velocity vo in registers; the only
+// runtime indices are the model's body indices of the chain, never a function of q.
+__device__ __forceinline__ void frame_velocity(const DynModel &m, const DynFrame &f, const double *__restrict__ q,
+                                               const double *__restrict__ qd, double *v) {
+  double Rw[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0}, pw[3] = {0.0, 0.0, 0.0};
+  double w[3] = {0.0, 0.0, 0.0}, vo[3] = {0.0, 0.0, 0.0};
+  for (int i = 0; i < f.n; ++i) {
+    const int k = f.chain[i];
+    const double *bd = m.body[k];
+    double R[9], p[3], d[3], t[3], Rn[9];
+    const double qk = q[k];
+    TB_BODY_TRANSFORM(bd, qk, R, p);
+    mul3(Rw, p, d);                     // origin of body k relative to its parent's, world coordinates
+    cross3(w, d, t);
+    for (int j = 0; j < 3; ++j) { pw[j] = pw[j] + d[j]; vo[j] = vo[j] + t[j]; }
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) Rn[3 * r + c] = Rw[3 * r] * R[c] + Rw[3 * r + 1] * R[3 + c] + Rw[3 * r + 2] * R[6 + c];
+    for (int j = 0; j < 9; ++j) Rw[j] = Rn[j];
+    double s[3];
+    mul3(Rw, bd + 2, s);                // joint axis, world coordinates
+    const double qdk = qd[k];
+    if (bd[1] == TBD_REVOLUTE) {
+      for (int j = 0; j < 3; ++j) w[j] = w[j] + s[j] * qdk;
+    } else {
+      for (int j = 0; j < 3; ++j) vo[j] = vo[j] + s[j] * qdk;
+    }
+  }
+  double d[3], t[3], pd[3];
+  mul3(Rw, f.p, d);                     // frame origin relative to the body origin, world coordinates
+  cross3(w, d, t);
+  for (int j = 0; j < 3; ++j) pd[j] = vo[j] + t[j];
+  if (f.ref == TBD_LOCAL) {
+    double Rf[9];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) Rf[3 * r + c] = Rw[3 * r] * f.R[c] + Rw[3 * r + 1] * f.R[3 + c] + Rw[3 * r + 2] * f.R[6 + c];
+    mul3t(Rf, pd, v);
+    mul3t(Rf, w, v + 3);
+  } else if (f.ref == TBD_WORLD) {
+    double pf[3];
+    for (int j = 0; j < 3; ++j) pf[j] = pw[j] + d[j];
+    cross3(w, pf, t);
+    for (int j = 0; j < 3; ++j) { v[j] = pd[j] - t[j]; v[3 + j] = w[j]; }
+  } else {                              // TBD_LOCAL_WORLD_ALIGNED
+    for (int j = 0; j < 3; ++j) { v[j] = pd[j]; v[3 + j] = w[j]; }
+  }
+}
+
+__global__ void __launch_bounds__(THREADS)
+frame_velocity_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame f, const int nv, const int M,
+                      const double *__restrict__ q, const double *__restrict__ qd, double *__restrict__ v) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double x[6];
+  frame_velocity(m, f, q + o, qd + o, x);
+  for (int j = 0; j < 6; ++j) v[(size_t)pt * 6 + j] = x[j];
+}
+
+// b = v^T (S v) at (q, q'): S v row by row, then v . (S v), each sum left to right (cartesian_velocity_norm.cpp).
+__global__ void __launch_bounds__(THREADS)
+velocity_norm_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame f, const int nv,
+                           const int M, const double *__restrict__ q, const double *__restrict__ qs,
+                           double *__restrict__ b) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double x[6];
+  frame_velocity(m, f, q + o, qs + o, x);
+  double acc = 0.0;
+  for (int i = 0; i < 6; ++i) {
+    double sv = f.S[6 * i] * x[0];
+    for (int j = 1; j < 6; ++j) sv = sv + f.S[6 * i + j] * x[j];
+    acc = i == 0 ? x[0] * sv : acc + x[i] * sv;
+  }
+  b[pt] = acc;
+}
+
 int launch_status(const char *what) {
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -243,6 +344,36 @@ int load_model(const double *host, const int nv, const int M, DynModel *m, const
   return 0;
 }
 
+// Validates the packed frame (include/toppra_b200_dyn.h) of a model already loaded by load_model and copies it, the
+// root-to-body chain and S (nullable) into the by-value launch parameter: 0, or the TB_ERR_* code (message set).
+int load_frame(const double *host, const DynModel &m, const int nv, const double *S, DynFrame *f, const char *what) {
+  const double body = host[0];
+  if (!(body >= -1.0 && body < (double)nv && body == std::floor(body))) {
+    set_error("%s: frame body %g must be an integer in [-1, %d)", what, body, nv);
+    return TB_ERR_ARG;
+  }
+  const double ref = host[13];
+  if (ref != TBD_WORLD && ref != TBD_LOCAL && ref != TBD_LOCAL_WORLD_ALIGNED) {
+    set_error("%s: unknown reference frame %g", what, ref);
+    return TB_ERR_ARG;
+  }
+  for (int j = 0; j < 12; ++j)
+    if (!std::isfinite(host[1 + j])) { set_error("%s: frame placement is not finite", what); return TB_ERR_ARG; }
+  for (int j = 0; j < 9; ++j) f->R[j] = host[1 + j];
+  for (int j = 0; j < 3; ++j) f->p[j] = host[10 + j];
+  for (int j = 0; j < 36; ++j) {
+    f->S[j] = S ? S[j] : 0.0;
+    if (!std::isfinite(f->S[j])) { set_error("%s: S is not finite", what); return TB_ERR_ARG; }
+  }
+  f->ref = (int)ref;
+  int n = 0;
+  for (int k = (int)body; k >= 0; k = (int)m.body[k][0]) ++n;   // parents are validated: parent[k] < k
+  f->n = n;
+  for (int k = (int)body, i = n - 1; k >= 0; k = (int)m.body[k][0], --i) f->chain[i] = k;
+  for (int i = n; i < NB; ++i) f->chain[i] = 0;
+  return 0;
+}
+
 unsigned blocks(const int M) { return (unsigned)((M + THREADS - 1) / THREADS); }
 
 }  // namespace
@@ -269,4 +400,31 @@ extern "C" int tbd_torque_terms(const double *model_host, int nv, int M, const d
   if (const int rc = load_model(model_host, nv, M, &m, "tbd_torque_terms")) return rc;
   torque_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, nv, M, q, qs, qss, friction, a, b, c);
   return launch_status("tbd_torque_terms");
+}
+
+extern "C" int tbd_frame_velocity(const double *model_host, int nv, const double *frame_host, int M, const double *q,
+                                  const double *qd, double *v, void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !q || !qd || !v) { set_error("tbd_frame_velocity: null pointer"); return TB_ERR_ARG; }
+  DynModel m;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_frame_velocity")) return rc;
+  DynFrame f;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, &f, "tbd_frame_velocity")) return rc;
+  frame_velocity_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qd, v);
+  return launch_status("tbd_frame_velocity");
+}
+
+extern "C" int tbd_velocity_norm_terms(const double *model_host, int nv, const double *frame_host, const double *S_host,
+                                       int M, const double *q, const double *qs, double *b, void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !S_host || !q || !qs || !b) {
+    set_error("tbd_velocity_norm_terms: null pointer");
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_velocity_norm_terms")) return rc;
+  DynFrame f;
+  if (const int rc = load_frame(frame_host, m, nv, S_host, &f, "tbd_velocity_norm_terms")) return rc;
+  velocity_norm_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qs, b);
+  return launch_status("tbd_velocity_norm_terms");
 }

@@ -7,7 +7,11 @@ whose inverse dynamics run on the GPU (libtoppra_b200_dyn.so, Featherstone's rec
 
 A `RigidBodyModel` is a valid `inv_dyn` for `JointTorqueConstraint` and `SecondOrderConstraint.joint_torque_constraint`;
 there it takes the device route: the three inverse-dynamics terms of every gridpoint of the batch come from ONE fused
-launch (`torque_terms`).  The packed layout the library takes is documented in include/toppra_b200_dyn.h."""
+launch (`torque_terms`).  The packed layout the library takes is documented in include/toppra_b200_dyn.h.
+
+    tcp = model.frame("flange", xyz=(0, 0, 0.1))              # a RigidBodyFrame: the tool-centre point
+    v = tcp(q, qd)                                            # (M, 6) frame velocities, one kernel launch
+    pc = CartesianVelocityNorm(tcp, S, limit)                 # tool-speed limit, batched on the device"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -19,6 +23,8 @@ MAX_BODIES = 16
 BODY_DOUBLES = 27
 REVOLUTE, PRISMATIC = 0, 1
 _JOINT_TYPES = {"revolute": REVOLUTE, "continuous": REVOLUTE, "prismatic": PRISMATIC}
+# pinocchio's ReferenceFrame values (include/toppra_b200_dyn.h TBD_WORLD, TBD_LOCAL, TBD_LOCAL_WORLD_ALIGNED)
+REFERENCE_FRAMES = {"world": 0, "local": 1, "local_world_aligned": 2}
 
 
 def rpy_matrix(rpy):
@@ -48,7 +54,7 @@ class RigidBodyModel(object):
     centre of mass in the body frame; gravity (3,) in the base frame."""
 
     def __init__(self, parent, joint_type, axis, E, r, mass, com, inertia, gravity=(0.0, 0.0, -9.81), joint_names=None,
-                 effort_limit=None, velocity_limit=None):
+                 effort_limit=None, velocity_limit=None, frames=None):
         parent = np.asarray(parent, dtype=np.float64).reshape(-1)
         nv = parent.shape[0]
         if not 1 <= nv <= MAX_BODIES:
@@ -75,6 +81,9 @@ class RigidBodyModel(object):
         inf = np.full(nv, np.inf)
         self.effort_limit = inf.copy() if effort_limit is None else np.asarray(effort_limit, dtype=np.float64)
         self.velocity_limit = inf.copy() if velocity_limit is None else np.asarray(velocity_limit, dtype=np.float64)
+        # name -> (body index, R, p): frames rigidly attached to a body (-1 = the base), in that body's coordinates
+        self.frames = dict(frames) if frames is not None else {"body%d" % k: (k, np.eye(3), np.zeros(3))
+                                                               for k in range(nv)}
 
     @property
     def dof(self):
@@ -87,6 +96,19 @@ class RigidBodyModel(object):
     def body(self, k):
         """The 27 packed doubles of body k (include/toppra_b200_dyn.h)."""
         return self.packed[3 + BODY_DOUBLES * k:3 + BODY_DOUBLES * (k + 1)].copy()
+
+    def frame(self, name, xyz=(0.0, 0.0, 0.0), rpy=(0.0, 0.0, 0.0), reference_frame="local_world_aligned"):
+        """The frame `name` of the frame table (every URDF link, or "body<k>"), moved by the offset `xyz` / `rpy` in
+        its own coordinates (URDF origin convention; e.g. a tool-centre point), whose velocities are expressed in
+        `reference_frame`: "local", "world" or "local_world_aligned" (pinocchio's ReferenceFrame)."""
+        if name not in self.frames:
+            raise ValueError("RigidBodyModel has no frame %r (frames: %s)" % (name, sorted(self.frames)))
+        if reference_frame not in REFERENCE_FRAMES:
+            raise ValueError("unknown reference_frame %r (known: %s)" % (reference_frame, sorted(REFERENCE_FRAMES)))
+        body, R, p = self.frames[name]
+        Ro = rpy_matrix(np.asarray(rpy, dtype=np.float64).reshape(3))
+        return RigidBodyFrame(self, name, body, R @ Ro, p + R @ np.asarray(xyz, dtype=np.float64).reshape(3),
+                              reference_frame)
 
     def torque_limits(self):
         """(nv, 2) [-effort, effort] per joint, the tau_lim of JointTorqueConstraint (+-inf where the URDF has none)."""
@@ -182,6 +204,7 @@ class RigidBodyModel(object):
 
         bodies = []          # dicts of one moving body each, in DOF order
         parts = {-1: []}     # body index -> [(mass, com, inertia about com)] in the body frame
+        frames = {}          # link name -> (body index, R, p) of the link frame in the body frame
 
         def origin(el):
             o = el.find("origin") if el is not None else None
@@ -203,6 +226,7 @@ class RigidBodyModel(object):
             parts[body].append((m, R @ pi + p, Rb @ I @ Rb.T))
 
         def visit(link, body, R, p):
+            frames[link] = (body, R, p)
             add_inertial(body, link, R, p)
             for el in children[link]:
                 name, jtype = el.get("name"), el.get("type")
@@ -250,4 +274,67 @@ class RigidBodyModel(object):
         return cls([b["parent"] for b in bodies], [b["type"] for b in bodies], [b["axis"] for b in bodies],
                    [b["E"] for b in bodies], [b["r"] for b in bodies], mass, com, inertia, gravity,
                    joint_names=[b["name"] for b in bodies], effort_limit=[b["effort"] for b in bodies],
-                   velocity_limit=[b["velocity"] for b in bodies])
+                   velocity_limit=[b["velocity"] for b in bodies], frames=frames)
+
+
+class RigidBodyFrame(object):
+    """A frame rigidly attached to a body of a RigidBodyModel (model.frame(...)): body index (-1 = the base), its
+    placement (R, p) in the body frame and the reference frame of its velocities.  `packed` is the host array of
+    include/toppra_b200_dyn.h.
+
+    A velocity is [linear(3); angular(3)] (pinocchio's Motion::toVector()).  With p_f, R_f the frame's world placement
+    and w the world angular velocity: "local_world_aligned" (dp_f, w), "local" (R_f^T dp_f, R_f^T w), "world"
+    (dp_f - w x p_f, w), the spatial velocity at the world origin.  Calling the frame like `compute_velocity(q, qd)` makes
+    it the frame-velocity callback of CartesianVelocityNorm, which then takes its device route."""
+
+    def __init__(self, model, name, body, R, p, reference_frame="local_world_aligned"):
+        self.model = model
+        self.name = name
+        self.body = int(body)
+        self.R = np.array(R, dtype=np.float64).reshape(3, 3)
+        self.p = np.array(p, dtype=np.float64).reshape(3)
+        self.reference_frame = reference_frame
+        self.packed = np.concatenate(([float(self.body)], self.R.reshape(9), self.p,
+                                      [float(REFERENCE_FRAMES[reference_frame])]))
+
+    @property
+    def nv(self):
+        return self.model.nv
+
+    def _frame_ptr(self):
+        return ctypes.c_void_p(self.packed.ctypes.data)
+
+    def __call__(self, q, qd):
+        """Frame velocities.  CUDA tensors (M, nv) -> (M, 6), one tbd_frame_velocity launch on the current stream;
+        numpy (nv,) -> (6,) or (M, nv) -> (M, 6), through a device round trip."""
+        torch = _lib.require_cuda()
+        m = self.model
+        if isinstance(q, torch.Tensor) and q.is_cuda:
+            q, qd = m._prepare(torch, q, qd)
+            v = torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device)
+            with torch.cuda.device(q.device):
+                _lib.check(_lib_dyn.load().tbd_frame_velocity(m._model_ptr(), m.nv, self._frame_ptr(), q.shape[0],
+                                                              _lib.ptr(q), _lib.ptr(qd), _lib.ptr(v), _lib.stream_ptr()),
+                           "tbd_frame_velocity")
+            return v
+        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd)]
+        single = arrs[0].ndim == 1
+        v = self(*[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
+        return v[0] if single else v
+
+    def velocity_norm_terms(self, q, qs, S):
+        """b = v^T (S v), v the frame velocity at (q, qs = q'), for CUDA tensors (M, nv) -> (M,): one
+        tbd_velocity_norm_terms launch.  S: (6, 6)."""
+        torch = _lib.require_cuda()
+        m = self.model
+        q, qs = m._prepare(torch, q, qs)
+        S = np.ascontiguousarray(S, dtype=np.float64)
+        if S.shape != (6, 6):
+            raise ValueError("S matrix should be of size 6x6.")
+        b = torch.empty(q.shape[0], dtype=torch.float64, device=q.device)
+        with torch.cuda.device(q.device):
+            _lib.check(_lib_dyn.load().tbd_velocity_norm_terms(m._model_ptr(), m.nv, self._frame_ptr(),
+                                                               ctypes.c_void_p(S.ctypes.data), q.shape[0], _lib.ptr(q),
+                                                               _lib.ptr(qs), _lib.ptr(b), _lib.stream_ptr()),
+                       "tbd_velocity_norm_terms")
+        return b
