@@ -85,6 +85,29 @@ int tbd_frame_velocity(const double *model_host, int nv, const double *frame_hos
 int tbd_velocity_norm_terms(const double *model_host, int nv, const double *frame_host, const double *S_host, int M,
                             const double *q, const double *qs, double *b, void *stream);
 
+/* acc = the classical acceleration of the frame frame_host at (q, qd, qdd) for M points, one thread per point
+ * (pinocchio's getFrameClassicalAcceleration; no gravity, purely kinematic).  [linear(3); angular(3)]: the second time
+ * derivative of the frame origin's world position p_f and dw/dt, expressed as
+ *   TBD_LOCAL_WORLD_ALIGNED   (d2p_f/dt2, dw/dt)
+ *   TBD_LOCAL                 (R_f^T d2p_f/dt2, R_f^T dw/dt)
+ * acc = J(q) qdd + dJ(q, qd) qd is affine in (s'', s'^2) along a path: with qd = q' s', qdd = q' s'' + q'' s'^2,
+ * acc = acc(q, 0, q') s'' + acc(q, q', q'') s'^2.
+ *   q, qd, qdd [M][nv]; acc [M][6].  TB_ERR_UNSUPPORTED for a TBD_WORLD frame; otherwise the checks of
+ *   tbd_frame_velocity. */
+int tbd_frame_acceleration(const double *model_host, int nv, const double *frame_host, int M, const double *q,
+                           const double *qd, const double *qdd, double *acc, void *stream);
+
+/* The rows of CartesianAccelerationConstraint in one launch, one chain walk per point (the joint transforms and their
+ * sincos are shared by both states):
+ *   a = acc(q, 0, qs);  b = acc(q, qs, qss)
+ * restricted to the components of the bit mask `components`: bit j selects component j of [ax, ay, az, wx, wy, wz];
+ * the k = popcount(components) columns come in increasing j.  Bit-identical to two tbd_frame_acceleration launches
+ * (with qd = 0 and qd = qs) followed by that column selection.
+ *   q, qs, qss [M][nv]; a, b [M][k].  TB_ERR_ARG for components outside 1..63; otherwise the checks of
+ *   tbd_frame_acceleration. */
+int tbd_acceleration_terms(const double *model_host, int nv, const double *frame_host, int components, int M,
+                           const double *q, const double *qs, const double *qss, double *a, double *b, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -6,8 +6,10 @@ from .linear_joint_velocity import JointVelocityConstraint, JointVelocityConstra
 from .linear_second_order import SecondOrderConstraint
 from .joint_torque import JointTorqueConstraint
 from .cartesian_velocity_norm import CartesianVelocityNorm
+from .cartesian_acceleration import CartesianAccelerationConstraint
 from .conic_constraint import ConicConstraint, RobustLinearConstraint
 
 __all__ = ["ConstraintType", "DiscretizationType", "Constraint", "LinearConstraint",
            "canlinear_colloc_to_interpolate", "JointAccelerationConstraint", "JointVelocityConstraint", "JointVelocityConstraintVarying",
-           "SecondOrderConstraint", "JointTorqueConstraint", "CartesianVelocityNorm", "RecordContext", "ConicConstraint", "RobustLinearConstraint"]
+           "SecondOrderConstraint", "JointTorqueConstraint", "CartesianVelocityNorm", "CartesianAccelerationConstraint",
+           "RecordContext", "ConicConstraint", "RobustLinearConstraint"]

@@ -13,6 +13,8 @@ The three inverse-dynamics evaluations per gridpoint are USER code.  Two ways to
   * a `toppra_b200.RigidBodyModel` as `inv_dyn` (joint_torque_constraint, JointTorqueConstraint): the batched route
     with the three terms from ONE fused rigid-body inverse-dynamics launch per batch (libtoppra_b200_dyn.so:
     tbd_torque_terms), bit-identical to three `model(...)` calls plus the operations below;
+  * a `toppra_b200.RigidBodyFrame` as `inv_dyn` (CartesianAccelerationConstraint): the same route with a and b of the
+    frame's acceleration from ONE launch per batch (tbd_acceleration_terms) and c = 0;
   * `device_model=(name, params)` (joint_torque_constraint only): the inverse dynamics is one of the models compiled
     into the library (`engine.DEVICE_MODELS`, include/toppra_b200.h TB_INVDYN_*): ONE kernel evaluates q, q', q'' and
     the three inverse-dynamics terms per gridpoint and writes the torque rows straight into the stage records
@@ -22,7 +24,7 @@ import numpy as np
 from .constraint import DiscretizationType
 from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate
 from .. import engine
-from ..dynamics import RigidBodyModel
+from ..dynamics import RigidBodyFrame, RigidBodyModel
 
 
 class SecondOrderConstraint(LinearConstraint):
@@ -112,7 +114,7 @@ class SecondOrderConstraint(LinearConstraint):
     # ---- device protocol ----------------------------------------------------------------------------------
     def _k(self):
         if self._eye_form is not None:
-            return 2 * self.dof
+            return self._eye_form[0].shape[-1]   # F = [I; -I]: 2 dof rows for torques, 2 k for frame accelerations
         if self.batched:
             raise NotImplementedError("batched SecondOrderConstraint with a general F: use joint_torque_constraint")
         return self.constraint_F(np.zeros(self.dof)).shape[0]
@@ -132,6 +134,11 @@ class SecondOrderConstraint(LinearConstraint):
             if isinstance(self.inv_dyn, RigidBodyModel) and self._eye_form is not None:
                 a, b, c = self.inv_dyn.torque_terms(q, qd, qdd, self._eye_form[1])
                 return (a.reshape(B, G, dof), b.reshape(B, G, dof), c.reshape(B, G, dof))
+            if isinstance(self.inv_dyn, RigidBodyFrame) and self._eye_form is not None:
+                # CartesianAccelerationConstraint: acc(q, 0, 0) = 0, so c = 0 and a, b need no subtraction
+                a, b = self.inv_dyn.acceleration_terms(q, qd, qdd, self.components)
+                m = a.shape[-1]
+                return a.reshape(B, G, m), b.reshape(B, G, m), torch.zeros((B, G, m), dtype=a.dtype, device=a.device)
             zero = torch.zeros_like(q)
             c = self.inv_dyn(q, zero, zero)
             a = self.inv_dyn(q, zero, qd) - c

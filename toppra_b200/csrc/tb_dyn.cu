@@ -13,6 +13,11 @@
 // Both run frame_velocity, which walks only the frame's root-to-body chain with its state in registers (no local
 // arrays); the per-body placement is TB_BODY_TRANSFORM, shared with joint_transforms.
 //
+//   frame_acceleration_kernel   acc = the classical 6-D acceleration of a frame at (q, qd, qdd), one thread per point;
+//   acceleration_terms_kernel   a = acc(q, 0, q'), b = acc(q, q', q''), selected components: the rows of
+//                               CartesianAccelerationConstraint, one thread and one chain walk per point.
+// Both run frame_acceleration, the same register walk with the angular acceleration and the origin acceleration.
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -306,6 +311,108 @@ velocity_norm_terms_kernel(const __grid_constant__ DynModel m, const __grid_cons
   b[pt] = acc;
 }
 
+// The classical acceleration [linear(3); angular(3)] of frame f at NS states (qd[s], qdd[s]) of one configuration q,
+// in f's reference frame (TBD_LOCAL or TBD_LOCAL_WORLD_ALIGNED; TBD_WORLD is refused on the host).  One walk of f's
+// chain from the root: the world rotation Rw and the joint transforms (with their sincos) are shared by the states,
+// each of which keeps w, dw and the body-origin acceleration ao in registers, in world coordinates.  For body k with
+// d = Rw p_k from the parent's Rw:
+//   ao += dw x d + w x (w x d);  Rw = Rw R_k;  s = Rw axis_k;
+//   revolute   dw += s qdd_k + w x (s qd_k);  w += s qd_k
+//   prismatic  ao += s qdd_k + 2 w x (s qd_k)
+// and at the frame origin, d = Rw p_f:  a_f = ao + dw x d + w x (w x d).  A null qd[s] stands for qd = 0: the state
+// then runs the same operations on a literal 0.0, so its result is bit-identical to a call with a zero array.
+template <int NS>
+__device__ __forceinline__ void frame_acceleration(const DynModel &m, const DynFrame &f, const double *__restrict__ q,
+                                                   const double *const (&qd)[NS], const double *const (&qdd)[NS],
+                                                   double (&acc)[NS][6]) {
+  double Rw[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+  double w[NS][3], dw[NS][3], ao[NS][3];
+  for (int s = 0; s < NS; ++s)
+    for (int j = 0; j < 3; ++j) { w[s][j] = 0.0; dw[s][j] = 0.0; ao[s][j] = 0.0; }
+  for (int i = 0; i < f.n; ++i) {
+    const int k = f.chain[i];
+    const double *bd = m.body[k];
+    double R[9], p[3], d[3], Rn[9];
+    const double qk = q[k];
+    TB_BODY_TRANSFORM(bd, qk, R, p);
+    mul3(Rw, p, d);                     // origin of body k relative to its parent's, world coordinates
+    for (int s = 0; s < NS; ++s) {
+      double t1[3], t2[3], t3[3];
+      cross3(dw[s], d, t1);
+      cross3(w[s], d, t2);
+      cross3(w[s], t2, t3);
+      for (int j = 0; j < 3; ++j) ao[s][j] = ao[s][j] + t1[j] + t3[j];
+    }
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) Rn[3 * r + c] = Rw[3 * r] * R[c] + Rw[3 * r + 1] * R[3 + c] + Rw[3 * r + 2] * R[6 + c];
+    for (int j = 0; j < 9; ++j) Rw[j] = Rn[j];
+    double sx[3];
+    mul3(Rw, bd + 2, sx);               // joint axis, world coordinates
+    const bool revolute = bd[1] == TBD_REVOLUTE;
+    for (int s = 0; s < NS; ++s) {
+      const double qdk = qd[s] ? qd[s][k] : 0.0, qddk = qdd[s][k];
+      double sq[3], c[3];
+      for (int j = 0; j < 3; ++j) sq[j] = sx[j] * qdk;
+      cross3(w[s], sq, c);
+      if (revolute) {
+        for (int j = 0; j < 3; ++j) { dw[s][j] = dw[s][j] + sx[j] * qddk + c[j]; w[s][j] = w[s][j] + sq[j]; }
+      } else {
+        for (int j = 0; j < 3; ++j) ao[s][j] = ao[s][j] + sx[j] * qddk + 2.0 * c[j];
+      }
+    }
+  }
+  double d[3], Rf[9];
+  mul3(Rw, f.p, d);                     // frame origin relative to the body origin, world coordinates
+  if (f.ref == TBD_LOCAL)
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) Rf[3 * r + c] = Rw[3 * r] * f.R[c] + Rw[3 * r + 1] * f.R[3 + c] + Rw[3 * r + 2] * f.R[6 + c];
+  for (int s = 0; s < NS; ++s) {
+    double t1[3], t2[3], t3[3], af[3];
+    cross3(dw[s], d, t1);
+    cross3(w[s], d, t2);
+    cross3(w[s], t2, t3);
+    for (int j = 0; j < 3; ++j) af[j] = ao[s][j] + t1[j] + t3[j];
+    if (f.ref == TBD_LOCAL) {
+      mul3t(Rf, af, acc[s]);
+      mul3t(Rf, dw[s], acc[s] + 3);
+    } else {                            // TBD_LOCAL_WORLD_ALIGNED
+      for (int j = 0; j < 3; ++j) { acc[s][j] = af[j]; acc[s][3 + j] = dw[s][j]; }
+    }
+  }
+}
+
+__global__ void __launch_bounds__(THREADS)
+frame_acceleration_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame f, const int nv,
+                          const int M, const double *__restrict__ q, const double *__restrict__ qd,
+                          const double *__restrict__ qdd, double *__restrict__ acc) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  const double *const qds[1] = {qd + o}, *const qdds[1] = {qdd + o};
+  double x[1][6];
+  frame_acceleration<1>(m, f, q + o, qds, qdds, x);
+  for (int j = 0; j < 6; ++j) acc[(size_t)pt * 6 + j] = x[0][j];
+}
+
+// a = acc(q, 0, q'), b = acc(q, q', q''): the rows of CartesianAccelerationConstraint, the components of bit mask
+// `components` in increasing order (k = popcount columns).  One chain walk for both states.
+__global__ void __launch_bounds__(THREADS)
+acceleration_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame f, const int nv,
+                          const int components, const int k, const int M, const double *__restrict__ q,
+                          const double *__restrict__ qs, const double *__restrict__ qss, double *__restrict__ a,
+                          double *__restrict__ b) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  const double *const qds[2] = {nullptr, qs + o}, *const qdds[2] = {qs + o, qss + o};
+  double x[2][6];
+  frame_acceleration<2>(m, f, q + o, qds, qdds, x);
+  double *ao = a + (size_t)pt * k, *bo = b + (size_t)pt * k;
+  int c = 0;
+  for (int j = 0; j < 6; ++j)
+    if ((components >> j) & 1) { ao[c] = x[0][j]; bo[c] = x[1][j]; ++c; }
+}
+
 int launch_status(const char *what) {
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -427,4 +534,56 @@ extern "C" int tbd_velocity_norm_terms(const double *model_host, int nv, const d
   if (const int rc = load_frame(frame_host, m, nv, S_host, &f, "tbd_velocity_norm_terms")) return rc;
   velocity_norm_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qs, b);
   return launch_status("tbd_velocity_norm_terms");
+}
+
+namespace {
+// load_model and load_frame, then refuse TBD_WORLD: a classical acceleration "at the world origin" is no limit a user
+// means.
+int load_accel(const double *model_host, const int nv, const double *frame_host, const int M, tb::DynModel *m,
+               tb::DynFrame *f, const char *what) {
+  using namespace tb;
+  if (const int rc = load_model(model_host, nv, M, m, what)) return rc;
+  if (const int rc = load_frame(frame_host, *m, nv, nullptr, f, what)) return rc;
+  if (f->ref == TBD_WORLD) {
+    set_error("%s: the world reference frame is not supported for accelerations (use local or local_world_aligned)",
+              what);
+    return TB_ERR_UNSUPPORTED;
+  }
+  return 0;
+}
+}  // namespace
+
+extern "C" int tbd_frame_acceleration(const double *model_host, int nv, const double *frame_host, int M,
+                                      const double *q, const double *qd, const double *qdd, double *acc, void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !q || !qd || !qdd || !acc) {
+    set_error("tbd_frame_acceleration: null pointer");
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynFrame f;
+  if (const int rc = load_accel(model_host, nv, frame_host, M, &m, &f, "tbd_frame_acceleration")) return rc;
+  frame_acceleration_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qd, qdd, acc);
+  return launch_status("tbd_frame_acceleration");
+}
+
+extern "C" int tbd_acceleration_terms(const double *model_host, int nv, const double *frame_host, int components, int M,
+                                      const double *q, const double *qs, const double *qss, double *a, double *b,
+                                      void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !q || !qs || !qss || !a || !b) {
+    set_error("tbd_acceleration_terms: null pointer");
+    return TB_ERR_ARG;
+  }
+  if (components < 1 || components > 63) {
+    set_error("tbd_acceleration_terms: components=%d must be a bit mask in 1..63", components);
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynFrame f;
+  if (const int rc = load_accel(model_host, nv, frame_host, M, &m, &f, "tbd_acceleration_terms")) return rc;
+  const int k = __builtin_popcount((unsigned)components);
+  acceleration_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, components, k, M, q, qs, qss,
+                                                                              a, b);
+  return launch_status("tbd_acceleration_terms");
 }

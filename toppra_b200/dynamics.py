@@ -11,7 +11,9 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
 
     tcp = model.frame("flange", xyz=(0, 0, 0.1))              # a RigidBodyFrame: the tool-centre point
     v = tcp(q, qd)                                            # (M, 6) frame velocities, one kernel launch
-    pc = CartesianVelocityNorm(tcp, S, limit)                 # tool-speed limit, batched on the device"""
+    pc = CartesianVelocityNorm(tcp, S, limit)                 # tool-speed limit, batched on the device
+    acc = tcp.acceleration(q, qd, qdd)                        # (M, 6) classical frame accelerations, one launch
+    pc = CartesianAccelerationConstraint(tcp, alim)           # tool-acceleration limit, batched on the device"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -338,3 +340,61 @@ class RigidBodyFrame(object):
                                                                _lib.ptr(qs), _lib.ptr(b), _lib.stream_ptr()),
                        "tbd_velocity_norm_terms")
         return b
+
+    def _check_acceleration(self):
+        if self.reference_frame == "world":
+            raise ValueError("RigidBodyFrame %r: frame accelerations are classical accelerations of the frame origin; "
+                             "the \"world\" reference frame is not supported (use \"local\" or \"local_world_aligned\")"
+                             % self.name)
+
+    def acceleration(self, q, qd, qdd):
+        """Classical frame accelerations [linear(3); angular(3)] (pinocchio's getFrameClassicalAcceleration, no
+        gravity): "local_world_aligned" (d2p_f/dt2, dw/dt), "local" (R_f^T d2p_f/dt2, R_f^T dw/dt).  CUDA tensors
+        (M, nv) -> (M, 6), one tbd_frame_acceleration launch on the current stream; numpy (nv,) -> (6,) or (M, nv) ->
+        (M, 6), through a device round trip.  On one numpy point it is an `inv_dyn` of SecondOrderConstraint."""
+        self._check_acceleration()
+        torch = _lib.require_cuda()
+        m = self.model
+        if isinstance(q, torch.Tensor) and q.is_cuda:
+            q, qd, qdd = m._prepare(torch, q, qd, qdd)
+            acc = torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device)
+            with torch.cuda.device(q.device):
+                _lib.check(_lib_dyn.load().tbd_frame_acceleration(m._model_ptr(), m.nv, self._frame_ptr(), q.shape[0],
+                                                                  _lib.ptr(q), _lib.ptr(qd), _lib.ptr(qdd),
+                                                                  _lib.ptr(acc), _lib.stream_ptr()),
+                           "tbd_frame_acceleration")
+            return acc
+        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd, qdd)]
+        single = arrs[0].ndim == 1
+        acc = self.acceleration(*[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
+        return acc[0] if single else acc
+
+    def acceleration_terms(self, q, qs, qss, components):
+        """a = acc(q, 0, qs), b = acc(q, qs, qss) for CUDA tensors (M, nv), restricted to `components` (indices into
+        [ax, ay, az, wx, wy, wz]; the columns come in increasing index order): one tbd_acceleration_terms launch.
+        Returns (a, b), each (M, k)."""
+        self._check_acceleration()
+        comps = component_indices(components)
+        torch = _lib.require_cuda()
+        m = self.model
+        q, qs, qss = m._prepare(torch, q, qs, qss)
+        a = torch.empty((q.shape[0], len(comps)), dtype=torch.float64, device=q.device)
+        b = torch.empty_like(a)
+        mask = sum(1 << j for j in comps)
+        with torch.cuda.device(q.device):
+            _lib.check(_lib_dyn.load().tbd_acceleration_terms(m._model_ptr(), m.nv, self._frame_ptr(), mask, q.shape[0],
+                                                              _lib.ptr(q), _lib.ptr(qs), _lib.ptr(qss), _lib.ptr(a),
+                                                              _lib.ptr(b), _lib.stream_ptr()),
+                       "tbd_acceleration_terms")
+        return a, b
+
+
+def component_indices(components):
+    """Sorted indices into [ax, ay, az, wx, wy, wz] of a frame acceleration; ValueError when `components` is empty,
+    repeats an index or has one outside 0..5."""
+    comps = np.asarray(components).reshape(-1)
+    if (comps.size == 0 or comps.dtype.kind not in "iu" or len(set(comps.tolist())) != comps.size
+            or comps.min() < 0 or comps.max() > 5):
+        raise ValueError("components %r: expected distinct indices in 0..5 of [ax, ay, az, wx, wy, wz]"
+                         % (components,))
+    return sorted(comps.tolist())
