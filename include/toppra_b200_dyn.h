@@ -57,6 +57,7 @@ extern "C" {
 #define TBD_WORLD 0
 #define TBD_LOCAL 1
 #define TBD_LOCAL_WORLD_ALIGNED 2
+#define TBD_OBJECT_DOUBLES 10
 
 int tbd_version(void);
 
@@ -107,6 +108,33 @@ int tbd_frame_acceleration(const double *model_host, int nv, const double *frame
  *   tbd_frame_acceleration. */
 int tbd_acceleration_terms(const double *model_host, int nv, const double *frame_host, int components, int M,
                            const double *q, const double *qs, const double *qss, double *a, double *b, void *stream);
+
+/* w = the wrench [f(3); tau(3)] the contact frame frame_host exerts on an object it carries, at (q, qd, qdd) for M
+ * points, one thread per point (toppra_b200.constraint.ContactStabilityConstraint).  The frame's origin is the centre
+ * of the contact area and its z axis the support normal, pointing into the object.  object_host is a HOST array of
+ * TBD_OBJECT_DOUBLES doubles, all in contact-frame coordinates:
+ *
+ *   +0              mass m
+ *   +1  .. +3       r: centre of mass
+ *   +4  .. +9       rotational inertia Ic about the centre of mass: Ixx, Ixy, Ixz, Iyy, Iyz, Izz
+ *
+ * With R_f the frame's world orientation, g_l = R_f^T g (g the model's gravity), a_r the classical acceleration of
+ * the centre of mass, w and dw the frame's angular velocity and acceleration, all in frame axes:
+ *   f = m (a_r - g_l);  tau = Ic dw + w x (Ic w) + r x f      (tau about the frame origin)
+ * The wrench is always in the frame's own axes: the reference-frame field of frame_host (+13) is ignored.
+ *   q, qd, qdd [M][nv]; w [M][6].  TB_ERR_ARG for a null or non-finite object or m <= 0; otherwise the model and frame
+ *   checks of tbd_frame_acceleration. */
+int tbd_contact_wrench(const double *model_host, int nv, const double *frame_host, const double *object_host, int M,
+                       const double *q, const double *qd, const double *qdd, double *w, void *stream);
+
+/* The three terms of SecondOrderConstraint with the contact wrench as inverse dynamics, in one launch and one chain
+ * walk per point:
+ *   c = w(q, 0, 0);  a = w(q, 0, qs) - c;  b = w(q, qs, qss) - c
+ * Bit-identical to three tbd_contact_wrench launches followed by the two subtractions.
+ *   q, qs, qss [M][nv]; a, b, c [M][6].  The checks of tbd_contact_wrench. */
+int tbd_contact_wrench_terms(const double *model_host, int nv, const double *frame_host, const double *object_host,
+                             int M, const double *q, const double *qs, const double *qss, double *a, double *b,
+                             double *c, void *stream);
 
 #ifdef __cplusplus
 }

@@ -22,6 +22,9 @@ _PROTOS = {
     "tbd_velocity_norm_terms": ([_c_dp, _int, _c_dp, _c_dp, _int, _c_dp, _c_dp, _c_dp, _stream], _int),
     "tbd_frame_acceleration": ([_c_dp, _int, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
     "tbd_acceleration_terms": ([_c_dp, _int, _c_dp, _int, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
+    "tbd_contact_wrench": ([_c_dp, _int, _c_dp, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
+    "tbd_contact_wrench_terms": ([_c_dp, _int, _c_dp, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream],
+                                 _int),
 }
 
 _dlib = None

@@ -7,9 +7,11 @@ from .linear_second_order import SecondOrderConstraint
 from .joint_torque import JointTorqueConstraint
 from .cartesian_velocity_norm import CartesianVelocityNorm
 from .cartesian_acceleration import CartesianAccelerationConstraint
+from .contact_stability import ContactStabilityConstraint, contact_wrench_cone
 from .conic_constraint import ConicConstraint, RobustLinearConstraint
 
 __all__ = ["ConstraintType", "DiscretizationType", "Constraint", "LinearConstraint",
            "canlinear_colloc_to_interpolate", "JointAccelerationConstraint", "JointVelocityConstraint", "JointVelocityConstraintVarying",
            "SecondOrderConstraint", "JointTorqueConstraint", "CartesianVelocityNorm", "CartesianAccelerationConstraint",
-           "RecordContext", "ConicConstraint", "RobustLinearConstraint"]
+           "ContactStabilityConstraint", "contact_wrench_cone", "RecordContext", "ConicConstraint",
+           "RobustLinearConstraint"]

@@ -18,6 +18,12 @@
 //                               CartesianAccelerationConstraint, one thread and one chain walk per point.
 // Both run frame_acceleration, the same register walk with the angular acceleration and the origin acceleration.
 //
+//   contact_wrench_kernel        w = the wrench a contact frame exerts on an object it carries, at (q, qd, qdd);
+//   contact_wrench_terms_kernel  c = w(q, 0, 0), a = w(q, 0, q') - c, b = w(q, q', q'') - c: the terms of
+//                                ContactStabilityConstraint, one thread and one chain walk per point.
+// Both run frame_acceleration<NS, true>, which also hands out the frame's orientation and angular velocity, and then
+// contact_wrench.
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -321,10 +327,13 @@ velocity_norm_terms_kernel(const __grid_constant__ DynModel m, const __grid_cons
 //   prismatic  ao += s qdd_k + 2 w x (s qd_k)
 // and at the frame origin, d = Rw p_f:  a_f = ao + dw x d + w x (w x d).  A null qd[s] stands for qd = 0: the state
 // then runs the same operations on a literal 0.0, so its result is bit-identical to a call with a zero array.
-template <int NS>
+// ROT (the contact wrench; f.ref is TBD_LOCAL): also hands out the frame's world orientation Rf_out = Rw R_f and each
+// state's angular velocity in frame axes, wl[s] = Rf^T w; a null qdd[s] then stands for qdd = 0 like a null qd[s].
+template <int NS, bool ROT = false>
 __device__ __forceinline__ void frame_acceleration(const DynModel &m, const DynFrame &f, const double *__restrict__ q,
                                                    const double *const (&qd)[NS], const double *const (&qdd)[NS],
-                                                   double (&acc)[NS][6]) {
+                                                   double (&acc)[NS][6], double (*wl)[3] = nullptr,
+                                                   double *Rf_out = nullptr) {
   double Rw[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
   double w[NS][3], dw[NS][3], ao[NS][3];
   for (int s = 0; s < NS; ++s)
@@ -350,7 +359,7 @@ __device__ __forceinline__ void frame_acceleration(const DynModel &m, const DynF
     mul3(Rw, bd + 2, sx);               // joint axis, world coordinates
     const bool revolute = bd[1] == TBD_REVOLUTE;
     for (int s = 0; s < NS; ++s) {
-      const double qdk = qd[s] ? qd[s][k] : 0.0, qddk = qdd[s][k];
+      const double qdk = qd[s] ? qd[s][k] : 0.0, qddk = (ROT && !qdd[s]) ? 0.0 : qdd[s][k];
       double sq[3], c[3];
       for (int j = 0; j < 3; ++j) sq[j] = sx[j] * qdk;
       cross3(w[s], sq, c);
@@ -363,7 +372,7 @@ __device__ __forceinline__ void frame_acceleration(const DynModel &m, const DynF
   }
   double d[3], Rf[9];
   mul3(Rw, f.p, d);                     // frame origin relative to the body origin, world coordinates
-  if (f.ref == TBD_LOCAL)
+  if (ROT || f.ref == TBD_LOCAL)
     for (int r = 0; r < 3; ++r)
       for (int c = 0; c < 3; ++c) Rf[3 * r + c] = Rw[3 * r] * f.R[c] + Rw[3 * r + 1] * f.R[3 + c] + Rw[3 * r + 2] * f.R[6 + c];
   for (int s = 0; s < NS; ++s) {
@@ -372,13 +381,16 @@ __device__ __forceinline__ void frame_acceleration(const DynModel &m, const DynF
     cross3(w[s], d, t2);
     cross3(w[s], t2, t3);
     for (int j = 0; j < 3; ++j) af[j] = ao[s][j] + t1[j] + t3[j];
-    if (f.ref == TBD_LOCAL) {
+    if (ROT || f.ref == TBD_LOCAL) {
       mul3t(Rf, af, acc[s]);
       mul3t(Rf, dw[s], acc[s] + 3);
+      if constexpr (ROT) mul3t(Rf, w[s], wl[s]);
     } else {                            // TBD_LOCAL_WORLD_ALIGNED
       for (int j = 0; j < 3; ++j) { acc[s][j] = af[j]; acc[s][3 + j] = dw[s][j]; }
     }
   }
+  if constexpr (ROT)
+    for (int j = 0; j < 9; ++j) Rf_out[j] = Rf[j];
 }
 
 __global__ void __launch_bounds__(THREADS)
@@ -411,6 +423,64 @@ acceleration_terms_kernel(const __grid_constant__ DynModel m, const __grid_const
   int c = 0;
   for (int j = 0; j < 6; ++j)
     if ((components >> j) & 1) { ao[c] = x[0][j]; bo[c] = x[1][j]; ++c; }
+}
+
+// An object rigidly held by a contact frame (include/toppra_b200_dyn.h): mass, centre of mass r and rotational inertia
+// Ic about it, both in contact-frame axes.
+struct DynObject {
+  double mass, r[3], Ic[6];
+};
+
+// The wrench [f; tau] the contact frame exerts on the object, at the frame origin in frame axes, from the frame's
+// classical acceleration acc = [a_f; dw] and angular velocity wl (frame axes, frame_acceleration<NS, true>) and
+// gl = Rf^T g:
+//   a_r = a_f + dw x r + w x (w x r);  f = m (a_r - gl);  tau = Ic dw + w x (Ic w) + r x f.
+__device__ __forceinline__ void contact_wrench(const DynObject &o, const double *gl, const double *acc, const double *wl,
+                                               double *out) {
+  double t1[3], t2[3], t3[3], f[3], n[3], Iw[3];
+  cross3(acc + 3, o.r, t1);
+  cross3(wl, o.r, t2);
+  cross3(wl, t2, t3);
+  for (int j = 0; j < 3; ++j) f[j] = o.mass * (acc[j] + t1[j] + t3[j] - gl[j]);
+  mul_inertia(o.Ic, acc + 3, n);
+  mul_inertia(o.Ic, wl, Iw);
+  cross3(wl, Iw, t1);
+  cross3(o.r, f, t2);
+  for (int j = 0; j < 3; ++j) { out[j] = f[j]; out[3 + j] = n[j] + t1[j] + t2[j]; }
+}
+
+__global__ void __launch_bounds__(THREADS)
+contact_wrench_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame f,
+                      const __grid_constant__ DynObject obj, const int nv, const int M, const double *__restrict__ q,
+                      const double *__restrict__ qd, const double *__restrict__ qdd, double *__restrict__ w) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  const double *const qds[1] = {qd + o}, *const qdds[1] = {qdd + o};
+  double x[1][6], wl[1][3], Rf[9], gl[3], y[6];
+  frame_acceleration<1, true>(m, f, q + o, qds, qdds, x, wl, Rf);
+  mul3t(Rf, m.g, gl);
+  contact_wrench(obj, gl, x[0], wl[0], y);
+  for (int j = 0; j < 6; ++j) w[(size_t)pt * 6 + j] = y[j];
+}
+
+// c = w(q, 0, 0), a = w(q, 0, q') - c, b = w(q, q', q'') - c: the terms of ContactStabilityConstraint, one chain walk
+// for the three states.
+__global__ void __launch_bounds__(THREADS)
+contact_wrench_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame f,
+                            const __grid_constant__ DynObject obj, const int nv, const int M,
+                            const double *__restrict__ q, const double *__restrict__ qs, const double *__restrict__ qss,
+                            double *__restrict__ a, double *__restrict__ b, double *__restrict__ c) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  const double *const qds[3] = {nullptr, nullptr, qs + o}, *const qdds[3] = {nullptr, qs + o, qss + o};
+  double x[3][6], wl[3][3], Rf[9], gl[3], y[3][6];
+  frame_acceleration<3, true>(m, f, q + o, qds, qdds, x, wl, Rf);
+  mul3t(Rf, m.g, gl);
+  for (int s = 0; s < 3; ++s) contact_wrench(obj, gl, x[s], wl[s], y[s]);
+  const size_t r = (size_t)pt * 6;
+  for (int j = 0; j < 6; ++j) { c[r + j] = y[0][j]; a[r + j] = y[1][j] - y[0][j]; b[r + j] = y[2][j] - y[0][j]; }
 }
 
 int launch_status(const char *what) {
@@ -586,4 +656,58 @@ extern "C" int tbd_acceleration_terms(const double *model_host, int nv, const do
   acceleration_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, components, k, M, q, qs, qss,
                                                                               a, b);
   return launch_status("tbd_acceleration_terms");
+}
+
+namespace {
+// load_model and load_frame with the frame's reference-frame field ignored (a contact wrench is always in the frame's
+// own axes), then the object: finite, with a positive mass.
+int load_contact(const double *model_host, const int nv, const double *frame_host, const double *object_host,
+                 const int M, tb::DynModel *m, tb::DynFrame *f, tb::DynObject *o, const char *what) {
+  using namespace tb;
+  if (const int rc = load_model(model_host, nv, M, m, what)) return rc;
+  double frame[TBD_FRAME_DOUBLES];
+  for (int j = 0; j < TBD_FRAME_DOUBLES; ++j) frame[j] = frame_host[j];
+  frame[13] = TBD_LOCAL;
+  if (const int rc = load_frame(frame, *m, nv, nullptr, f, what)) return rc;
+  for (int j = 0; j < TBD_OBJECT_DOUBLES; ++j)
+    if (!std::isfinite(object_host[j])) { set_error("%s: object parameters are not finite", what); return TB_ERR_ARG; }
+  if (!(object_host[0] > 0.0)) { set_error("%s: object mass %g must be positive", what, object_host[0]); return TB_ERR_ARG; }
+  o->mass = object_host[0];
+  for (int j = 0; j < 3; ++j) o->r[j] = object_host[1 + j];
+  for (int j = 0; j < 6; ++j) o->Ic[j] = object_host[4 + j];
+  return 0;
+}
+}  // namespace
+
+extern "C" int tbd_contact_wrench(const double *model_host, int nv, const double *frame_host, const double *object_host,
+                                  int M, const double *q, const double *qd, const double *qdd, double *w,
+                                  void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !object_host || !q || !qd || !qdd || !w) {
+    set_error("tbd_contact_wrench: null pointer");
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynFrame f;
+  DynObject o;
+  if (const int rc = load_contact(model_host, nv, frame_host, object_host, M, &m, &f, &o, "tbd_contact_wrench")) return rc;
+  contact_wrench_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, o, nv, M, q, qd, qdd, w);
+  return launch_status("tbd_contact_wrench");
+}
+
+extern "C" int tbd_contact_wrench_terms(const double *model_host, int nv, const double *frame_host,
+                                        const double *object_host, int M, const double *q, const double *qs,
+                                        const double *qss, double *a, double *b, double *c, void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !object_host || !q || !qs || !qss || !a || !b || !c) {
+    set_error("tbd_contact_wrench_terms: null pointer");
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynFrame f;
+  DynObject o;
+  if (const int rc = load_contact(model_host, nv, frame_host, object_host, M, &m, &f, &o, "tbd_contact_wrench_terms"))
+    return rc;
+  contact_wrench_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, o, nv, M, q, qs, qss, a, b, c);
+  return launch_status("tbd_contact_wrench_terms");
 }

@@ -13,7 +13,8 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     v = tcp(q, qd)                                            # (M, 6) frame velocities, one kernel launch
     pc = CartesianVelocityNorm(tcp, S, limit)                 # tool-speed limit, batched on the device
     acc = tcp.acceleration(q, qd, qdd)                        # (M, 6) classical frame accelerations, one launch
-    pc = CartesianAccelerationConstraint(tcp, alim)           # tool-acceleration limit, batched on the device"""
+    pc = CartesianAccelerationConstraint(tcp, alim)           # tool-acceleration limit, batched on the device
+    pc = ContactStabilityConstraint(tray, m, com, I, (X, Y), mu)  # an object carried on a tray must not slide or tip"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -387,6 +388,57 @@ class RigidBodyFrame(object):
                                                               _lib.ptr(b), _lib.stream_ptr()),
                        "tbd_acceleration_terms")
         return a, b
+
+    def contact_wrench(self, obj, q, qd, qdd):
+        """The wrench [f; tau] this frame, as a contact frame, exerts on an object it carries, at its origin in its own
+        axes (the reference frame is ignored); `obj` is the packed object of include/toppra_b200_dyn.h (m, r, Ic; see
+        ContactStabilityConstraint).  CUDA tensors (M, nv) -> (M, 6), one tbd_contact_wrench launch on the current
+        stream; numpy (nv,) -> (6,) or (M, nv) -> (M, 6), through a device round trip."""
+        obj = _packed_object(obj)
+        torch = _lib.require_cuda()
+        m = self.model
+        if isinstance(q, torch.Tensor) and q.is_cuda:
+            q, qd, qdd = m._prepare(torch, q, qd, qdd)
+            w = torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device)
+            with torch.cuda.device(q.device):
+                _lib.check(_lib_dyn.load().tbd_contact_wrench(m._model_ptr(), m.nv, self._frame_ptr(),
+                                                              ctypes.c_void_p(obj.ctypes.data), q.shape[0], _lib.ptr(q),
+                                                              _lib.ptr(qd), _lib.ptr(qdd), _lib.ptr(w),
+                                                              _lib.stream_ptr()),
+                           "tbd_contact_wrench")
+            return w
+        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd, qdd)]
+        single = arrs[0].ndim == 1
+        w = self.contact_wrench(obj, *[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
+        return w[0] if single else w
+
+    def contact_wrench_terms(self, obj, q, qs, qss):
+        """c = w(q, 0, 0), a = w(q, 0, qs) - c, b = w(q, qs, qss) - c of the contact wrench (contact_wrench) for CUDA
+        tensors (M, nv): one tbd_contact_wrench_terms launch.  Returns (a, b, c), each (M, 6)."""
+        obj = _packed_object(obj)
+        torch = _lib.require_cuda()
+        m = self.model
+        q, qs, qss = m._prepare(torch, q, qs, qss)
+        a, b, c = (torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device) for _ in range(3))
+        with torch.cuda.device(q.device):
+            _lib.check(_lib_dyn.load().tbd_contact_wrench_terms(m._model_ptr(), m.nv, self._frame_ptr(),
+                                                                ctypes.c_void_p(obj.ctypes.data), q.shape[0],
+                                                                _lib.ptr(q), _lib.ptr(qs), _lib.ptr(qss), _lib.ptr(a),
+                                                                _lib.ptr(b), _lib.ptr(c), _lib.stream_ptr()),
+                       "tbd_contact_wrench_terms")
+        return a, b, c
+
+
+OBJECT_DOUBLES = 10
+
+
+def _packed_object(obj):
+    """The packed object of include/toppra_b200_dyn.h (TBD_OBJECT_DOUBLES = 10 doubles: m, r, Ic) as a contiguous
+    float64 array; the library reads exactly 10 doubles from it."""
+    obj = np.ascontiguousarray(obj, dtype=np.float64)
+    if obj.shape != (OBJECT_DOUBLES,):
+        raise ValueError("packed object: expected %d doubles (m, r, Ic), got shape %s" % (OBJECT_DOUBLES, obj.shape))
+    return obj
 
 
 def component_indices(components):
