@@ -136,6 +136,33 @@ int tbd_contact_wrench_terms(const double *model_host, int nv, const double *fra
                              int M, const double *q, const double *qs, const double *qss, double *a, double *b,
                              double *c, void *stream);
 
+/* Lambda_v^-1 = J_v M(q)^-1 J_v^T: the inverse of the operational-space (Khatib) inertia of the origin of frame_host
+ * for linear motion, 3x3 row-major, for M points, one thread per point.  J_v (3 x nv) maps qd to the world velocity
+ * of the frame origin, M(q) is the joint-space mass matrix of the whole tree.  The robot's effective mass at the
+ * origin in the unit direction u is m_R(u) = 1 / (u^T Lambda_v^-1 u).  Expressed in the frame's reference axes:
+ *   TBD_LOCAL_WORLD_ALIGNED   Lambda_v^-1 as is (world axes)
+ *   TBD_LOCAL                 R_f^T Lambda_v^-1 R_f
+ * Computed as M = L L^T (Cholesky, M from the composite-rigid-body algorithm), Y = L^-1 J_v^T, Lambda_v^-1 = Y^T Y:
+ * symmetric and positive semi-definite by construction; 0 for a frame on the base.  Where a Cholesky pivot is not
+ * positive (M singular or not finite at that q), all nine entries of that point are NaN.
+ *   q [M][nv]; Linv [M][9].  TB_ERR_UNSUPPORTED for a TBD_WORLD frame; otherwise the checks of tbd_frame_velocity. */
+int tbd_frame_inverse_inertia(const double *model_host, int nv, const double *frame_host, int M, const double *q,
+                              double *Linv, void *stream);
+
+/* The row of CollisionEnergyConstraint: the energy a collision at the frame origin could transfer to a human body
+ * region of effective mass m_H = human_mass (ISO/TS 15066, Annex A), E = 1/2 mu |v|^2 with
+ * mu = (1/m_H + 1/m_R)^-1 and m_R the robot's effective mass in the direction of v, is b s'^2 along a path, with
+ *   v = the world linear velocity of the frame origin at (q, qs = q')   (tbd_frame_velocity, first three entries)
+ *   vv = v.v;  w = v.(Lambda_v^-1 v), Lambda_v^-1 v row by row;  b = 0.5 * vv * vv / (vv / m_H + w)
+ * each sum left to right, and b = +0 where vv == 0 and w is not NaN.  m_H = +inf gives the robot-only energy
+ * 1/2 m_R |v|^2.  Bit-identical to tbd_frame_inverse_inertia and tbd_frame_velocity with the frame's reference-frame
+ * field set to TBD_LOCAL_WORLD_ALIGNED, followed by those operations; the field of frame_host (+13) is ignored.  NaN
+ * where Lambda_v^-1 is NaN.
+ *   q, qs [M][nv]; b [M].  TB_ERR_ARG for human_mass not > 0 (NaN included); otherwise the checks of
+ *   tbd_frame_velocity. */
+int tbd_collision_energy_terms(const double *model_host, int nv, const double *frame_host, double human_mass, int M,
+                               const double *q, const double *qs, double *b, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -8,10 +8,11 @@ from .joint_torque import JointTorqueConstraint
 from .cartesian_velocity_norm import CartesianVelocityNorm
 from .cartesian_acceleration import CartesianAccelerationConstraint
 from .contact_stability import ContactStabilityConstraint, contact_wrench_cone
+from .collision_energy import CollisionEnergyConstraint
 from .conic_constraint import ConicConstraint, RobustLinearConstraint
 
 __all__ = ["ConstraintType", "DiscretizationType", "Constraint", "LinearConstraint",
            "canlinear_colloc_to_interpolate", "JointAccelerationConstraint", "JointVelocityConstraint", "JointVelocityConstraintVarying",
            "SecondOrderConstraint", "JointTorqueConstraint", "CartesianVelocityNorm", "CartesianAccelerationConstraint",
-           "ContactStabilityConstraint", "contact_wrench_cone", "RecordContext", "ConicConstraint",
+           "ContactStabilityConstraint", "contact_wrench_cone", "CollisionEnergyConstraint", "RecordContext", "ConicConstraint",
            "RobustLinearConstraint"]

@@ -124,19 +124,28 @@ class CartesianVelocityNorm(LinearConstraint):
         if not self._device():
             return super(CartesianVelocityNorm, self).append_records(ctx, records, R_total, row0)
         self._check_batch(ctx)
-        torch = engine.torch_mod()
-        bp = ctx.bpath
-        B, G, dof = ctx.B, ctx.G, bp.dof
-        q = bp.eval_device(ctx.d_grid, 0).reshape(B * G, dof)
-        qs = bp.eval_device(ctx.d_grid, 1).reshape(B * G, dof)
-        b = self.compute_velocity.velocity_norm_terms(q, qs, self.S).reshape(B, G, 1)
-        # c = 0 - limit, not -limit: a zero limit gives +0 like the reference's F.c - g = 1 * 0 - 0
-        if self._path_limits is None:
-            c = torch.full((B, G, 1), 0.0 - self.limit, dtype=torch.float64, device=ctx.device)
-        else:
-            lim = engine.as_device(0.0 - self._path_limits[ctx.lo:ctx.hi], ctx.device)
-            c = lim.reshape(B, 1, 1).expand(B, G, 1).contiguous()
-        a = torch.zeros_like(b)
-        F = engine.as_device(np.ones((1, 1)), ctx.device)
-        g = engine.as_device(np.zeros(1), ctx.device)
-        engine.rows_canlinear(a, b, c, F, g, 0, ctx.d_grid, self._interp(), records, R_total, row0)
+        append_sd2_rows(ctx, lambda q, qs: self.compute_velocity.velocity_norm_terms(q, qs, self.S), self.limit,
+                        self._path_limits, self._interp(), records, R_total, row0)
+
+
+def append_sd2_rows(ctx, terms, limit, path_limits, interp, records, R_total, row0):
+    """The device rows of a limit b(q, q') s'^2 <= limit: ONE `terms(q, qs) -> b (B G,)` call on q, q' of the B x G
+    gridpoints of `ctx`, then a = 0, b, c = 0 - limit (a float, or path_limits (Bfull,) sliced to the context) with
+    F = [1], g = [0] through tb_rows_canlinear, with the interpolation lift if `interp`.  Shared by the device routes
+    of CartesianVelocityNorm and CollisionEnergyConstraint."""
+    torch = engine.torch_mod()
+    bp = ctx.bpath
+    B, G, dof = ctx.B, ctx.G, bp.dof
+    q = bp.eval_device(ctx.d_grid, 0).reshape(B * G, dof)
+    qs = bp.eval_device(ctx.d_grid, 1).reshape(B * G, dof)
+    b = terms(q, qs).reshape(B, G, 1)
+    # c = 0 - limit, not -limit: a zero limit gives +0 like the reference's F.c - g = 1 * 0 - 0
+    if path_limits is None:
+        c = torch.full((B, G, 1), 0.0 - limit, dtype=torch.float64, device=ctx.device)
+    else:
+        lim = engine.as_device(0.0 - path_limits[ctx.lo:ctx.hi], ctx.device)
+        c = lim.reshape(B, 1, 1).expand(B, G, 1).contiguous()
+    a = torch.zeros_like(b)
+    F = engine.as_device(np.ones((1, 1)), ctx.device)
+    g = engine.as_device(np.zeros(1), ctx.device)
+    engine.rows_canlinear(a, b, c, F, g, 0, ctx.d_grid, interp, records, R_total, row0)

@@ -24,6 +24,12 @@
 // Both run frame_acceleration<NS, true>, which also hands out the frame's orientation and angular velocity, and then
 // contact_wrench.
 //
+//   frame_inverse_inertia_kernel   Lambda_v^-1 = J_v M(q)^-1 J_v^T of a frame origin (3x3), one thread per point;
+//   collision_energy_terms_kernel  b = 1/2 |v|^4 / (|v|^2 / m_H + v^T Lambda_v^-1 v) at (q, q'): the row of
+//                                  CollisionEnergyConstraint, one thread per point.
+// Both run frame_inverse_inertia: the composite-rigid-body mass matrix of the whole tree in per-thread local arrays,
+// its Cholesky factor and a forward substitution; the terms kernel adds frame_velocity.
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -483,6 +489,196 @@ contact_wrench_terms_kernel(const __grid_constant__ DynModel m, const __grid_con
   for (int j = 0; j < 6; ++j) { c[r + j] = y[0][j]; a[r + j] = y[1][j] - y[0][j]; b[r + j] = y[2][j] - y[0][j]; }
 }
 
+// Lambda_v^-1 = J_v M(q)^-1 J_v^T (3x3 row-major) of the origin of frame f at q, in world axes, or in frame axes
+// R_f^T (.) R_f when f.ref is TBD_LOCAL.  False, with every entry NaN, where a Cholesky pivot of M is not positive.
+//   J_v     the chain walk of frame_velocity on the transforms X: column k is s_k x (p_f - o_k) (revolute) or s_k
+//           (prismatic) for the bodies on f's chain, 0 elsewhere (s_k the world joint axis, o_k the body origin);
+//   M(q)    the composite-rigid-body algorithm in body coordinates: every body's inertia (m, h = m c, Io about the
+//           body origin) is folded into its parent's, then F = Ic_k S_k is carried up to the root, M_kj = S_j^T F;
+//   M = L L^T in place (packed lower triangle), Y = L^-1 J_v^T by forward substitution, Lambda_v^-1 = Y^T Y.
+// Every sum is taken left to right.  M couples all bodies, so the whole tree is walked, not only f's chain.
+__device__ bool frame_inverse_inertia(const DynModel &m, const DynFrame &f, const int nv, const double *__restrict__ q,
+                                      double *Linv) {
+  double X[NB][12], ic[NB][10], L[NB * (NB + 1) / 2], Y[NB][3];
+  joint_transforms(m, nv, q, X);
+  // J_v^T into Y: world placement of f's chain, joint axes and origins
+  double Rw[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0}, pw[3] = {0.0, 0.0, 0.0};
+  double s[NB][3], o[NB][3];
+  for (int k = 0; k < nv; ++k)
+    for (int j = 0; j < 3; ++j) Y[k][j] = 0.0;
+  for (int i = 0; i < f.n; ++i) {
+    const int k = f.chain[i];
+    const double *R = X[k], *p = X[k] + 9;
+    double d[3], Rn[9];
+    mul3(Rw, p, d);
+    for (int j = 0; j < 3; ++j) pw[j] = pw[j] + d[j];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) Rn[3 * r + c] = Rw[3 * r] * R[c] + Rw[3 * r + 1] * R[3 + c] + Rw[3 * r + 2] * R[6 + c];
+    for (int j = 0; j < 9; ++j) Rw[j] = Rn[j];
+    mul3(Rw, m.body[k] + 2, s[i]);
+    for (int j = 0; j < 3; ++j) o[i][j] = pw[j];
+  }
+  double pf[3], d[3];
+  mul3(Rw, f.p, d);
+  for (int j = 0; j < 3; ++j) pf[j] = pw[j] + d[j];
+  for (int i = 0; i < f.n; ++i) {
+    const int k = f.chain[i];
+    if (m.body[k][1] == TBD_REVOLUTE) {
+      const double r[3] = {pf[0] - o[i][0], pf[1] - o[i][1], pf[2] - o[i][2]};
+      cross3(s[i], r, Y[k]);
+    } else {
+      for (int j = 0; j < 3; ++j) Y[k][j] = s[i][j];
+    }
+  }
+  // composite inertias: (m, h, Io = Ixx, Ixy, Ixz, Iyy, Iyz, Izz about the body origin), body coordinates
+  for (int k = 0; k < nv; ++k) {
+    const double *bd = m.body[k];
+    const double mass = bd[17], *c = bd + 18, *Ic = bd + 21;
+    double *e = ic[k];
+    e[0] = mass;
+    for (int j = 0; j < 3; ++j) e[1 + j] = mass * c[j];
+    // Io = Ic + m (|c|^2 I - c c^T)
+    const double cc = c[0] * c[0] + c[1] * c[1] + c[2] * c[2];
+    e[4] = Ic[0] + mass * (cc - c[0] * c[0]);
+    e[5] = Ic[1] - mass * (c[0] * c[1]);
+    e[6] = Ic[2] - mass * (c[0] * c[2]);
+    e[7] = Ic[3] + mass * (cc - c[1] * c[1]);
+    e[8] = Ic[4] - mass * (c[1] * c[2]);
+    e[9] = Ic[5] + mass * (cc - c[2] * c[2]);
+  }
+  for (int k = nv - 1; k >= 0; --k) {
+    const int par = (int)m.body[k][0];
+    if (par < 0) continue;
+    // parent coordinates: h' = R h + m p;  Io' = R Io R^T + m (|p|^2 I - p p^T) + 2 (p.hr) I - p hr^T - hr p^T
+    const double *R = X[k], *p = X[k] + 9, *e = ic[k];
+    double hr[3], A[9], B[9];
+    mul3(R, e + 1, hr);
+    const double I3[9] = {e[4], e[5], e[6], e[5], e[7], e[8], e[6], e[8], e[9]};
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) A[3 * r + c] = R[3 * r] * I3[c] + R[3 * r + 1] * I3[3 + c] + R[3 * r + 2] * I3[6 + c];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) B[3 * r + c] = A[3 * r] * R[3 * c] + A[3 * r + 1] * R[3 * c + 1] + A[3 * r + 2] * R[3 * c + 2];
+    const double pp = p[0] * p[0] + p[1] * p[1] + p[2] * p[2];
+    const double ph = p[0] * hr[0] + p[1] * hr[1] + p[2] * hr[2];
+    const double diag = e[0] * pp + 2.0 * ph;
+    double *t = ic[par];
+    t[0] = t[0] + e[0];
+    for (int j = 0; j < 3; ++j) t[1 + j] = t[1 + j] + (hr[j] + e[0] * p[j]);
+    const int rr[6] = {0, 0, 0, 1, 1, 2}, cc[6] = {0, 1, 2, 1, 2, 2};
+    for (int j = 0; j < 6; ++j) {
+      const int r = rr[j], c = cc[j];
+      double v = B[3 * r + c] - (e[0] * p[r] * p[c] + p[r] * hr[c] + hr[r] * p[c]);
+      if (r == c) v = v + diag;
+      t[4 + j] = t[4 + j] + v;
+    }
+  }
+  // M: F = Ic_k S_k = (n, f) about body k's origin, carried up the tree
+  for (int k = 0; k < nv; ++k) {
+    const double *bd = m.body[k], *ax = bd + 2, *e = ic[k];
+    double n[3], fl[3];
+    if (bd[1] == TBD_REVOLUTE) {
+      mul_inertia(e + 4, ax, n);
+      cross3(ax, e + 1, fl);
+    } else {
+      cross3(e + 1, ax, n);
+      for (int j = 0; j < 3; ++j) fl[j] = e[0] * ax[j];
+    }
+    int j = k;
+    for (;;) {
+      const double *bj = m.body[j], *aj = bj + 2;
+      const double *g = bj[1] == TBD_REVOLUTE ? n : fl;
+      L[k * (k + 1) / 2 + j] = aj[0] * g[0] + aj[1] * g[1] + aj[2] * g[2];
+      const int par = (int)bj[0];
+      if (par < 0) break;
+      const double *R = X[j], *p = X[j] + 9;
+      double Rf[3], Rn[3], u[3];
+      mul3(R, fl, Rf);
+      mul3(R, n, Rn);
+      cross3(p, Rf, u);
+      for (int i = 0; i < 3; ++i) { n[i] = Rn[i] + u[i]; fl[i] = Rf[i]; }
+      for (int i = par + 1; i < j; ++i) L[k * (k + 1) / 2 + i] = 0.0;   // bodies off k's chain to the root
+      j = par;
+    }
+    for (int i = 0; i < j; ++i) L[k * (k + 1) / 2 + i] = 0.0;
+  }
+  // M = L L^T (packed lower triangle, row k at k (k + 1) / 2), then Y = L^-1 J_v^T
+  bool ok = true;
+  for (int j = 0; j < nv && ok; ++j) {
+    double *Lj = L + j * (j + 1) / 2;
+    double dd = Lj[j];
+    for (int k = 0; k < j; ++k) dd = dd - Lj[k] * Lj[k];
+    if (!(dd > 0.0)) { ok = false; break; }
+    Lj[j] = sqrt(dd);
+    for (int i = j + 1; i < nv; ++i) {
+      double *Li = L + i * (i + 1) / 2;
+      double v = Li[j];
+      for (int k = 0; k < j; ++k) v = v - Li[k] * Lj[k];
+      Li[j] = v / Lj[j];
+    }
+  }
+  if (!ok) {
+    for (int j = 0; j < 9; ++j) Linv[j] = nan("");
+    return false;
+  }
+  for (int i = 0; i < nv; ++i) {
+    const double *Li = L + i * (i + 1) / 2;
+    for (int c = 0; c < 3; ++c) {
+      double v = Y[i][c];
+      for (int k = 0; k < i; ++k) v = v - Li[k] * Y[k][c];
+      Y[i][c] = v / Li[i];
+    }
+  }
+  double W[9];
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) {
+      double v = Y[0][r] * Y[0][c];
+      for (int i = 1; i < nv; ++i) v = v + Y[i][r] * Y[i][c];
+      W[3 * r + c] = v;
+    }
+  if (f.ref == TBD_LOCAL) {
+    double Rf[9], T[9];
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) Rf[3 * r + c] = Rw[3 * r] * f.R[c] + Rw[3 * r + 1] * f.R[3 + c] + Rw[3 * r + 2] * f.R[6 + c];
+    for (int r = 0; r < 3; ++r)                                        // T = W R_f
+      for (int c = 0; c < 3; ++c) T[3 * r + c] = W[3 * r] * Rf[c] + W[3 * r + 1] * Rf[3 + c] + W[3 * r + 2] * Rf[6 + c];
+    for (int r = 0; r < 3; ++r)                                        // R_f^T T
+      for (int c = 0; c < 3; ++c) Linv[3 * r + c] = Rf[r] * T[c] + Rf[3 + r] * T[3 + c] + Rf[6 + r] * T[6 + c];
+  } else {
+    for (int j = 0; j < 9; ++j) Linv[j] = W[j];
+  }
+  return true;
+}
+
+__global__ void __launch_bounds__(THREADS)
+frame_inverse_inertia_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame f, const int nv,
+                             const int M, const double *__restrict__ q, double *__restrict__ Linv) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  double W[9];
+  frame_inverse_inertia(m, f, nv, q + (size_t)pt * nv, W);
+  for (int j = 0; j < 9; ++j) Linv[(size_t)pt * 9 + j] = W[j];
+}
+
+// b = 1/2 vv^2 / (vv / m_H + w) with v the world linear velocity of f at (q, q'), vv = v.v, w = v.(Lambda_v^-1 v)
+// (Lambda_v^-1 v row by row), each sum left to right; b = +0 where vv == 0 and w is not NaN.  f.ref is
+// TBD_LOCAL_WORLD_ALIGNED (set on the host).
+__global__ void __launch_bounds__(THREADS)
+collision_energy_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame f, const int nv,
+                              const double human_mass, const int M, const double *__restrict__ q,
+                              const double *__restrict__ qs, double *__restrict__ b) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double W[9], x[6];
+  frame_inverse_inertia(m, f, nv, q + o, W);
+  frame_velocity(m, f, q + o, qs + o, x);
+  const double vv = x[0] * x[0] + x[1] * x[1] + x[2] * x[2];
+  double Wv[3];
+  for (int i = 0; i < 3; ++i) Wv[i] = W[3 * i] * x[0] + W[3 * i + 1] * x[1] + W[3 * i + 2] * x[2];
+  const double w = x[0] * Wv[0] + x[1] * Wv[1] + x[2] * Wv[2];
+  b[pt] = (vv == 0.0 && !isnan(w)) ? 0.0 : 0.5 * vv * vv / (vv / human_mass + w);
+}
+
 int launch_status(const char *what) {
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -710,4 +906,52 @@ extern "C" int tbd_contact_wrench_terms(const double *model_host, int nv, const 
     return rc;
   contact_wrench_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, o, nv, M, q, qs, qss, a, b, c);
   return launch_status("tbd_contact_wrench_terms");
+}
+
+namespace {
+// load_model, then load_frame with the reference-frame field set to `ref` (or as given when ref < 0).
+int load_energy(const double *model_host, const int nv, const double *frame_host, const int M, const int ref,
+                tb::DynModel *m, tb::DynFrame *f, const char *what) {
+  using namespace tb;
+  if (const int rc = load_model(model_host, nv, M, m, what)) return rc;
+  double frame[TBD_FRAME_DOUBLES];
+  for (int j = 0; j < TBD_FRAME_DOUBLES; ++j) frame[j] = frame_host[j];
+  if (ref >= 0) frame[13] = ref;
+  return load_frame(frame, *m, nv, nullptr, f, what);
+}
+}  // namespace
+
+extern "C" int tbd_frame_inverse_inertia(const double *model_host, int nv, const double *frame_host, int M,
+                                         const double *q, double *Linv, void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !q || !Linv) { set_error("tbd_frame_inverse_inertia: null pointer"); return TB_ERR_ARG; }
+  DynModel m;
+  DynFrame f;
+  if (const int rc = load_energy(model_host, nv, frame_host, M, -1, &m, &f, "tbd_frame_inverse_inertia")) return rc;
+  if (f.ref == TBD_WORLD) {
+    set_error("tbd_frame_inverse_inertia: the world reference frame is not supported (use local or local_world_aligned)");
+    return TB_ERR_UNSUPPORTED;
+  }
+  frame_inverse_inertia_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, Linv);
+  return launch_status("tbd_frame_inverse_inertia");
+}
+
+extern "C" int tbd_collision_energy_terms(const double *model_host, int nv, const double *frame_host, double human_mass,
+                                          int M, const double *q, const double *qs, double *b, void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !q || !qs || !b) {
+    set_error("tbd_collision_energy_terms: null pointer");
+    return TB_ERR_ARG;
+  }
+  if (!(human_mass > 0.0)) {
+    set_error("tbd_collision_energy_terms: human_mass %g must be positive (inf allowed)", human_mass);
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynFrame f;
+  if (const int rc = load_energy(model_host, nv, frame_host, M, TBD_LOCAL_WORLD_ALIGNED, &m, &f,
+                                 "tbd_collision_energy_terms"))
+    return rc;
+  collision_energy_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, human_mass, M, q, qs, b);
+  return launch_status("tbd_collision_energy_terms");
 }

@@ -14,7 +14,10 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     pc = CartesianVelocityNorm(tcp, S, limit)                 # tool-speed limit, batched on the device
     acc = tcp.acceleration(q, qd, qdd)                        # (M, 6) classical frame accelerations, one launch
     pc = CartesianAccelerationConstraint(tcp, alim)           # tool-acceleration limit, batched on the device
-    pc = ContactStabilityConstraint(tray, m, com, I, (X, Y), mu)  # an object carried on a tray must not slide or tip"""
+    pc = ContactStabilityConstraint(tray, m, com, I, (X, Y), mu)  # an object carried on a tray must not slide or tip
+    Linv = tcp.inverse_inertia(q)                             # (M, 3, 3) J_v M(q)^-1 J_v^T, one launch
+    pc = CollisionEnergyConstraint(tcp, E_max, m_H)           # collision energy next to people (ISO/TS 15066)
+    loaded = model.with_payload("flange", m, com, I)          # a rigidly held payload folded into the flange's body"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -116,6 +119,51 @@ class RigidBodyModel(object):
     def torque_limits(self):
         """(nv, 2) [-effort, effort] per joint, the tau_lim of JointTorqueConstraint (+-inf where the URDF has none)."""
         return np.stack([-self.effort_limit, self.effort_limit], axis=1)
+
+    def with_payload(self, frame, mass, com, inertia):
+        """A new model with a payload rigidly held by `frame` (a frame name or a RigidBodyFrame of this model) folded
+        into the frame's body by the parallel-axis theorem: mass > 0, centre of mass com (3,) and rotational inertia
+        (6,) = Ixx, Ixy, Ixz, Iyy, Iyz, Izz about it (positive semi-definite), both in the frame's axes.  Joint names,
+        limits, gravity and the frame table are kept."""
+        if isinstance(frame, RigidBodyFrame):
+            if frame.model is not self:
+                raise ValueError("with_payload: the frame %r belongs to another model" % frame.name)
+            body, R, p = frame.body, frame.R, frame.p
+        else:
+            if frame not in self.frames:
+                raise ValueError("RigidBodyModel has no frame %r (frames: %s)" % (frame, sorted(self.frames)))
+            body, R, p = self.frames[frame]
+        mass, com, I = _rigid_inertia("with_payload", mass, com, inertia)
+        if body < 0:
+            raise ValueError("with_payload: frame %r is on the base, where a payload moves no joint" % (frame,))
+        bodies = self.packed[3:].reshape(self.nv, BODY_DOUBLES).copy()
+        bd = bodies[body]
+        mb, cb = bd[17], bd[18:21].copy()
+        Ib = _inertia3(bd[21:27])
+        cp, Ip = R @ com + p, R @ I @ R.T                      # the payload in body coordinates
+        m = mb + mass
+        c = (mb * cb + mass * cp) / m
+        Ic = np.zeros((3, 3))
+        for pm, pc, pI in ((mb, cb, Ib), (mass, cp, Ip)):
+            d = pc - c
+            Ic = Ic + pI + pm * (np.dot(d, d) * np.eye(3) - np.outer(d, d))
+        bd[17], bd[18:21] = m, c
+        bd[21:27] = [Ic[0, 0], Ic[0, 1], Ic[0, 2], Ic[1, 1], Ic[1, 2], Ic[2, 2]]
+        return RigidBodyModel(bodies[:, 0], bodies[:, 1], bodies[:, 2:5], bodies[:, 5:14].reshape(-1, 3, 3),
+                              bodies[:, 14:17], bodies[:, 17], bodies[:, 18:21], bodies[:, 21:27], self.gravity,
+                              joint_names=self.joint_names, effort_limit=self.effort_limit.copy(),
+                              velocity_limit=self.velocity_limit.copy(), frames=self.frames)
+
+    def inertialess_joints(self):
+        """Names of the moving joints that move no inertia: the joint's body and all its descendants have zero mass and
+        zero rotational inertia, so the mass matrix M(q) is singular at every q."""
+        bodies = self.packed[3:].reshape(self.nv, BODY_DOUBLES)
+        empty = [bool(bd[17] == 0 and not np.any(bd[21:27])) for bd in bodies]
+        for k in range(self.nv - 1, -1, -1):                   # children come after their parent
+            par = int(bodies[k, 0])
+            if par >= 0 and not empty[k]:
+                empty[par] = False
+        return [self.joint_names[k] for k in range(self.nv) if empty[k]]
 
     # ---- evaluation on the GPU ----------------------------------------------------------------------------------
     def _model_ptr(self):
@@ -427,6 +475,69 @@ class RigidBodyFrame(object):
                                                                 _lib.ptr(b), _lib.ptr(c), _lib.stream_ptr()),
                        "tbd_contact_wrench_terms")
         return a, b, c
+
+    def inverse_inertia(self, q):
+        """Lambda_v^-1 = J_v M(q)^-1 J_v^T of the frame origin: the inverse operational-space inertia for linear motion
+        (Khatib), whose quadratic form u^T Lambda_v^-1 u = 1 / m_R(u) gives the robot's effective mass in the unit
+        direction u.  "local_world_aligned": world axes; "local": R_f^T Lambda_v^-1 R_f; "world" raises ValueError.
+        NaN where M(q) is singular.  CUDA tensors (M, nv) -> (M, 3, 3), one tbd_frame_inverse_inertia launch on the
+        current stream; numpy (nv,) -> (3, 3) or (M, nv) -> (M, 3, 3), through a device round trip."""
+        if self.reference_frame == "world":
+            raise ValueError("RigidBodyFrame %r: the inverse inertia is that of the frame origin; the \"world\" "
+                             "reference frame is not supported (use \"local\" or \"local_world_aligned\")" % self.name)
+        torch = _lib.require_cuda()
+        m = self.model
+        if isinstance(q, torch.Tensor) and q.is_cuda:
+            q, = m._prepare(torch, q)
+            L = torch.empty((q.shape[0], 3, 3), dtype=torch.float64, device=q.device)
+            with torch.cuda.device(q.device):
+                _lib.check(_lib_dyn.load().tbd_frame_inverse_inertia(m._model_ptr(), m.nv, self._frame_ptr(),
+                                                                     q.shape[0], _lib.ptr(q), _lib.ptr(L),
+                                                                     _lib.stream_ptr()),
+                           "tbd_frame_inverse_inertia")
+            return L
+        q = np.asarray(q, dtype=np.float64)
+        L = self.inverse_inertia(torch.as_tensor(np.atleast_2d(q), device="cuda")).cpu().numpy()
+        return L[0] if q.ndim == 1 else L
+
+    def collision_energy_terms(self, q, qs, human_mass):
+        """b = 1/2 |v|^4 / (|v|^2 / m_H + v^T Lambda_v^-1 v), v the world linear velocity of the frame origin at
+        (q, qs = q'), m_H = human_mass (> 0, inf allowed): the collision energy E = b s'^2 of
+        CollisionEnergyConstraint, for CUDA tensors (M, nv) -> (M,): one tbd_collision_energy_terms launch.  The
+        reference frame is ignored."""
+        torch = _lib.require_cuda()
+        m = self.model
+        q, qs = m._prepare(torch, q, qs)
+        b = torch.empty(q.shape[0], dtype=torch.float64, device=q.device)
+        with torch.cuda.device(q.device):
+            _lib.check(_lib_dyn.load().tbd_collision_energy_terms(m._model_ptr(), m.nv, self._frame_ptr(),
+                                                                  float(human_mass), q.shape[0], _lib.ptr(q),
+                                                                  _lib.ptr(qs), _lib.ptr(b), _lib.stream_ptr()),
+                       "tbd_collision_energy_terms")
+        return b
+
+
+def _inertia3(I6):
+    Ixx, Ixy, Ixz, Iyy, Iyz, Izz = I6
+    return np.array([[Ixx, Ixy, Ixz], [Ixy, Iyy, Iyz], [Ixz, Iyz, Izz]], dtype=np.float64)
+
+
+def _rigid_inertia(what, mass, com, inertia):
+    """(mass, com (3,), inertia 3x3) of a rigid body, or ValueError: finite, mass > 0, inertia positive semi-definite."""
+    mass = np.asarray(mass, dtype=np.float64)
+    com = np.asarray(com, dtype=np.float64)
+    inertia = np.asarray(inertia, dtype=np.float64)
+    if mass.shape != () or com.shape != (3,) or inertia.shape != (6,):
+        raise ValueError("%s: expected a scalar mass, com (3,) and inertia (6,); got shapes %s, %s, %s"
+                         % (what, mass.shape, com.shape, inertia.shape))
+    if not (np.isfinite(mass) and np.isfinite(com).all() and np.isfinite(inertia).all()):
+        raise ValueError("%s: mass, com and inertia must be finite" % what)
+    if not mass > 0:
+        raise ValueError("%s: mass %r must be positive" % (what, float(mass)))
+    I = _inertia3(inertia)
+    if np.linalg.eigvalsh(I).min() < -1e-12 * max(1e-300, np.abs(I).max()):
+        raise ValueError("%s: the inertia matrix is not positive semi-definite" % what)
+    return float(mass), com, I
 
 
 OBJECT_DOUBLES = 10
