@@ -58,6 +58,7 @@ extern "C" {
 #define TBD_LOCAL 1
 #define TBD_LOCAL_WORLD_ALIGNED 2
 #define TBD_OBJECT_DOUBLES 10
+#define TBD_BASE_DOUBLES 4
 
 int tbd_version(void);
 
@@ -162,6 +163,35 @@ int tbd_frame_inverse_inertia(const double *model_host, int nv, const double *fr
  *   tbd_frame_velocity. */
 int tbd_collision_energy_terms(const double *model_host, int nv, const double *frame_host, double human_mass, int M,
                                const double *q, const double *qs, double *b, void *stream);
+
+/* w = the wrench [f(3); tau(3)] the support exerts on the whole robot, at (q, qd, qdd) for M points, one thread per
+ * point (toppra_b200.constraint.SupportStabilityConstraint).  The support frame frame_host is a frame on the base
+ * (body -1): its origin lies on the support plane and its z axis is the support normal, pointing into the robot.
+ * base_host is a HOST array of TBD_BASE_DOUBLES doubles describing the static base, which the model's bodies leave
+ * out:
+ *
+ *   +0              mass m_b >= 0
+ *   +1  .. +3       c_b: centre of mass, base coordinates
+ *
+ * With R_s, p_s the support frame's placement in base coordinates, g the model's gravity and (f_k, n_k) the force of
+ * the recursive Newton-Euler pass (gravity as base acceleration -g) that each root child k would hand to the base:
+ *   f_b = sum_k R_k f_k;  n_b = sum_k (R_k n_k + p_k x R_k f_k);  f_b += -m_b g;  n_b += c_b x (-m_b g)
+ *   w = [R_s^T f_b; R_s^T (n_b - p_s x f_b)]
+ * The wrench is always in support axes: the reference-frame field of frame_host (+13) is ignored.  The zero-moment
+ * point (centre of pressure) is (-tau_y / f_z, tau_x / f_z) in support axes.
+ *   q, qd, qdd [M][nv]; w [M][6].  TB_ERR_ARG for a frame whose body is not -1, a null or non-finite base or m_b < 0;
+ *   otherwise the model and frame checks of tbd_frame_velocity. */
+int tbd_support_wrench(const double *model_host, int nv, const double *frame_host, const double *base_host, int M,
+                       const double *q, const double *qd, const double *qdd, double *w, void *stream);
+
+/* The three terms of SecondOrderConstraint with the support wrench as inverse dynamics, in one launch; the joint
+ * transforms are computed once per point and shared by the three passes:
+ *   c = w(q, 0, 0);  a = w(q, 0, qs) - c;  b = w(q, qs, qss) - c
+ * Bit-identical to three tbd_support_wrench launches followed by the two subtractions.
+ *   q, qs, qss [M][nv]; a, b, c [M][6].  The checks of tbd_support_wrench. */
+int tbd_support_wrench_terms(const double *model_host, int nv, const double *frame_host, const double *base_host,
+                             int M, const double *q, const double *qs, const double *qss, double *a, double *b,
+                             double *c, void *stream);
 
 #ifdef __cplusplus
 }

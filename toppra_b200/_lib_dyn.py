@@ -27,6 +27,9 @@ _PROTOS = {
                                  _int),
     "tbd_frame_inverse_inertia": ([_c_dp, _int, _c_dp, _int, _c_dp, _c_dp, _stream], _int),
     "tbd_collision_energy_terms": ([_c_dp, _int, _c_dp, ctypes.c_double, _int, _c_dp, _c_dp, _c_dp, _stream], _int),
+    "tbd_support_wrench": ([_c_dp, _int, _c_dp, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
+    "tbd_support_wrench_terms": ([_c_dp, _int, _c_dp, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream],
+                                 _int),
 }
 
 _dlib = None

@@ -679,6 +679,80 @@ collision_energy_terms_kernel(const __grid_constant__ DynModel m, const __grid_c
   b[pt] = (vv == 0.0 && !isnan(w)) ? 0.0 : 0.5 * vv * vv / (vv / human_mass + w);
 }
 
+// The static base under the moving tree (include/toppra_b200_dyn.h): mass and centre of mass in base coordinates.
+struct DynBase {
+  double mass, c[3];
+};
+
+// The wrench [f; tau] the support exerts on the whole robot, at the origin of the support frame s (a frame on the base)
+// in its axes, from the forces f of a finished rnea_pass.  rnea_pass carries each body's force up to its parent and
+// drops it at the base, so f[k] of a root child k is then the wrench of k's whole subtree about k's origin, in k's
+// coordinates:
+//   f_b = sum_k R_k f_k,  n_b = sum_k R_k n_k + p_k x R_k f_k   (root children k, in base coordinates)
+//   f_b += -m_b g;  n_b += c_b x (-m_b g)                       (the static base's weight)
+//   w = [R_s^T f_b; R_s^T (n_b - p_s x f_b)]
+// Every sum is taken in body order, left to right.
+__device__ __forceinline__ void support_wrench(const DynModel &m, const DynFrame &s, const DynBase &base, const int nv,
+                                               const double (*X)[12], const double (*f)[6], double *out) {
+  double fb[3] = {0.0, 0.0, 0.0}, nb[3] = {0.0, 0.0, 0.0};
+  for (int k = 0; k < nv; ++k) {
+    if ((int)m.body[k][0] >= 0) continue;
+    const double *R = X[k], *p = X[k] + 9;
+    double Rf[3], Rn[3], u[3];
+    mul3(R, f[k] + 3, Rf);
+    mul3(R, f[k], Rn);
+    cross3(p, Rf, u);
+    for (int i = 0; i < 3; ++i) { nb[i] = nb[i] + Rn[i] + u[i]; fb[i] = fb[i] + Rf[i]; }
+  }
+  double wb[3], u[3], t[3];
+  for (int i = 0; i < 3; ++i) wb[i] = -(base.mass * m.g[i]);
+  cross3(base.c, wb, u);
+  for (int i = 0; i < 3; ++i) { nb[i] = nb[i] + u[i]; fb[i] = fb[i] + wb[i]; }
+  cross3(s.p, fb, u);
+  for (int i = 0; i < 3; ++i) t[i] = nb[i] - u[i];
+  mul3t(s.R, fb, out);
+  mul3t(s.R, t, out + 3);
+}
+
+__global__ void __launch_bounds__(THREADS)
+support_wrench_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame s,
+                      const __grid_constant__ DynBase base, const int nv, const int M, const double *__restrict__ q,
+                      const double *__restrict__ qd, const double *__restrict__ qdd, double *__restrict__ w) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double X[NB][12], st[NB][12], f[NB][6], t[NB], y[6];
+  joint_transforms(m, nv, q + o, X);
+  rnea_pass(m, nv, X, qd + o, qdd + o, st, f, t);
+  support_wrench(m, s, base, nv, X, f, y);
+  for (int j = 0; j < 6; ++j) w[(size_t)pt * 6 + j] = y[j];
+}
+
+// c = w(q, 0, 0), a = w(q, 0, q') - c, b = w(q, q', q'') - c: the terms of SupportStabilityConstraint; the joint
+// transforms (and their sincos) are computed once per point and shared by the three passes.
+__global__ void __launch_bounds__(THREADS)
+support_wrench_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame s,
+                            const __grid_constant__ DynBase base, const int nv, const int M,
+                            const double *__restrict__ q, const double *__restrict__ qs, const double *__restrict__ qss,
+                            double *__restrict__ a, double *__restrict__ b, double *__restrict__ c) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double X[NB][12], st[NB][12], f[NB][6], zero[NB], t[NB], y0[6], y[6];
+  for (int k = 0; k < nv; ++k) zero[k] = 0.0;
+  joint_transforms(m, nv, q + o, X);
+  rnea_pass(m, nv, X, zero, zero, st, f, t);
+  support_wrench(m, s, base, nv, X, f, y0);
+  const size_t r = (size_t)pt * 6;
+  for (int j = 0; j < 6; ++j) c[r + j] = y0[j];
+  rnea_pass(m, nv, X, zero, qs + o, st, f, t);
+  support_wrench(m, s, base, nv, X, f, y);
+  for (int j = 0; j < 6; ++j) a[r + j] = y[j] - y0[j];
+  rnea_pass(m, nv, X, qs + o, qss + o, st, f, t);
+  support_wrench(m, s, base, nv, X, f, y);
+  for (int j = 0; j < 6; ++j) b[r + j] = y[j] - y0[j];
+}
+
 int launch_status(const char *what) {
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -954,4 +1028,61 @@ extern "C" int tbd_collision_energy_terms(const double *model_host, int nv, cons
     return rc;
   collision_energy_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, human_mass, M, q, qs, b);
   return launch_status("tbd_collision_energy_terms");
+}
+
+namespace {
+// load_model and load_frame with the frame's reference-frame field ignored (the support wrench is always in the
+// support's own axes); the support must be on the base.  Then the base: finite, with a non-negative mass.
+int load_support(const double *model_host, const int nv, const double *frame_host, const double *base_host,
+                 const int M, tb::DynModel *m, tb::DynFrame *s, tb::DynBase *base, const char *what) {
+  using namespace tb;
+  if (const int rc = load_model(model_host, nv, M, m, what)) return rc;
+  double frame[TBD_FRAME_DOUBLES];
+  for (int j = 0; j < TBD_FRAME_DOUBLES; ++j) frame[j] = frame_host[j];
+  frame[13] = TBD_LOCAL;
+  if (const int rc = load_frame(frame, *m, nv, nullptr, s, what)) return rc;
+  if (frame[0] != -1.0) {
+    set_error("%s: the support must be on the base (frame body %g, expected -1)", what, frame[0]);
+    return TB_ERR_ARG;
+  }
+  for (int j = 0; j < TBD_BASE_DOUBLES; ++j)
+    if (!std::isfinite(base_host[j])) { set_error("%s: base parameters are not finite", what); return TB_ERR_ARG; }
+  if (!(base_host[0] >= 0.0)) { set_error("%s: base mass %g must be non-negative", what, base_host[0]); return TB_ERR_ARG; }
+  base->mass = base_host[0];
+  for (int j = 0; j < 3; ++j) base->c[j] = base_host[1 + j];
+  return 0;
+}
+}  // namespace
+
+extern "C" int tbd_support_wrench(const double *model_host, int nv, const double *frame_host, const double *base_host,
+                                  int M, const double *q, const double *qd, const double *qdd, double *w,
+                                  void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !base_host || !q || !qd || !qdd || !w) {
+    set_error("tbd_support_wrench: null pointer");
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynFrame s;
+  DynBase base;
+  if (const int rc = load_support(model_host, nv, frame_host, base_host, M, &m, &s, &base, "tbd_support_wrench")) return rc;
+  support_wrench_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, s, base, nv, M, q, qd, qdd, w);
+  return launch_status("tbd_support_wrench");
+}
+
+extern "C" int tbd_support_wrench_terms(const double *model_host, int nv, const double *frame_host,
+                                        const double *base_host, int M, const double *q, const double *qs,
+                                        const double *qss, double *a, double *b, double *c, void *stream) {
+  using namespace tb;
+  if (!model_host || !frame_host || !base_host || !q || !qs || !qss || !a || !b || !c) {
+    set_error("tbd_support_wrench_terms: null pointer");
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynFrame s;
+  DynBase base;
+  if (const int rc = load_support(model_host, nv, frame_host, base_host, M, &m, &s, &base, "tbd_support_wrench_terms"))
+    return rc;
+  support_wrench_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, s, base, nv, M, q, qs, qss, a, b, c);
+  return launch_status("tbd_support_wrench_terms");
 }

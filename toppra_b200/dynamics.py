@@ -17,7 +17,10 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     pc = ContactStabilityConstraint(tray, m, com, I, (X, Y), mu)  # an object carried on a tray must not slide or tip
     Linv = tcp.inverse_inertia(q)                             # (M, 3, 3) J_v M(q)^-1 J_v^T, one launch
     pc = CollisionEnergyConstraint(tcp, E_max, m_H)           # collision energy next to people (ISO/TS 15066)
-    loaded = model.with_payload("flange", m, com, I)          # a rigidly held payload folded into the flange's body"""
+    loaded = model.with_payload("flange", m, com, I)          # a rigidly held payload folded into the flange's body
+    floor = model.frame("base_footprint")                     # a support frame on the base (z: the support normal)
+    w = floor.support_wrench(None, q, qd, qdd)                # (M, 6) the support's wrench on the whole robot, one launch
+    pc = SupportStabilityConstraint(floor, half_lengths=(X, Y), friction=mu)  # the robot must not tip over or slide"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -57,10 +60,12 @@ class RigidBodyModel(object):
     parent (nv,); joint_type (nv,) of "revolute" / "prismatic" (or 0 / 1); axis (nv, 3) in the joint frame;
     E (nv, 3, 3), r (nv, 3): placement of the joint frame in the parent frame at q = 0 (E maps body to parent
     coordinates); mass (nv,); com (nv, 3) in the body frame; inertia (nv, 6) = Ixx, Ixy, Ixz, Iyy, Iyz, Izz about the
-    centre of mass in the body frame; gravity (3,) in the base frame."""
+    centre of mass in the body frame; gravity (3,) in the base frame; base_mass >= 0 and base_com (3,), in base
+    coordinates, of the static base itself, which moves no joint and enters only the support wrench
+    (RigidBodyFrame.support_wrench)."""
 
     def __init__(self, parent, joint_type, axis, E, r, mass, com, inertia, gravity=(0.0, 0.0, -9.81), joint_names=None,
-                 effort_limit=None, velocity_limit=None, frames=None):
+                 effort_limit=None, velocity_limit=None, frames=None, base_mass=0.0, base_com=(0.0, 0.0, 0.0)):
         parent = np.asarray(parent, dtype=np.float64).reshape(-1)
         nv = parent.shape[0]
         if not 1 <= nv <= MAX_BODIES:
@@ -90,6 +95,7 @@ class RigidBodyModel(object):
         # name -> (body index, R, p): frames rigidly attached to a body (-1 = the base), in that body's coordinates
         self.frames = dict(frames) if frames is not None else {"body%d" % k: (k, np.eye(3), np.zeros(3))
                                                                for k in range(nv)}
+        self.base_mass, self.base_com = _base_inertia("RigidBodyModel", base_mass, base_com)
 
     @property
     def dof(self):
@@ -116,6 +122,10 @@ class RigidBodyModel(object):
         return RigidBodyFrame(self, name, body, R @ Ro, p + R @ np.asarray(xyz, dtype=np.float64).reshape(3),
                               reference_frame)
 
+    def packed_base(self):
+        """The packed base of include/toppra_b200_dyn.h: (base_mass, base_com)."""
+        return np.concatenate(([self.base_mass], self.base_com))
+
     def torque_limits(self):
         """(nv, 2) [-effort, effort] per joint, the tau_lim of JointTorqueConstraint (+-inf where the URDF has none)."""
         return np.stack([-self.effort_limit, self.effort_limit], axis=1)
@@ -124,7 +134,7 @@ class RigidBodyModel(object):
         """A new model with a payload rigidly held by `frame` (a frame name or a RigidBodyFrame of this model) folded
         into the frame's body by the parallel-axis theorem: mass > 0, centre of mass com (3,) and rotational inertia
         (6,) = Ixx, Ixy, Ixz, Iyy, Iyz, Izz about it (positive semi-definite), both in the frame's axes.  Joint names,
-        limits, gravity and the frame table are kept."""
+        limits, gravity, the frame table and the base's mass and centre of mass are kept."""
         if isinstance(frame, RigidBodyFrame):
             if frame.model is not self:
                 raise ValueError("with_payload: the frame %r belongs to another model" % frame.name)
@@ -152,7 +162,8 @@ class RigidBodyModel(object):
         return RigidBodyModel(bodies[:, 0], bodies[:, 1], bodies[:, 2:5], bodies[:, 5:14].reshape(-1, 3, 3),
                               bodies[:, 14:17], bodies[:, 17], bodies[:, 18:21], bodies[:, 21:27], self.gravity,
                               joint_names=self.joint_names, effort_limit=self.effort_limit.copy(),
-                              velocity_limit=self.velocity_limit.copy(), frames=self.frames)
+                              velocity_limit=self.velocity_limit.copy(), frames=self.frames, base_mass=self.base_mass,
+                              base_com=self.base_com)
 
     def inertialess_joints(self):
         """Names of the moving joints that move no inertia: the joint's body and all its descendants have zero mass and
@@ -220,8 +231,9 @@ class RigidBodyModel(object):
         revolute / continuous joints become revolute bodies, prismatic ones prismatic; fixed joints and the joints named
         in `locked_joints` (name -> position) fold their child link into the parent body (mass, centre of mass, inertia
         by the parallel-axis theorem).  DOF order is depth-first with children in file order; `joint_names` lists it.
-        floating, planar and unlocked mimic joints, a missing or ambiguous root and more than 16 moving bodies raise
-        ValueError."""
+        The root link and the links folded into it (e.g. locked wheels) make the static base: `base_mass` and
+        `base_com` (base coordinates).  floating, planar and unlocked mimic joints, a missing or ambiguous root and more
+        than 16 moving bodies raise ValueError."""
         text = urdf if urdf.lstrip().startswith("<") else open(urdf).read()
         robot = ET.fromstring(text)
         locked = dict(locked_joints or {})
@@ -322,10 +334,13 @@ class RigidBodyModel(object):
             mass.append(m)
             com.append(c)
             inertia.append([Ic[0, 0], Ic[0, 1], Ic[0, 2], Ic[1, 1], Ic[1, 2], Ic[2, 2]])
+        base_mass = sum(pm for pm, _, _ in parts[-1])
+        base_com = sum(pm * pc for pm, pc, _ in parts[-1]) / base_mass if base_mass > 0 else np.zeros(3)
         return cls([b["parent"] for b in bodies], [b["type"] for b in bodies], [b["axis"] for b in bodies],
                    [b["E"] for b in bodies], [b["r"] for b in bodies], mass, com, inertia, gravity,
                    joint_names=[b["name"] for b in bodies], effort_limit=[b["effort"] for b in bodies],
-                   velocity_limit=[b["velocity"] for b in bodies], frames=frames)
+                   velocity_limit=[b["velocity"] for b in bodies], frames=frames, base_mass=base_mass,
+                   base_com=base_com)
 
 
 class RigidBodyFrame(object):
@@ -516,6 +531,54 @@ class RigidBodyFrame(object):
                        "tbd_collision_energy_terms")
         return b
 
+    def _check_support(self):
+        if self.body != -1:
+            raise ValueError("RigidBodyFrame %r: the support must be on the base (frame body %d, expected -1)"
+                             % (self.name, self.body))
+
+    def support_wrench(self, base, q, qd, qdd):
+        """The wrench [f; tau] the support exerts on the whole robot, at this frame's origin in its axes (the reference
+        frame is ignored); this frame must be on the base, its z axis the support normal pointing into the robot.
+        `base` is the packed base of include/toppra_b200_dyn.h (m_b, c_b), or None for the model's (base_mass,
+        base_com).  CUDA tensors (M, nv) -> (M, 6), one tbd_support_wrench launch on the current stream; numpy (nv,) ->
+        (6,) or (M, nv) -> (M, 6), through a device round trip: on one numpy point an `inv_dyn` of
+        SecondOrderConstraint."""
+        self._check_support()
+        base = self.model.packed_base() if base is None else _packed_base(base)
+        torch = _lib.require_cuda()
+        m = self.model
+        if isinstance(q, torch.Tensor) and q.is_cuda:
+            q, qd, qdd = m._prepare(torch, q, qd, qdd)
+            w = torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device)
+            with torch.cuda.device(q.device):
+                _lib.check(_lib_dyn.load().tbd_support_wrench(m._model_ptr(), m.nv, self._frame_ptr(),
+                                                              ctypes.c_void_p(base.ctypes.data), q.shape[0],
+                                                              _lib.ptr(q), _lib.ptr(qd), _lib.ptr(qdd), _lib.ptr(w),
+                                                              _lib.stream_ptr()),
+                           "tbd_support_wrench")
+            return w
+        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd, qdd)]
+        single = arrs[0].ndim == 1
+        w = self.support_wrench(base, *[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
+        return w[0] if single else w
+
+    def support_wrench_terms(self, base, q, qs, qss):
+        """c = w(q, 0, 0), a = w(q, 0, qs) - c, b = w(q, qs, qss) - c of the support wrench (support_wrench) for CUDA
+        tensors (M, nv): one tbd_support_wrench_terms launch.  Returns (a, b, c), each (M, 6)."""
+        self._check_support()
+        base = self.model.packed_base() if base is None else _packed_base(base)
+        torch = _lib.require_cuda()
+        m = self.model
+        q, qs, qss = m._prepare(torch, q, qs, qss)
+        a, b, c = (torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device) for _ in range(3))
+        with torch.cuda.device(q.device):
+            _lib.check(_lib_dyn.load().tbd_support_wrench_terms(m._model_ptr(), m.nv, self._frame_ptr(),
+                                                                ctypes.c_void_p(base.ctypes.data), q.shape[0],
+                                                                _lib.ptr(q), _lib.ptr(qs), _lib.ptr(qss), _lib.ptr(a),
+                                                                _lib.ptr(b), _lib.ptr(c), _lib.stream_ptr()),
+                       "tbd_support_wrench_terms")
+        return a, b, c
+
 
 def _inertia3(I6):
     Ixx, Ixy, Ixz, Iyy, Iyz, Izz = I6
@@ -550,6 +613,32 @@ def _packed_object(obj):
     if obj.shape != (OBJECT_DOUBLES,):
         raise ValueError("packed object: expected %d doubles (m, r, Ic), got shape %s" % (OBJECT_DOUBLES, obj.shape))
     return obj
+
+
+BASE_DOUBLES = 4
+
+
+def _base_inertia(what, mass, com):
+    """(mass, com (3,)) of a static base, or ValueError: finite, mass >= 0."""
+    mass = np.asarray(mass, dtype=np.float64)
+    com = np.asarray(com, dtype=np.float64)
+    if mass.shape != () or com.shape != (3,):
+        raise ValueError("%s: expected a scalar base mass and a base com (3,); got shapes %s, %s"
+                         % (what, mass.shape, com.shape))
+    if not (np.isfinite(mass) and np.isfinite(com).all()):
+        raise ValueError("%s: the base mass and base com must be finite" % what)
+    if not mass >= 0:
+        raise ValueError("%s: the base mass %r must be non-negative" % (what, float(mass)))
+    return float(mass), com.copy()
+
+
+def _packed_base(base):
+    """The packed base of include/toppra_b200_dyn.h (TBD_BASE_DOUBLES = 4 doubles: m_b, c_b) as a contiguous float64
+    array; the library reads exactly 4 doubles from it."""
+    base = np.ascontiguousarray(base, dtype=np.float64)
+    if base.shape != (BASE_DOUBLES,):
+        raise ValueError("packed base: expected %d doubles (m_b, c_b), got shape %s" % (BASE_DOUBLES, base.shape))
+    return base
 
 
 def component_indices(components):
