@@ -221,6 +221,8 @@ def _transforms(packed, q):
 
 
 def _pass(packed, Rs, ps, qd, qdd):
+    """The recursive Newton-Euler pass of the device's rnea_pass: (tau (M, nv), f), f[k] = [n, f] the force of body k
+    plus those its children carried up (root children keep theirs)."""
     M, nv = qd.shape
     g = packed[:3]
     st, f = [], []
@@ -263,14 +265,14 @@ def _pass(packed, Rs, ps, qd, qdd):
             Rf = np.einsum("mij,mj->mi", Rs[k], f[k][1])
             f[par][0] = f[par][0] + np.einsum("mij,mj->mi", Rs[k], f[k][0]) + _cross_np(ps[k], Rf)
             f[par][1] = f[par][1] + Rf
-    return tau
+    return tau, f
 
 
 def rnea_packed(packed, q, qd, qdd):
     """float64 double of tbd_rnea: (M, nv) arrays -> tau (M, nv)."""
     q, qd, qdd = (np.atleast_2d(np.asarray(x, dtype=np.float64)) for x in (q, qd, qdd))
     Rs, ps = _transforms(np.asarray(packed, dtype=np.float64), q)
-    return _pass(packed, Rs, ps, qd, qdd)
+    return _pass(packed, Rs, ps, qd, qdd)[0]
 
 
 def torque_terms_packed(packed, q, qs, qss, friction=None):
@@ -278,9 +280,9 @@ def torque_terms_packed(packed, q, qs, qss, friction=None):
     q, qs, qss = (np.atleast_2d(np.asarray(x, dtype=np.float64)) for x in (q, qs, qss))
     Rs, ps = _transforms(np.asarray(packed, dtype=np.float64), q)
     zero = np.zeros_like(q)
-    c = _pass(packed, Rs, ps, zero, zero)
-    a = _pass(packed, Rs, ps, zero, qs) - c
-    b = _pass(packed, Rs, ps, qs, qss) - c
+    c = _pass(packed, Rs, ps, zero, zero)[0]
+    a = _pass(packed, Rs, ps, zero, qs)[0] - c
+    b = _pass(packed, Rs, ps, qs, qss)[0] - c
     if friction is not None and np.any(np.asarray(friction) != 0):
         c = c + np.sign(qs) * np.asarray(friction, dtype=np.float64)
     return a, b, c

@@ -86,52 +86,6 @@ def mp_total_com(robot, q):
 
 
 # ==== float64 numpy double of the device algorithm ====================================================================
-def _forces(packed, Rs, ps, qd, qdd):
-    """The forces f[k] = (n, f) of every body after the recursive Newton-Euler pass of rnea_ref._pass (the device's
-    rnea_pass): each body's own force plus those its children carried up; root children keep theirs."""
-    M, nv = qd.shape
-    g = packed[:3]
-    cross = rnea_ref._cross_np
-    st, f = [], []
-    for k in range(nv):
-        bd = packed[3 + 27 * k:3 + 27 * (k + 1)]
-        par = int(bd[0])
-        if par < 0:
-            wp, vp, dwp = np.zeros((M, 3)), np.zeros((M, 3)), np.zeros((M, 3))
-            dvp = np.broadcast_to(-g, (M, 3))
-        else:
-            wp, vp, dwp, dvp = st[par]
-        R, p = Rs[k], ps[k]
-        RT = lambda x: np.einsum("mji,mj->mi", R, x)   # noqa: E731
-        w, v = RT(wp), RT(vp + cross(wp, p))
-        dw, dv = RT(dwp), RT(dvp + cross(dwp, p))
-        ax = bd[2:5][None]
-        sq, sqq = ax * qd[:, k:k + 1], ax * qdd[:, k:k + 1]
-        if bd[1] == 0:
-            w = w + sq
-            dw = dw + sqq + cross(w, sq)
-            dv = dv + cross(v, sq)
-        else:
-            v = v + sq
-            dv = dv + sqq + cross(w, sq)
-        st.append((w, v, dw, dv))
-        m, c = bd[17], np.broadcast_to(bd[18:21], (M, 3))
-        Ixx, Ixy, Ixz, Iyy, Iyz, Izz = bd[21:27]
-        Ic = np.array([[Ixx, Ixy, Ixz], [Ixy, Iyy, Iyz], [Ixz, Iyz, Izz]])
-        hl = m * (v + cross(w, c))
-        ha = w @ Ic.T + cross(c, hl)
-        fl = m * (dv + cross(dw, c))
-        n = dw @ Ic.T + cross(c, fl)
-        f.append([n + cross(w, ha) + cross(v, hl), fl + cross(w, hl)])
-    for k in range(nv - 1, -1, -1):
-        par = int(packed[3 + 27 * k])
-        if par >= 0:
-            Rf = np.einsum("mij,mj->mi", Rs[k], f[k][1])
-            f[par][0] = f[par][0] + np.einsum("mij,mj->mi", Rs[k], f[k][0]) + cross(ps[k], Rf)
-            f[par][1] = f[par][1] + Rf
-    return f
-
-
 def _wrench(packed, frame, base, Rs, ps, f, M):
     cross = rnea_ref._cross_np
     nv = len(Rs)
@@ -155,7 +109,7 @@ def support_wrench_packed(packed, frame, base, q, qd, qdd):
     packed = np.asarray(packed, dtype=np.float64)
     q, qd, qdd = (np.atleast_2d(np.asarray(x, dtype=np.float64)) for x in (q, qd, qdd))
     Rs, ps = rnea_ref._transforms(packed, q)
-    return _wrench(packed, frame, np.asarray(base, dtype=np.float64), Rs, ps, _forces(packed, Rs, ps, qd, qdd),
+    return _wrench(packed, frame, np.asarray(base, dtype=np.float64), Rs, ps, rnea_ref._pass(packed, Rs, ps, qd, qdd)[1],
                    q.shape[0])
 
 

@@ -30,18 +30,9 @@ import pytest
 import kin_acc_ref as kar
 import kin_ref as kr
 import rnea_ref as rr
-from test_cartesian_velocity import (CASES, DYN_LIB, LOCKED, OFFSET, TB_ERR_ARG, TB_ERR_UNSUPPORTED, _assert_solution,
-                                     _dev, _eq, _gpu_present, _model_from_packed, _problems, close, model_of, urdf)
-
-
-class FakePath(object):
-    def __init__(self, B, dof):
-        self.B, self.dof, self.device = B, dof, "cpu"
-
-
-def _offset_spec(off):
-    from toppra_b200.dynamics import rpy_matrix
-    return (rpy_matrix(off["rpy"]) if off else np.eye(3)), (np.asarray(off["xyz"]) if off else np.zeros(3))
+from dyn_common import (CASES, DYN_LIB, FakePath, LOCKED, OFFSET, TB_ERR_ARG, TB_ERR_UNSUPPORTED, close, model_of, urdf,
+                        _assert_one_terms_launch, _assert_solution, _dev, _dyn_header, _eq, _gpu_present,
+                        _model_from_packed, _offset_spec, _problems)
 
 
 # ==== CPU: numpy double vs the 50-digit reference, errors, C-ABI =====================================================
@@ -120,7 +111,6 @@ def test_value_errors():
 
 
 def test_dyn_header_prototypes_of_acceleration_entries():
-    from test_rigid_body import _dyn_header
     from toppra_b200 import _lib_dyn
     declared = _dyn_header()
     assert declared["tbd_frame_acceleration"] == ["ptr", "int", "ptr", "int", "ptr", "ptr", "ptr", "ptr", "ptr"]
@@ -514,3 +504,13 @@ def test_gpu_with_torque_and_velocity_limits_vs_oracle(ta):
         _assert_solution((h["K"][i], h["sd"][i]), o["K"], o["sd"], h["status"][i], o["status"])
         n_ok += int(o["status"] == 0)
     assert n_ok > 0.8 * B
+
+
+@pytest.mark.gpu
+def test_gpu_one_terms_launch_per_batch_or_chunk(ta, monkeypatch):
+    m = model_of("arm6.urdf")
+    f = m.frame("flange", xyz=(0, 0, 0.1))
+    ss, way, vlim, alim = _problems(10, 6, 31, m.velocity_limit)
+    climit = np.tile([[-4.0, 4.0]], (3, 1))
+    _assert_one_terms_launch(ta, monkeypatch, lambda: _cons(ta, f, climit, (0, 1, 2), vlim, alim),
+                             ta.BatchSplineInterpolator(ss, way), np.linspace(0, 1, 80), "tbd_acceleration_terms")

@@ -24,32 +24,9 @@ import pytest
 
 import kin_ref as kr
 import rnea_ref as rr
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ROBOTS = os.path.join(ROOT, "tests", "golden", "robots")
-DYN_LIB = os.path.join(ROOT, "toppra_b200", "libtoppra_b200_dyn.so")
-LOCKED = {"finger_left_joint": 0.013, "finger_right_joint": 0.021}
-TB_ERR_ARG, TB_ERR_UNSUPPORTED = -1, -2
-CASES = [("arm6.urdf", None), ("arm7_gripper.urdf", LOCKED), ("arm7_gripper.urdf", None)]
-OFFSET = dict(xyz=(0.03, -0.02, 0.1), rpy=(0.3, -0.2, 0.5))
-
-
-def urdf(name):
-    return open(os.path.join(ROBOTS, name)).read()
-
-
-def model_of(name, locked=None):
-    from toppra_b200 import RigidBodyModel
-    return RigidBodyModel.from_urdf(urdf(name), locked_joints=locked)
-
-
-def close(got, ref, tol):
-    """|got - ref| <= tol * max(1, max|ref|) (the scale of the state)."""
-    ref = np.asarray(ref, dtype=np.float64)
-    scale = max(1.0, float(np.max(np.abs(ref))))
-    err = float(np.max(np.abs(np.asarray(got) - ref)))
-    assert err <= tol * scale, (err, scale)
-    return err / scale
+from dyn_common import (CASES, DYN_LIB, FakePath, LOCKED, OFFSET, ROOT, TB_ERR_ARG, TB_ERR_UNSUPPORTED, close, model_of,
+                        urdf, _assert_one_terms_launch, _assert_solution, _dev, _dyn_header, _eq, _gpu_present,
+                        _model_from_packed, _problems)
 
 
 def _mp_check(m, mp, frames, q, qd, tol):
@@ -122,9 +99,6 @@ def test_value_errors():
     with pytest.raises(ValueError, match="dof"):
         CartesianVelocityNorm(f, S, 0.25, dof=7)
 
-    class FakePath(object):
-        def __init__(self, B, dof):
-            self.B, self.dof, self.device = B, dof, "cpu"
     grid = np.linspace(0, 1, 10)
     c = CartesianVelocityNorm(f, S, [0.2, 0.3, 0.4])
     assert c.get_dof() == 6 and c.num_rows(RecordContext(FakePath(3, 6), grid, grid)) == 1
@@ -143,7 +117,6 @@ def test_value_errors():
 
 
 def test_dyn_header_prototypes_of_frame_entries():
-    from test_rigid_body import _dyn_header
     from toppra_b200 import _lib_dyn
     declared = _dyn_header()
     assert declared["tbd_frame_velocity"] == ["ptr", "int", "ptr", "int", "ptr", "ptr", "ptr", "ptr"]
@@ -157,11 +130,6 @@ def test_dyn_header_prototypes_of_frame_entries():
     for key, code in (("WORLD", 0), ("LOCAL", 1), ("LOCAL_WORLD_ALIGNED", 2)):
         assert "#define TBD_%s %d" % (key, code) in text and REFERENCE_FRAMES[key.lower()] == code
     assert "#define TBD_FRAME_DOUBLES 14" in text and model_of("arm6.urdf").frame("flange").packed.shape == (14,)
-
-
-def _gpu_present():
-    import torch
-    return torch.cuda.is_available()
 
 
 # host addresses stand in for device arrays: a case that slipped through the validation would launch a kernel on them
@@ -231,18 +199,6 @@ def ta():
     return toppra_b200
 
 
-def _dev(x):
-    import torch
-    return torch.as_tensor(np.asarray(x, dtype=np.float64), device="cuda")
-
-
-def _model_from_packed(ta, packed):
-    nv = (len(packed) - 3) // 27
-    b = packed[3:].reshape(nv, 27)
-    return ta.RigidBodyModel(b[:, 0], b[:, 1], b[:, 2:5], b[:, 5:14], b[:, 14:17], b[:, 17], b[:, 18:21], b[:, 21:27],
-                             gravity=packed[:3])
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("nv", [1, 2, 3, 5, 8, 12, 16])
 def test_gpu_frame_velocity_random_trees_vs_mp(ta, nv):
@@ -304,13 +260,6 @@ def test_gpu_velocity_norm_terms_bit_equal_frame_velocity(ta):
     assert np.array_equal(vn[keep], v[keep]) and np.isfinite(bn[keep]).all()
 
 
-def _assert_solution(got, ref_K, ref_sd, st, ref_st):
-    assert st == ref_st
-    if ref_st == 0:
-        np.testing.assert_allclose(got[0], ref_K, rtol=1e-8, atol=1e-9)
-        np.testing.assert_allclose(got[1], ref_sd, rtol=1e-8, atol=1e-9)
-
-
 def _golden_frame(g, robot, m):
     return m.frame(str(g[robot + "/link"]), xyz=g[robot + "/xyz"], rpy=g[robot + "/rpy"],
                    reference_frame=str(g[robot + "/ref"]))
@@ -347,15 +296,6 @@ def test_gpu_reference_golden(ta, golden, robot, name, locked):
         for i in range(B):
             _assert_solution((h["K"][i], h["sd"][i]), g["%s/s%d/K" % (robot, scheme)][i],
                              g["%s/s%d/sd" % (robot, scheme)][i], h["status"][i], g["%s/s%d/status" % (robot, scheme)][i])
-
-
-def _problems(B, nv, seed, velocity):
-    rng = np.random.RandomState(seed)
-    way = np.cumsum(rng.uniform(-0.7, 0.7, (B, 5, nv)), axis=1)
-    vel = np.where(np.isfinite(velocity), velocity, 3.0)
-    vlim = np.tile(np.stack([-vel, vel], axis=1), (B, 1, 1))
-    al = rng.uniform(6, 10, (B, nv))
-    return np.linspace(0, 1, 5), way, vlim, np.stack([-al, al], axis=-1)
 
 
 def _active_limits(ta, f, S, path, grid, vlim, alim, share=0.5):
@@ -402,10 +342,6 @@ def test_gpu_256_paths_per_path_limits_vs_oracle(ta):
 def _cart_cons(ta, f, S, vlim, alim, limit, scheme=0):
     return [ta.constraint.JointVelocityConstraint(vlim), ta.constraint.JointAccelerationConstraint(alim),
             ta.constraint.CartesianVelocityNorm(f, S, limit, discretization_scheme=scheme)]
-
-
-def _eq(x, y):
-    return np.array_equal(np.asarray(x), np.asarray(y), equal_nan=True)
 
 
 @pytest.mark.gpu
@@ -531,3 +467,12 @@ def test_gpu_with_joint_torque_constraint_vs_oracle(ta):
         _assert_solution((h["K"][i], h["sd"][i]), o["K"], o["sd"], h["status"][i], o["status"])
         n_ok += int(o["status"] == 0)
     assert n_ok > 0.8 * B
+
+
+@pytest.mark.gpu
+def test_gpu_one_terms_launch_per_batch_or_chunk(ta, monkeypatch):
+    m = model_of("arm6.urdf")
+    f = m.frame("flange", xyz=(0, 0, 0.1))
+    ss, way, vlim, alim = _problems(10, 6, 29, m.velocity_limit)
+    _assert_one_terms_launch(ta, monkeypatch, lambda: _cart_cons(ta, f, np.eye(6), vlim, alim, np.full(10, 1.5)),
+                             ta.BatchSplineInterpolator(ss, way), np.linspace(0, 1, 80), "tbd_velocity_norm_terms")

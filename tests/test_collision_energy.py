@@ -33,15 +33,11 @@ import pytest
 import energy_ref as er
 import kin_ref as kr
 import rnea_ref as rr
-from test_cartesian_velocity import (CASES, DYN_LIB, LOCKED, OFFSET, ROOT, TB_ERR_ARG, TB_ERR_UNSUPPORTED,
-                                     _assert_solution, _dev, _eq, _gpu_present, _model_from_packed, model_of, urdf)
+from dyn_common import (CASES, DYN_LIB, FakePath, LOCKED, OFFSET, TB_ERR_ARG, TB_ERR_UNSUPPORTED, model_of, urdf,
+                        _assert_one_terms_launch, _assert_solution, _dev, _dyn_header, _eq, _gpu_present,
+                        _model_from_packed, _problems)
 
 HUMAN_MASS = 0.6
-
-
-class FakePath(object):
-    def __init__(self, B, dof):
-        self.B, self.dof, self.device = B, dof, "cpu"
 
 
 def rel_err(got, ref):
@@ -256,7 +252,6 @@ def test_value_errors():
 
 
 def test_dyn_header_prototypes_of_energy_entries():
-    from test_rigid_body import _dyn_header
     from toppra_b200 import _lib_dyn
     declared = _dyn_header()
     assert declared["tbd_frame_inverse_inertia"] == ["ptr", "int", "ptr", "int", "ptr", "ptr", "ptr"]
@@ -550,15 +545,6 @@ def test_gpu_reference_golden(ta, golden, robot, name, locked):
             _assert_solution((h["K"][i], h["sd"][i]), key("K", i), key("sd", i), h["status"][i], key("status", i))
 
 
-def _problems(B, nv, seed, velocity):
-    rng = np.random.RandomState(seed)
-    way = np.cumsum(rng.uniform(-0.7, 0.7, (B, 5, nv)), axis=1)
-    vel = np.where(np.isfinite(velocity), velocity, 3.0)
-    vlim = np.tile(np.stack([-vel, vel], axis=1), (B, 1, 1))
-    al = rng.uniform(6, 10, (B, nv))
-    return np.linspace(0, 1, 5), way, vlim, np.stack([-al, al], axis=-1)
-
-
 def _active_limits(ta, f, mh, path, grid, vlim, alim, share=0.3):
     """Per path: `share` of the largest b sd^2 of the solution without the energy limit (so that it is active)."""
     h = ta.BatchTOPPRA([ta.constraint.JointVelocityConstraint(vlim), ta.constraint.JointAccelerationConstraint(alim)],
@@ -761,39 +747,12 @@ def test_gpu_with_torque_and_velocity_limits_vs_oracle(ta):
     assert n_ok > 0.8 * B
 
 
-class _CountingLib(object):
-    """Forwards to libtoppra_b200_dyn.so and counts the calls of each entry."""
-
-    def __init__(self, lib):
-        self._lib, self.calls = lib, {}
-
-    def __getattr__(self, name):
-        fn = getattr(self._lib, name)
-
-        def call(*args):
-            self.calls[name] = self.calls.get(name, 0) + 1
-            return fn(*args)
-        return call
-
-
 @pytest.mark.gpu
 def test_gpu_one_terms_launch_per_batch_or_chunk(ta, monkeypatch):
-    from toppra_b200 import _lib_dyn
     m = model_of("arm6.urdf")
     f = m.frame("flange", xyz=(0, 0, 0.1))
     B = 10
     ss, way, vlim, alim = _problems(B, 6, 47, m.velocity_limit)
-    path = ta.BatchSplineInterpolator(ss, way)
-    grid = np.linspace(0, 1, 80)
     limit = np.full(B, 2.0)
-    counting = _CountingLib(_lib_dyn.load())
-    monkeypatch.setattr(_lib_dyn, "_dlib", counting)
-    whole = ta.BatchTOPPRA(_cons(ta, f, vlim, alim, limit, HUMAN_MASS), path, grid)
-    whole.compute_parameterization(0, 0)
-    assert counting.calls == {"tbd_collision_energy_terms": 1}, counting.calls
-    per_path = 8 * ta.engine.record_doubles(whole.R) * whole.G
-    counting.calls.clear()
-    parts = ta.BatchTOPPRA(_cons(ta, f, vlim, alim, limit, HUMAN_MASS), path, grid, max_record_bytes=4 * per_path)
-    assert parts.chunk_size() == 4
-    parts.compute_parameterization(0, 0)
-    assert counting.calls == {"tbd_collision_energy_terms": 3}, counting.calls          # chunks of 4, 4, 2
+    _assert_one_terms_launch(ta, monkeypatch, lambda: _cons(ta, f, vlim, alim, limit, HUMAN_MASS),
+                             ta.BatchSplineInterpolator(ss, way), np.linspace(0, 1, 80), "tbd_collision_energy_terms")

@@ -30,23 +30,13 @@ import pytest
 
 import contact_ref as cref
 import rnea_ref as rr
-from test_cartesian_velocity import (CASES, DYN_LIB, LOCKED, OFFSET, ROOT, TB_ERR_ARG, TB_ERR_UNSUPPORTED,
-                                     _assert_solution, _dev, _eq, _gpu_present, _model_from_packed, close, model_of,
-                                     urdf)
+from dyn_common import (CASES, DYN_LIB, FakePath, LOCKED, OFFSET, ROOT, TB_ERR_ARG, TB_ERR_UNSUPPORTED, close, model_of,
+                        urdf, _assert_one_terms_launch, _assert_solution, _dev, _dyn_header, _eq, _gpu_present,
+                        _model_from_packed, _offset_spec, _oracle_joint_rows, _oracle_rows)
 
 OBJECT = cref.object_packed(0.8, (0.006, -0.004, 0.06), (0.0021, 0.0001, -0.0002, 0.0026, 0.0001, 0.0017))
 HALF_LENGTHS, FRICTION = (0.05, 0.04), 0.5
 G0 = 9.81
-
-
-class FakePath(object):
-    def __init__(self, B, dof):
-        self.B, self.dof, self.device = B, dof, "cpu"
-
-
-def _offset_spec(off):
-    from toppra_b200.dynamics import rpy_matrix
-    return (rpy_matrix(off["rpy"]) if off else np.eye(3)), (np.asarray(off["xyz"]) if off else np.zeros(3))
 
 
 def _cone():
@@ -231,7 +221,6 @@ def test_value_errors():
 
 
 def test_dyn_header_prototypes_of_contact_entries():
-    from test_rigid_body import _dyn_header
     from toppra_b200 import _lib_dyn
     declared = _dyn_header()
     assert declared["tbd_contact_wrench"] == ["ptr", "int", "ptr", "ptr", "int", "ptr", "ptr", "ptr", "ptr", "ptr"]
@@ -373,15 +362,6 @@ def _terms(f, obj, path, grid):
     d = _dev(grid)
     out = f.contact_wrench_terms(obj, *(path.eval_device(d, o).reshape(-1, f.nv) for o in (0, 1, 2)))
     return [x.reshape(path.B, len(grid), 6).cpu().numpy() for x in out]
-
-
-def _oracle_rows(F, a, b, c, grid, interp):
-    """(G, 3, R) rows a F^T, b F^T, c F^T - 0 of the constraint for the oracle."""
-    from toppra_b200.constraint.linear_constraint import canlinear_colloc_to_interpolate
-    g = np.zeros(F.shape[0])
-    if interp:
-        a, b, c, F, g = canlinear_colloc_to_interpolate(a, b, c, F, g, None, None, grid, identical=True)[:5]
-    return np.stack((a.dot(F.T), b.dot(F.T), c.dot(F.T) - g), axis=1)
 
 
 def _in_cone(F, a, b, c, sd, sdd):
@@ -585,16 +565,6 @@ def test_gpu_toppra_sd_and_quintic_piecewise_poly_path_vs_oracle(ta, golden):
         assert abs(got - want) <= 1e-4 * max(1.0, want), (got, want)
 
 
-def _oracle_joint_rows(qs, qss, vlim, alim):
-    """(G, 3, 2 nv) rows of JointAccelerationConstraint under collocation for the oracle: a = q', b = q'', c = 0,
-    F = [I; -I], g = [upper; -lower]."""
-    nv = qs.shape[1]
-    Fj = np.vstack((np.eye(nv), -np.eye(nv)))
-    g = np.concatenate((alim[:, 1], -alim[:, 0]))
-    G = qs.shape[0]
-    return np.stack((qs.dot(Fj.T), qss.dot(Fj.T), np.zeros((G, nv)).dot(Fj.T) - g), axis=1)
-
-
 @pytest.mark.gpu
 def test_gpu_with_torque_and_velocity_limits_vs_oracle(ta, golden):
     from oracle import oracle as orc
@@ -635,39 +605,11 @@ def test_gpu_with_torque_and_velocity_limits_vs_oracle(ta, golden):
     assert n_ok > 0.8 * B
 
 
-class _CountingLib(object):
-    """Forwards to libtoppra_b200_dyn.so and counts the calls of each entry."""
-
-    def __init__(self, lib):
-        self._lib, self.calls = lib, {}
-
-    def __getattr__(self, name):
-        fn = getattr(self._lib, name)
-
-        def call(*args):
-            self.calls[name] = self.calls.get(name, 0) + 1
-            return fn(*args)
-        return call
-
-
 @pytest.mark.gpu
 def test_gpu_one_terms_launch_per_batch_or_chunk(ta, golden, monkeypatch):
-    from toppra_b200 import _lib_dyn
     g = golden("contact_stability")
     m = model_of("arm6.urdf")
     f = _golden_frame(g, "arm6", m)
-    B = 10
-    ss, way, vlim, alim = _tray_problems(B, g["arm6/up"], 67, m.velocity_limit)
-    path = ta.BatchSplineInterpolator(ss, way)
-    grid = np.linspace(0, 1, 80)
-    counting = _CountingLib(_lib_dyn.load())
-    monkeypatch.setattr(_lib_dyn, "_dlib", counting)
-    whole = ta.BatchTOPPRA(_cons(ta, f, vlim, alim), path, grid)
-    whole.compute_parameterization(0, 0)
-    assert counting.calls == {"tbd_contact_wrench_terms": 1}, counting.calls
-    per_path = 8 * ta.engine.record_doubles(whole.R) * whole.G
-    counting.calls.clear()
-    parts = ta.BatchTOPPRA(_cons(ta, f, vlim, alim), path, grid, max_record_bytes=4 * per_path)
-    assert parts.chunk_size() == 4
-    parts.compute_parameterization(0, 0)
-    assert counting.calls == {"tbd_contact_wrench_terms": 3}, counting.calls          # chunks of 4, 4, 2
+    ss, way, vlim, alim = _tray_problems(10, g["arm6/up"], 67, m.velocity_limit)
+    _assert_one_terms_launch(ta, monkeypatch, lambda: _cons(ta, f, vlim, alim), ta.BatchSplineInterpolator(ss, way),
+                             np.linspace(0, 1, 80), "tbd_contact_wrench_terms")

@@ -17,37 +17,13 @@ GPU:
     BatchPiecewisePolyPath."""
 import ctypes
 import os
-import re
 
 import numpy as np
 import pytest
 
 import rnea_ref as rr
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-ROBOTS = os.path.join(ROOT, "tests", "golden", "robots")
-DYN_LIB = os.path.join(ROOT, "toppra_b200", "libtoppra_b200_dyn.so")
-LOCKED = {"finger_left_joint": 0.013, "finger_right_joint": 0.021}
-TB_ERR_ARG, TB_ERR_UNSUPPORTED = -1, -2
-CASES = [("arm6.urdf", None), ("arm7_gripper.urdf", LOCKED), ("arm7_gripper.urdf", None)]
-
-
-def urdf(name):
-    return open(os.path.join(ROBOTS, name)).read()
-
-
-def model_of(name, locked=None):
-    from toppra_b200 import RigidBodyModel
-    return RigidBodyModel.from_urdf(urdf(name), locked_joints=locked)
-
-
-def close(got, ref, tol):
-    """|got - ref| <= tol * max(1, max|ref|) (the torque scale of the state)."""
-    ref = np.asarray(ref, dtype=np.float64)
-    scale = max(1.0, float(np.max(np.abs(ref))))
-    err = float(np.max(np.abs(np.asarray(got) - ref)))
-    assert err <= tol * scale, (err, scale)
-    return err / scale
+from dyn_common import (CASES, DYN_LIB, LOCKED, TB_ERR_ARG, TB_ERR_UNSUPPORTED, close, model_of, urdf,
+                        _assert_one_terms_launch, _assert_solution, _dev, _dyn_header, _eq, _gpu_present)
 
 
 # ==== CPU: parsing, folding, errors ==================================================================================
@@ -120,16 +96,6 @@ def test_rigid_body_model_routes_torque_constraints_to_the_device():
     assert jt._second_order().batched and jt._second_order().inv_dyn is m
 
 
-def _dyn_header():
-    text = open(os.path.join(ROOT, "include", "toppra_b200_dyn.h")).read()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    out = {}
-    for name, args in re.findall(r"\bint\s+(tbd_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", text):
-        out[name] = ["ptr" if "*" in a else ("double" if "double" in a else "int")
-                     for a in (x.strip() for x in args.split(",")) if a not in ("", "void")]
-    return out
-
-
 def test_dyn_header_matches_prototypes():
     from toppra_b200 import _lib_dyn
     declared = _dyn_header()
@@ -137,11 +103,6 @@ def test_dyn_header_matches_prototypes():
     for name, (argtypes, restype) in _lib_dyn._PROTOS.items():
         assert [{ctypes.c_int: "int", ctypes.c_double: "double"}.get(t, "ptr") for t in argtypes] == declared[name], name
         assert restype is ctypes.c_int
-
-
-def _gpu_present():
-    import torch
-    return torch.cuda.is_available()
 
 
 # host addresses stand in for device arrays: a case that slipped through the validation would launch a kernel on them
@@ -198,11 +159,6 @@ def test_dyn_argument_checks():
 def ta():
     import toppra_b200
     return toppra_b200
-
-
-def _dev(x):
-    import torch
-    return torch.as_tensor(np.asarray(x, dtype=np.float64), device="cuda")
 
 
 @pytest.mark.gpu
@@ -288,13 +244,6 @@ def test_gpu_torque_terms_bit_equal_three_calls(ta, fric):
 def _golden_problem(g, robot, b):
     return (g[robot + "/way"][b], g[robot + "/vlim"][b], g[robot + "/alim"][b], g[robot + "/taulim"][b],
             g[robot + "/fric"][b])
-
-
-def _assert_solution(got, ref_K, ref_sd, st, ref_st):
-    assert st == ref_st
-    if ref_st == 0:
-        np.testing.assert_allclose(got[0], ref_K, rtol=1e-8, atol=1e-9)
-        np.testing.assert_allclose(got[1], ref_sd, rtol=1e-8, atol=1e-9)
 
 
 @pytest.mark.gpu
@@ -383,10 +332,6 @@ def _torque_cons(ta, m, vlim, alim, taulim, fric):
             ta.constraint.SecondOrderConstraint.joint_torque_constraint(m, taulim, fric)]
 
 
-def _eq(x, y):
-    return np.array_equal(np.asarray(x), np.asarray(y), equal_nan=True)
-
-
 @pytest.mark.gpu
 def test_gpu_ragged_chunked_and_single_path_bit_equal(ta):
     m = model_of("arm7_gripper.urdf", LOCKED)
@@ -454,3 +399,12 @@ def test_gpu_quintic_piecewise_poly_path(ta):
         assert _eq(h[key], ht[key]), key
     assert (h["status"] == 0).sum() >= B // 2
     assert isinstance(path.eval_device(torch.as_tensor(grid, device="cuda"), 2), torch.Tensor)
+
+
+@pytest.mark.gpu
+def test_gpu_one_terms_launch_per_batch_or_chunk(ta, monkeypatch):
+    m = model_of("arm6.urdf")
+    ss, way, vlim, alim, taulim = _random_problems(10, m.nv, 23, np.where(np.isfinite(m.effort_limit), m.effort_limit,
+                                                                          8.0), m.velocity_limit)
+    _assert_one_terms_launch(ta, monkeypatch, lambda: _torque_cons(ta, m, vlim, alim, taulim, 0.2 * np.ones(m.nv)),
+                             ta.BatchSplineInterpolator(ss, way), np.linspace(0, 1, 80), "tbd_torque_terms")

@@ -35,20 +35,15 @@ import pytest
 
 import rnea_ref as rr
 import support_ref as sref
-from test_cartesian_velocity import (DYN_LIB, ROOT, TB_ERR_ARG, TB_ERR_UNSUPPORTED, _assert_solution, _dev, _eq,
-                                     _gpu_present, _model_from_packed, close, model_of, urdf)
-from test_contact_stability import _CountingLib, _oracle_joint_rows, _oracle_rows
+from dyn_common import (DYN_LIB, FakePath, ROOT, TB_ERR_ARG, TB_ERR_UNSUPPORTED, close, model_of, urdf,
+                        _assert_one_terms_launch, _assert_solution, _dev, _dyn_header, _eq, _gpu_present,
+                        _model_from_packed, _oracle_joint_rows, _oracle_rows)
 
 WHEELS = {"wheel_fl_joint": 0.3, "wheel_fr_joint": -1.2, "wheel_rl_joint": 2.0, "wheel_rr_joint": 0.0}
 CASES = [("mobile_arm.urdf", WHEELS), ("mobile_arm.urdf", None), ("arm6.urdf", None)]
 ROOT_LINK = {"mobile_arm.urdf": "base_footprint", "arm6.urdf": "base_link"}
 OFFSETS = [dict(), dict(xyz=(0.03, -0.02, 0.0), rpy=(0.0, 0.0, 0.7)), dict(xyz=(-0.1, 0.05, 0.2), rpy=(0.3, -0.2, 0.5))]
 G0 = 9.81
-
-
-class FakePath(object):
-    def __init__(self, B, dof):
-        self.B, self.dof, self.device = B, dof, "cpu"
 
 
 def _support(m, name, off=None, ref="local_world_aligned"):
@@ -260,7 +255,6 @@ def test_value_errors():
 
 
 def test_dyn_header_prototypes_of_support_entries():
-    from test_rigid_body import _dyn_header
     from toppra_b200 import _lib_dyn
     declared = _dyn_header()
     assert declared["tbd_support_wrench"] == ["ptr", "int", "ptr", "ptr", "int", "ptr", "ptr", "ptr", "ptr", "ptr"]
@@ -711,22 +705,9 @@ def test_gpu_with_torque_and_velocity_limits_vs_oracle(ta, golden):
 
 @pytest.mark.gpu
 def test_gpu_one_terms_launch_per_batch_or_chunk(ta, golden, monkeypatch):
-    from toppra_b200 import _lib_dyn
     g = golden("support_stability")
     m, f = _golden_setup(g, "mobile")
     sup = lambda s: _cons_of(ta, f, g, "mobile", "poly", s)  # noqa: E731
-    B = 10
-    ss, way, vlim, alim = _problems(B, g["mobile/up"], 67, m)
-    path = ta.BatchSplineInterpolator(ss, way)
-    grid = np.linspace(0, 1, 80)
-    counting = _CountingLib(_lib_dyn.load())
-    monkeypatch.setattr(_lib_dyn, "_dlib", counting)
-    whole = ta.BatchTOPPRA(_cons(ta, sup, vlim, alim), path, grid)
-    whole.compute_parameterization(0, 0)
-    assert counting.calls == {"tbd_support_wrench_terms": 1}, counting.calls
-    per_path = 8 * ta.engine.record_doubles(whole.R) * whole.G
-    counting.calls.clear()
-    parts = ta.BatchTOPPRA(_cons(ta, sup, vlim, alim), path, grid, max_record_bytes=4 * per_path)
-    assert parts.chunk_size() == 4
-    parts.compute_parameterization(0, 0)
-    assert counting.calls == {"tbd_support_wrench_terms": 3}, counting.calls          # chunks of 4, 4, 2
+    ss, way, vlim, alim = _problems(10, g["mobile/up"], 67, m)
+    _assert_one_terms_launch(ta, monkeypatch, lambda: _cons(ta, sup, vlim, alim), ta.BatchSplineInterpolator(ss, way),
+                             np.linspace(0, 1, 80), "tbd_support_wrench_terms")

@@ -7,14 +7,15 @@ whose user callback returns the frame's acceleration (`examples-old/cartesian_ac
     along the path:  acc = acc(q, 0, q') u + acc(q, q', q'') x,   u = s'', x = s'^2,   acc(q, 0, 0) = 0
     lower <= acc[components] <= upper   =>   F = [I_k; -I_k],  g = [upper; -lower],  a, b as above,  c = 0
 
-It is `SecondOrderConstraint`'s eye form with the frame as `inv_dyn`: every a and b of the batch (or record chunk) come
-from ONE `tbd_acceleration_terms` launch (RigidBodyFrame.acceleration_terms), and the rows go through the same
-`tb_rows_canlinear` call as joint torque limits.  So TOPPRA, BatchTOPPRA, BatchTOPPRAsd, feasible, reachable and
+It is `SecondOrderConstraint`'s eye form with the frame's acceleration as `inv_dyn`: every a and b of the batch (or
+record chunk) come from ONE `tbd_acceleration_terms` launch (RigidBodyFrame.acceleration_terms, its `device_terms`),
+and the rows go through the same `tb_rows_canlinear` call as joint torque limits.  So TOPPRA, BatchTOPPRA, BatchTOPPRAsd, feasible, reachable and
 controllable sets, ragged grids, record chunks and order-k paths take it unchanged."""
 import numpy as np
 
 from .constraint import DiscretizationType
 from .linear_second_order import SecondOrderConstraint
+from .. import engine
 from ..dynamics import RigidBodyFrame, component_indices
 
 
@@ -44,27 +45,24 @@ class CartesianAccelerationConstraint(SecondOrderConstraint):
         eyes = np.vstack((np.eye(k), -np.eye(k)))
         g_aug = np.concatenate((alim[..., 1], -alim[..., 0]), axis=-1)
         g_single = g_aug if g_aug.ndim == 1 else g_aug[0]
-        super(CartesianAccelerationConstraint, self).__init__(frame, lambda _: eyes, lambda _: g_single, frame.nv,
-                                                              discretization_scheme=discretization_scheme, batched=True)
+        super(CartesianAccelerationConstraint, self).__init__(frame.acceleration, lambda _: eyes, lambda _: g_single,
+                                                              frame.nv, discretization_scheme=discretization_scheme,
+                                                              batched=True)
         self._eye_form = (g_aug, np.zeros(k))
+        self.device_terms = self._terms
         self.frame = frame
         self.components = tuple(comps)
         self.limits = alim          # not `alim`: BatchTOPPRA checks attributes of that name against the path's dof
         self._format_string = "    Kind: Cartesian acceleration limit of frame %r, components %s\n" % (
             frame.name, self.components)
 
+    def _terms(self, q, qs, qss):
+        """acc(q, 0, 0) = 0: c = 0, and a, b need no subtraction."""
+        a, b = self.frame.acceleration_terms(q, qs, qss, self.components)
+        return a, b, engine.torch_mod().zeros_like(a)
+
     def _check_batch(self, ctx):
-        if ctx.bpath.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, ctx.bpath.dof))
+        super(CartesianAccelerationConstraint, self)._check_batch(ctx)
         if self.limits.ndim == 3 and self.limits.shape[0] != ctx.total:
             raise ValueError("CartesianAccelerationConstraint: alim has shape %s; expected (%d, 2) or (%d, %d, 2)"
                              % (self.limits.shape, len(self.components), ctx.total, len(self.components)))
-
-    def num_rows(self, ctx):
-        self._check_batch(ctx)
-        return super(CartesianAccelerationConstraint, self).num_rows(ctx)
-
-    def append_records(self, ctx, records, R_total, row0):
-        self._check_batch(ctx)
-        super(CartesianAccelerationConstraint, self).append_records(ctx, records, R_total, row0)

@@ -17,7 +17,7 @@ single-path host route."""
 import numpy as np
 
 from .constraint import DiscretizationType
-from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate
+from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate, check_dof
 from .. import engine
 from ..dynamics import RigidBodyFrame
 
@@ -66,17 +66,12 @@ class CartesianVelocityNorm(LinearConstraint):
         return self.dof
 
     def compute_constraint_params(self, path, gridpoints):
-        if self.dof is not None and path.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, path.dof))
+        if self.dof is not None:
+            check_dof(self.dof, path.dof)
         gridpoints = np.asarray(gridpoints, dtype=float)
         G = gridpoints.shape[0]
         q, qd = path(gridpoints), path(gridpoints, 1)
-        limit = self.limit
-        if self._path_limits is not None:
-            if self._path_limits.shape != (1,):
-                raise ValueError("a single path takes one limit; got %d" % self._path_limits.shape[0])
-            limit = float(self._path_limits[0])
+        limit = single_path_limit(self)
         a, b, c = np.zeros((G, 1)), np.zeros((G, 1)), np.zeros((G, 1))
         F = np.ones((1, 1)) if self.identical else np.ones((G, 1, 1))
         g = np.full(1, limit) if self.identical else np.zeros((G, 1))
@@ -104,35 +99,47 @@ class CartesianVelocityNorm(LinearConstraint):
     def _interp(self):
         return self.discretization_type == DiscretizationType.Interpolation
 
-    def _check_batch(self, ctx):
-        if ctx.bpath.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, ctx.bpath.dof))
-        if self._path_limits is not None and self._path_limits.shape[0] != ctx.total:
-            raise ValueError("CartesianVelocityNorm: limit has shape %s; expected a float or (%d,)"
-                             % (self._path_limits.shape, ctx.total))
-
     def num_rows(self, ctx):
         if not self._device():
             return super(CartesianVelocityNorm, self).num_rows(ctx)
-        self._check_batch(ctx)
-        return 2 if self._interp() else 1
+        return sd2_num_rows(self, ctx)
 
     def append_records(self, ctx, records, R_total, row0):
         """One tbd_velocity_norm_terms launch for the B x G gridpoints of this context, then the rows a = 0, b,
         c = -limit (F = [1], g = [0]) through tb_rows_canlinear (with the interpolation lift if selected)."""
         if not self._device():
             return super(CartesianVelocityNorm, self).append_records(ctx, records, R_total, row0)
-        self._check_batch(ctx)
-        append_sd2_rows(ctx, lambda q, qs: self.compute_velocity.velocity_norm_terms(q, qs, self.S), self.limit,
-                        self._path_limits, self._interp(), records, R_total, row0)
+        append_sd2_rows(self, ctx, lambda q, qs: self.compute_velocity.velocity_norm_terms(q, qs, self.S), records,
+                        R_total, row0)
 
 
-def append_sd2_rows(ctx, terms, limit, path_limits, interp, records, R_total, row0):
-    """The device rows of a limit b(q, q') s'^2 <= limit: ONE `terms(q, qs) -> b (B G,)` call on q, q' of the B x G
-    gridpoints of `ctx`, then a = 0, b, c = 0 - limit (a float, or path_limits (Bfull,) sliced to the context) with
-    F = [1], g = [0] through tb_rows_canlinear, with the interpolation lift if `interp`.  Shared by the device routes
-    of CartesianVelocityNorm and CollisionEnergyConstraint."""
+# ---- a limit b(q, q') s'^2 <= limit: the parts shared by CartesianVelocityNorm and CollisionEnergyConstraint, whose
+# `cons` has dof, limit (a float, or None) and _path_limits ((Bfull,) or None) and _interp() ------------------------
+def single_path_limit(cons):
+    """The limit of the single-path route: the float, or the only per-path limit."""
+    if cons._path_limits is None:
+        return cons.limit
+    if cons._path_limits.shape != (1,):
+        raise ValueError("a single path takes one limit; got %d" % cons._path_limits.shape[0])
+    return float(cons._path_limits[0])
+
+
+def sd2_num_rows(cons, ctx):
+    """Rows per stage of the device route, after checking the batch: the path's dof, and one limit per path of the
+    full batch when the limits are per path."""
+    check_dof(cons.dof, ctx.bpath.dof)
+    if cons._path_limits is not None and cons._path_limits.shape[0] != ctx.total:
+        raise ValueError("%s: limit has shape %s; expected a float or (%d,)"
+                         % (type(cons).__name__, cons._path_limits.shape, ctx.total))
+    return 2 if cons._interp() else 1
+
+
+def append_sd2_rows(cons, ctx, terms, records, R_total, row0):
+    """The device rows: ONE `terms(q, qs) -> b (B G,)` call on q, q' of the B x G gridpoints of `ctx`, then a = 0, b,
+    c = 0 - limit (the float, or the per-path limits sliced to the context) with F = [1], g = [0] through
+    tb_rows_canlinear, with the interpolation lift if selected."""
+    sd2_num_rows(cons, ctx)
+    limit, path_limits = cons.limit, cons._path_limits
     torch = engine.torch_mod()
     bp = ctx.bpath
     B, G, dof = ctx.B, ctx.G, bp.dof
@@ -148,4 +155,4 @@ def append_sd2_rows(ctx, terms, limit, path_limits, interp, records, R_total, ro
     a = torch.zeros_like(b)
     F = engine.as_device(np.ones((1, 1)), ctx.device)
     g = engine.as_device(np.zeros(1), ctx.device)
-    engine.rows_canlinear(a, b, c, F, g, 0, ctx.d_grid, interp, records, R_total, row0)
+    engine.rows_canlinear(a, b, c, F, g, 0, ctx.d_grid, cons._interp(), records, R_total, row0)

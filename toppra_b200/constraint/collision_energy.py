@@ -19,11 +19,11 @@ BatchTOPPRAsd, feasible, reachable and controllable sets, ragged grids, record c
 unchanged."""
 import numpy as np
 
-from .cartesian_velocity_norm import append_sd2_rows
+from .cartesian_velocity_norm import append_sd2_rows, sd2_num_rows, single_path_limit
 from .constraint import DiscretizationType
-from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate
+from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate, check_dof
 from .. import _lib
-from ..dynamics import RigidBodyFrame
+from ..dynamics import RigidBodyFrame, _is_cuda, _round_trip
 
 
 class CollisionEnergyConstraint(LinearConstraint):
@@ -71,24 +71,16 @@ class CollisionEnergyConstraint(LinearConstraint):
     def energy(self, q, qd):
         """E = 1/2 mu |v|^2 at the state (q, qd): CUDA tensors (M, nv) -> (M,), one launch; numpy (nv,) -> float or
         (M, nv) -> (M,), through a device round trip."""
-        torch = _lib.require_cuda()
-        if isinstance(q, torch.Tensor) and q.is_cuda:
+        if _is_cuda(q):
             return self.terms(q, qd)
-        q, qd = (np.asarray(x, dtype=np.float64) for x in (q, qd))
-        E = self.terms(*(torch.as_tensor(np.atleast_2d(x), device="cuda") for x in (q, qd))).cpu().numpy()
-        return float(E[0]) if q.ndim == 1 else E
+        E = _round_trip(self.terms, q, qd)
+        return float(E) if np.ndim(q) == 1 else E
 
     def compute_constraint_params(self, path, gridpoints):
         """The reference's 7-tuple for one path: a = 0, b from one launch on q, q' at the gridpoints, c = 0,
         F = [1], g = [limit]."""
-        if path.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, path.dof))
-        limit = self.limit
-        if self._path_limits is not None:
-            if self._path_limits.shape != (1,):
-                raise ValueError("a single path takes one limit; got %d" % self._path_limits.shape[0])
-            limit = float(self._path_limits[0])
+        check_dof(self.dof, path.dof)
+        limit = single_path_limit(self)
         gridpoints = np.asarray(gridpoints, dtype=float)
         G = gridpoints.shape[0]
         torch = _lib.require_cuda()
@@ -101,20 +93,10 @@ class CollisionEnergyConstraint(LinearConstraint):
         return a, b, c, F, g, None, None
 
     # ---- device route ------------------------------------------------------------------------------------------
-    def _check_batch(self, ctx):
-        if ctx.bpath.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, ctx.bpath.dof))
-        if self._path_limits is not None and self._path_limits.shape[0] != ctx.total:
-            raise ValueError("CollisionEnergyConstraint: limit has shape %s; expected a float or (%d,)"
-                             % (self._path_limits.shape, ctx.total))
-
     def num_rows(self, ctx):
-        self._check_batch(ctx)
-        return 2 if self._interp() else 1
+        return sd2_num_rows(self, ctx)
 
     def append_records(self, ctx, records, R_total, row0):
         """One tbd_collision_energy_terms launch for the B x G gridpoints of this context, then the rows a = 0, b,
         c = 0 - limit (F = [1], g = [0]) through tb_rows_canlinear (with the interpolation lift if selected)."""
-        self._check_batch(ctx)
-        append_sd2_rows(ctx, self.terms, self.limit, self._path_limits, self._interp(), records, R_total, row0)
+        append_sd2_rows(self, ctx, self.terms, records, R_total, row0)

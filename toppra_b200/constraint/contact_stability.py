@@ -13,15 +13,15 @@ mass r and rotational inertia Ic about it, in contact-frame coordinates.  In con
 F (16 x 6) is the contact wrench cone of the rectangle with friction coefficient mu (Caron, Pham, Nakamura, "Stability
 of surface contacts for humanoid robots: closed-form formulae of the contact wrench cone for rectangular support
 areas", ICRA 2015): the wrenches that are the sum, taken at the centre, of four corner forces each inside its friction
-pyramid.  Every a, b and c of the batch (or record chunk) come from ONE `tbd_contact_wrench_terms` launch, and the rows
-go through `tb_rows_canlinear` with the shared F and g = 0.  So TOPPRA, BatchTOPPRA, BatchTOPPRAsd, feasible, reachable
+pyramid.  Every a, b and c of the batch (or record chunk) come from ONE `tbd_contact_wrench_terms` launch (the
+constraint's `device_terms`), and the rows go through `tb_rows_canlinear` with the shared F and g = 0 (the constant-F
+form of `SecondOrderConstraint`).  So TOPPRA, BatchTOPPRA, BatchTOPPRAsd, feasible, reachable
 and controllable sets, ragged grids, record chunks and order-k paths take it unchanged."""
 import numpy as np
 
 from .constraint import DiscretizationType
 from .linear_second_order import SecondOrderConstraint
-from .. import engine
-from ..dynamics import RigidBodyFrame, _packed_object
+from ..dynamics import RigidBodyFrame, _packed_object, _rigid_inertia
 
 NUM_ROWS = 16
 
@@ -34,7 +34,8 @@ def contact_wrench_cone(half_lengths, friction):
       twisting  s1 (Y f_x - mu tau_x) + s2 (X f_y - mu tau_y) - mu (X + Y) f_z - tau_z  (lower bound on tau_z) and
                 s1 (Y f_x + mu tau_x) + s2 (X f_y + mu tau_y) - mu (X + Y) f_z + tau_z  (upper bound), each for
                 (s1, s2) = (+, +), (+, -), (-, +), (-, -)."""
-    X, Y, mu = _cone_parameters(half_lengths, friction)
+    X, Y = half_lengths_of(half_lengths)
+    mu = friction_of(friction)
     F = []
     for s in (1.0, -1.0):
         F.append([s, 0.0, -mu, 0.0, 0.0, 0.0])
@@ -51,17 +52,28 @@ def contact_wrench_cone(half_lengths, friction):
     return np.array(F, dtype=np.float64)
 
 
-def _cone_parameters(half_lengths, friction):
+def half_lengths_of(half_lengths):
+    """(X, Y) of a rectangle around the origin, or ValueError: both finite and positive."""
     hl = np.asarray(half_lengths, dtype=np.float64)
+    if hl.shape != (2,):
+        raise ValueError("half_lengths must be (X, Y); got shape %s" % (hl.shape,))
+    if not np.isfinite(hl).all():
+        raise ValueError("half_lengths must be finite")
+    if not (hl > 0).all():
+        raise ValueError("half_lengths must be positive; got %s" % hl)
+    return float(hl[0]), float(hl[1])
+
+
+def friction_of(friction):
+    """A friction coefficient, or ValueError: a finite, positive scalar."""
     mu = np.asarray(friction, dtype=np.float64)
-    if hl.shape != (2,) or mu.shape != ():
-        raise ValueError("contact cone: half_lengths must be (X, Y) and friction a scalar; got shapes %s, %s"
-                         % (hl.shape, mu.shape))
-    if not (np.isfinite(hl).all() and np.isfinite(mu)):
-        raise ValueError("contact cone: half_lengths and friction must be finite")
-    if not ((hl > 0).all() and mu > 0):
-        raise ValueError("contact cone: half_lengths and friction must be positive; got %s, %s" % (hl, mu))
-    return float(hl[0]), float(hl[1]), float(mu)
+    if mu.shape != ():
+        raise ValueError("friction must be a scalar; got shape %s" % (mu.shape,))
+    if not np.isfinite(mu):
+        raise ValueError("friction must be finite")
+    if not mu > 0:
+        raise ValueError("friction %r must be positive" % float(mu))
+    return float(mu)
 
 
 class ContactStabilityConstraint(SecondOrderConstraint):
@@ -76,27 +88,15 @@ class ContactStabilityConstraint(SecondOrderConstraint):
         if not isinstance(frame, RigidBodyFrame):
             raise ValueError("ContactStabilityConstraint needs a RigidBodyFrame (RigidBodyModel.frame(...)) as the "
                              "contact frame; for a user callback use SecondOrderConstraint")
-        mass = np.asarray(mass, dtype=np.float64)
-        com = np.asarray(com, dtype=np.float64)
-        inertia = np.asarray(inertia, dtype=np.float64)
-        if mass.shape != () or com.shape != (3,) or inertia.shape != (6,):
-            raise ValueError("ContactStabilityConstraint: expected a scalar mass, com (3,) and inertia (6,); got shapes "
-                             "%s, %s, %s" % (mass.shape, com.shape, inertia.shape))
-        if not (np.isfinite(mass) and np.isfinite(com).all() and np.isfinite(inertia).all()):
-            raise ValueError("ContactStabilityConstraint: mass, com and inertia must be finite")
-        if not mass > 0:
-            raise ValueError("ContactStabilityConstraint: mass %r must be positive" % float(mass))
-        Ixx, Ixy, Ixz, Iyy, Iyz, Izz = inertia
-        I = np.array([[Ixx, Ixy, Ixz], [Ixy, Iyy, Iyz], [Ixz, Iyz, Izz]])
-        if np.linalg.eigvalsh(I).min() < -1e-12 * max(1e-300, np.abs(I).max()):
-            raise ValueError("ContactStabilityConstraint: the inertia matrix is not positive semi-definite")
+        mass, com, _ = _rigid_inertia("ContactStabilityConstraint", mass, com, inertia)
         F = contact_wrench_cone(half_lengths, friction)
         zeros = np.zeros(NUM_ROWS)
         super(ContactStabilityConstraint, self).__init__(self.wrench, lambda _: F, lambda _: zeros, frame.nv,
                                                          discretization_scheme=discretization_scheme, batched=True)
         self.frame = frame
-        self.F = F
-        self.object = _packed_object(np.concatenate(([float(mass)], com, inertia)))
+        self.F = self._const_F = F
+        self.object = _packed_object(np.concatenate(([mass], com, np.asarray(inertia, dtype=np.float64))))
+        self.device_terms = lambda q, qs, qss: frame.contact_wrench_terms(self.object, q, qs, qss)
         self.half_lengths = tuple(float(x) for x in np.asarray(half_lengths, dtype=np.float64))
         self.friction = float(friction)
         self._format_string = "    Kind: contact stability of an object on frame %r, %d rows\n" % (frame.name, NUM_ROWS)
@@ -105,30 +105,3 @@ class ContactStabilityConstraint(SecondOrderConstraint):
         """The contact wrench [f; tau] (frame axes, at the contact origin).  CUDA tensors (M, nv) -> (M, 6), one
         tbd_contact_wrench launch; numpy (nv,) -> (6,) through a device round trip: a reference-style `inv_dyn`."""
         return self.frame.contact_wrench(self.object, q, qd, qdd)
-
-    def _k(self):
-        return NUM_ROWS
-
-    def _check_batch(self, ctx):
-        if ctx.bpath.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, ctx.bpath.dof))
-
-    def num_rows(self, ctx):
-        self._check_batch(ctx)
-        return super(ContactStabilityConstraint, self).num_rows(ctx)
-
-    def _colloc_device(self, ctx):
-        """(a, b, c) as CUDA tensors [B, G, 6]: one tbd_contact_wrench_terms launch for the batch or chunk."""
-        bp = ctx.bpath
-        B, G, dof = ctx.B, ctx.G, bp.dof
-        q, qd, qdd = (bp.eval_device(ctx.d_grid, o).reshape(B * G, dof) for o in (0, 1, 2))
-        a, b, c = self.frame.contact_wrench_terms(self.object, q, qd, qdd)
-        return a.reshape(B, G, 6), b.reshape(B, G, 6), c.reshape(B, G, 6)
-
-    def append_records(self, ctx, records, R_total, row0):
-        self._check_batch(ctx)
-        a, b, c = self._colloc_device(ctx)
-        Fd = engine.as_device(self.F, ctx.device)
-        gd = engine.as_device(np.zeros(NUM_ROWS), ctx.device)
-        engine.rows_canlinear(a, b, c, Fd, gd, 0, ctx.d_grid, self.interpolation, records, R_total, row0)

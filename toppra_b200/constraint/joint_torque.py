@@ -14,7 +14,7 @@ fused inverse-dynamics launch for the whole batch (libtoppra_b200_dyn.so), so Ba
 import numpy as np
 
 from .constraint import DiscretizationType
-from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate
+from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate, check_dof
 from .linear_second_order import SecondOrderConstraint
 
 
@@ -40,8 +40,7 @@ class JointTorqueConstraint(LinearConstraint):
         """Host 7-tuple (a, b, c, F, g, None, None) with the reference's shapes: collocation (G, dof) / F (2 dof, dof),
         interpolation (G, 2 dof) / F (4 dof, 2 dof); F and g are the same for every gridpoint (`identical`)."""
         n = self.get_dof()
-        if path.dof != n:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(n, path.dof))
+        check_dof(n, path.dof)
         grid = np.asarray(gridpoints)
         q, dq, ddq = (path(grid, order) for order in (0, 1, 2))
         rest = np.zeros(n)

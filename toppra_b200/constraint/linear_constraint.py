@@ -97,6 +97,12 @@ class RecordContext(object):
         return t[self.lo:self.hi] if (t is not None and t.dim() == 3) else t
 
 
+def check_dof(dof, path_dof):
+    """ValueError unless the path has the constraint's dof."""
+    if path_dof != dof:
+        raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(dof, path_dof))
+
+
 def canlinear_colloc_to_interpolate(a, b, c, F, g, xbound, ubound, gridpoints, identical=False):
     """Convert collocation parameters to the interpolation scheme (reference linear_constraint.py:84-192):
     the second block evaluates the constraint at s_{i+1} in stage-i variables,

@@ -10,11 +10,12 @@ The three inverse-dynamics evaluations per gridpoint are USER code.  Two ways to
     assembled on the GPU (csrc/tb_coeff.cu: tb_rows_canlinear);
   * `batched=True`: `inv_dyn(q, qd, qdd)` on CUDA tensors of shape (M, dof) -> (M, m); three calls in total for
     the whole batch x grid, everything stays on the device (general fallback for arbitrary models);
-  * a `toppra_b200.RigidBodyModel` as `inv_dyn` (joint_torque_constraint, JointTorqueConstraint): the batched route
-    with the three terms from ONE fused rigid-body inverse-dynamics launch per batch (libtoppra_b200_dyn.so:
-    tbd_torque_terms), bit-identical to three `model(...)` calls plus the operations below;
-  * a `toppra_b200.RigidBodyFrame` as `inv_dyn` (CartesianAccelerationConstraint): the same route with a and b of the
-    frame's acceleration from ONE launch per batch (tbd_acceleration_terms) and c = 0;
+  * `device_terms(q, qs, qss) -> (a, b, c)` on CUDA tensors (M, dof) -> (M, m), set by the constructors of the
+    rigid-body limits: the batched route with the three terms of every gridpoint of the batch from ONE fused launch of
+    libtoppra_b200_dyn.so.  A `toppra_b200.RigidBodyModel` as `inv_dyn` of joint_torque_constraint (and
+    JointTorqueConstraint) sets `model.torque_terms` with the friction, bit-identical to three `model(...)` calls plus
+    the operations above; CartesianAccelerationConstraint, ContactStabilityConstraint and SupportStabilityConstraint
+    set theirs;
   * `device_model=(name, params)` (joint_torque_constraint only): the inverse dynamics is one of the models compiled
     into the library (`engine.DEVICE_MODELS`, include/toppra_b200.h TB_INVDYN_*): ONE kernel evaluates q, q', q'' and
     the three inverse-dynamics terms per gridpoint and writes the torque rows straight into the stage records
@@ -22,14 +23,17 @@ The three inverse-dynamics evaluations per gridpoint are USER code.  Two ways to
 import numpy as np
 
 from .constraint import DiscretizationType
-from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate
+from .linear_constraint import LinearConstraint, canlinear_colloc_to_interpolate, check_dof
 from .. import engine
-from ..dynamics import RigidBodyFrame, RigidBodyModel
+from ..dynamics import RigidBodyModel
 
 
 class SecondOrderConstraint(LinearConstraint):
     """See module docstring.  `constraint_F(q) -> (k, m)`, `constraint_g(q) -> (k,)`;
-    `custom_term(path, s) -> (m,)` (reference style) or `custom_term(q, qd) -> (M, m)` tensors (batched)."""
+    `custom_term(path, s) -> (m,)` (reference style) or `custom_term(q, qd) -> (M, m)` tensors (batched).
+
+    Row forms on the device: the eye form (F = [I; -I], g per path or shared), the constant form (one F (k, m) for
+    every gridpoint, g = 0) and, reference style, the host F(q), g(q) of every gridpoint."""
 
     def __init__(self, inv_dyn, constraint_F, constraint_g, dof, custom_term=None, discretization_scheme=1,
                  batched=False):
@@ -42,7 +46,9 @@ class SecondOrderConstraint(LinearConstraint):
         self.custom_term = custom_term
         self.batched = batched
         self.device_model = None  # (name, params): inverse dynamics evaluated by tb_coeff_second_order
+        self.device_terms = None  # (q, qs, qss) -> (a, b, c): the fused terms launch of the batched route
         self._eye_form = None  # (g [k] or [B,k], friction [m] or None): F = [I;-I] fast form
+        self._const_F = None  # F (k, m) shared by every gridpoint, g = 0
         self._format_string = "    Kind: Generalized Second-order constraint\n"
         self._format_string = "    Dimension:\n"
         if not batched:
@@ -73,6 +79,8 @@ class SecondOrderConstraint(LinearConstraint):
             custom_term = lambda path, s: np.sign(path(s, 1)) * joint_friction  # noqa: E731
         obj = cls(inv_dyn, constraint_F, constraint_g, dof, custom_term, **kwargs)
         obj._eye_form = (g_aug, joint_friction)
+        if isinstance(inv_dyn, RigidBodyModel):
+            obj.device_terms = lambda q, qs, qss: inv_dyn.torque_terms(q, qs, qss, joint_friction)
         obj._taulim = taulim
         obj.device_model = device_model
         return obj
@@ -99,9 +107,7 @@ class SecondOrderConstraint(LinearConstraint):
         return a, b, c, F, g
 
     def compute_constraint_params(self, path, gridpoints):
-        if path.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, path.dof))
+        check_dof(self.dof, path.dof)
         if self.batched:
             raise NotImplementedError("batched SecondOrderConstraint: use BatchTOPPRA / TOPPRA, not the host 7-tuple")
         a_vec, b_vec, c_vec, F_vec, g_vec = self._colloc_host(path, np.asarray(gridpoints))
@@ -115,11 +121,18 @@ class SecondOrderConstraint(LinearConstraint):
     def _k(self):
         if self._eye_form is not None:
             return self._eye_form[0].shape[-1]   # F = [I; -I]: 2 dof rows for torques, 2 k for frame accelerations
+        if self._const_F is not None:
+            return self._const_F.shape[0]
         if self.batched:
             raise NotImplementedError("batched SecondOrderConstraint with a general F: use joint_torque_constraint")
         return self.constraint_F(np.zeros(self.dof)).shape[0]
 
+    def _check_batch(self, ctx):
+        """The checks of the device route, before its rows are counted and before they are written."""
+        check_dof(self.dof, ctx.bpath.dof)
+
     def num_rows(self, ctx):
+        self._check_batch(ctx)
         return (2 if self.interpolation else 1) * self._k()
 
     def _colloc_device(self, ctx):
@@ -131,14 +144,10 @@ class SecondOrderConstraint(LinearConstraint):
             q = bp.eval_device(ctx.d_grid, 0).reshape(B * G, dof)
             qd = bp.eval_device(ctx.d_grid, 1).reshape(B * G, dof)
             qdd = bp.eval_device(ctx.d_grid, 2).reshape(B * G, dof)
-            if isinstance(self.inv_dyn, RigidBodyModel) and self._eye_form is not None:
-                a, b, c = self.inv_dyn.torque_terms(q, qd, qdd, self._eye_form[1])
-                return (a.reshape(B, G, dof), b.reshape(B, G, dof), c.reshape(B, G, dof))
-            if isinstance(self.inv_dyn, RigidBodyFrame) and self._eye_form is not None:
-                # CartesianAccelerationConstraint: acc(q, 0, 0) = 0, so c = 0 and a, b need no subtraction
-                a, b = self.inv_dyn.acceleration_terms(q, qd, qdd, self.components)
-                m = a.shape[-1]
-                return a.reshape(B, G, m), b.reshape(B, G, m), torch.zeros((B, G, m), dtype=a.dtype, device=a.device)
+            if self.device_terms is not None:
+                a, b, c = self.device_terms(q, qd, qdd)
+                m = c.shape[-1]
+                return a.reshape(B, G, m), b.reshape(B, G, m), c.reshape(B, G, m)
             zero = torch.zeros_like(q)
             c = self.inv_dyn(q, zero, zero)
             a = self.inv_dyn(q, zero, qd) - c
@@ -158,9 +167,7 @@ class SecondOrderConstraint(LinearConstraint):
         return d(a), d(b), d(c)
 
     def append_records(self, ctx, records, R_total, row0):
-        if ctx.bpath.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, ctx.bpath.dof))
+        self._check_batch(ctx)
         if self.device_model is not None:
             cache = self.__dict__.setdefault("_d_taulim", {})   # limits stay resident across solves and chunks
             if str(ctx.device) not in cache:
@@ -181,6 +188,10 @@ class SecondOrderConstraint(LinearConstraint):
                 gd = gd[ctx.lo:ctx.hi].contiguous()
             mode = 2 if g.ndim == 1 else 3
             engine.rows_canlinear(a, b, c, None, gd, mode, ctx.d_grid, self.interpolation, records, R_total, row0)
+        elif self._const_F is not None:
+            Fd = engine.as_device(self._const_F, ctx.device)
+            gd = engine.as_device(np.zeros(self._const_F.shape[0]), ctx.device)
+            engine.rows_canlinear(a, b, c, Fd, gd, 0, ctx.d_grid, self.interpolation, records, R_total, row0)
         else:
             F, g = self._host_Fg
             Fd = engine.as_device(np.asarray(F, dtype=np.float64)[None], ctx.device)

@@ -14,15 +14,15 @@ normal, pointing into the robot.  In support axes, at the support origin, the su
 and the ZMP is (-tau_y / f_z, tau_x / f_z).  F is either the contact wrench cone of a rectangular footprint with
 friction (`contact_wrench_cone`: sliding, tipping and twisting; Caron, Pham, Nakamura, ICRA 2015) or the rows of a
 convex footprint polygon (`support_polygon_rows`: one ZMP row per edge, plus four sliding rows with friction).  Every
-a, b and c of the batch (or record chunk) come from ONE `tbd_support_wrench_terms` launch, and the rows go through
-`tb_rows_canlinear` with the shared F and g = 0.  So TOPPRA, BatchTOPPRA, BatchTOPPRAsd, feasible, reachable and
+a, b and c of the batch (or record chunk) come from ONE `tbd_support_wrench_terms` launch (the constraint's
+`device_terms`), and the rows go through `tb_rows_canlinear` with the shared F and g = 0 (the constant-F form of
+`SecondOrderConstraint`).  So TOPPRA, BatchTOPPRA, BatchTOPPRAsd, feasible, reachable and
 controllable sets, ragged grids, record chunks and order-k paths take it unchanged."""
 import numpy as np
 
 from .constraint import DiscretizationType
-from .contact_stability import contact_wrench_cone
+from .contact_stability import contact_wrench_cone, friction_of, half_lengths_of
 from .linear_second_order import SecondOrderConstraint
-from .. import engine
 from ..dynamics import RigidBodyFrame, _base_inertia
 
 
@@ -50,17 +50,6 @@ def _polygon(vertices):
     return v
 
 
-def _friction(friction):
-    mu = np.asarray(friction, dtype=np.float64)
-    if mu.shape != ():
-        raise ValueError("support: friction must be a scalar; got shape %s" % (mu.shape,))
-    if not np.isfinite(mu):
-        raise ValueError("support: friction must be finite")
-    if not mu > 0:
-        raise ValueError("support: friction %r must be positive" % float(mu))
-    return float(mu)
-
-
 def support_polygon_rows(vertices, friction=None):
     """F (n or n + 4, 6): rows on the wrench w = [f; tau] at the support origin (support axes) that keep the centre of
     pressure (-tau_y / f_z, tau_x / f_z) inside the convex polygon `vertices` ((n, 2), counter-clockwise seen from +z,
@@ -77,21 +66,10 @@ def support_polygon_rows(vertices, friction=None):
     F[:, 4] = -e[:, 1]
     F = F / np.hypot(e[:, 0], e[:, 1])[:, None]
     if friction is not None:
-        mu = _friction(friction)
+        mu = friction_of(friction)
         F = np.vstack((F, [[1.0, 0.0, -mu, 0.0, 0.0, 0.0], [-1.0, 0.0, -mu, 0.0, 0.0, 0.0],
                            [0.0, 1.0, -mu, 0.0, 0.0, 0.0], [0.0, -1.0, -mu, 0.0, 0.0, 0.0]]))
     return F
-
-
-def _half_lengths(half_lengths):
-    hl = np.asarray(half_lengths, dtype=np.float64)
-    if hl.shape != (2,):
-        raise ValueError("support: half_lengths must be (X, Y); got shape %s" % (hl.shape,))
-    if not np.isfinite(hl).all():
-        raise ValueError("support: half_lengths must be finite")
-    if not (hl > 0).all():
-        raise ValueError("support: half_lengths must be positive; got %s" % hl)
-    return float(hl[0]), float(hl[1])
 
 
 class SupportStabilityConstraint(SecondOrderConstraint):
@@ -120,9 +98,9 @@ class SupportStabilityConstraint(SecondOrderConstraint):
                                   model.base_mass if base_mass is None else base_mass,
                                   model.base_com if base_com is None else base_com)
         if half_lengths is not None:
-            X, Y = _half_lengths(half_lengths)
+            X, Y = half_lengths_of(half_lengths)
             if friction is not None:
-                F = contact_wrench_cone((X, Y), _friction(friction))
+                F = contact_wrench_cone((X, Y), friction)
             else:
                 F = support_polygon_rows([[-X, -Y], [X, -Y], [X, Y], [-X, Y]])
             self.half_lengths, self.polygon = (X, Y), None
@@ -133,9 +111,10 @@ class SupportStabilityConstraint(SecondOrderConstraint):
         super(SupportStabilityConstraint, self).__init__(self.wrench, lambda _: F, lambda _: zeros, support.nv,
                                                          discretization_scheme=discretization_scheme, batched=True)
         self.support = support
-        self.F = F
+        self.F = self._const_F = F
         self.friction = None if friction is None else float(friction)
         self.base = np.concatenate(([mass], com))
+        self.device_terms = lambda q, qs, qss: support.support_wrench_terms(self.base, q, qs, qss)
         self._format_string = "    Kind: support stability on frame %r, %d rows\n" % (support.name, F.shape[0])
 
     def wrench(self, q, qd, qdd):
@@ -152,30 +131,3 @@ class SupportStabilityConstraint(SecondOrderConstraint):
             return np.stack((x, y), axis=-1)
         import torch
         return torch.stack((x, y), dim=-1)
-
-    def _k(self):
-        return self.F.shape[0]
-
-    def _check_batch(self, ctx):
-        if ctx.bpath.dof != self.dof:
-            raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to path dof ({:d})".format(
-                self.dof, ctx.bpath.dof))
-
-    def num_rows(self, ctx):
-        self._check_batch(ctx)
-        return super(SupportStabilityConstraint, self).num_rows(ctx)
-
-    def _colloc_device(self, ctx):
-        """(a, b, c) as CUDA tensors [B, G, 6]: one tbd_support_wrench_terms launch for the batch or chunk."""
-        bp = ctx.bpath
-        B, G, dof = ctx.B, ctx.G, bp.dof
-        q, qd, qdd = (bp.eval_device(ctx.d_grid, o).reshape(B * G, dof) for o in (0, 1, 2))
-        a, b, c = self.support.support_wrench_terms(self.base, q, qd, qdd)
-        return a.reshape(B, G, 6), b.reshape(B, G, 6), c.reshape(B, G, 6)
-
-    def append_records(self, ctx, records, R_total, row0):
-        self._check_batch(ctx)
-        a, b, c = self._colloc_device(ctx)
-        Fd = engine.as_device(self.F, ctx.device)
-        gd = engine.as_device(np.zeros(self.F.shape[0]), ctx.device)
-        engine.rows_canlinear(a, b, c, Fd, gd, 0, ctx.d_grid, self.interpolation, records, R_total, row0)

@@ -792,16 +792,18 @@ int load_model(const double *host, const int nv, const int M, DynModel *m, const
 }
 
 // Validates the packed frame (include/toppra_b200_dyn.h) of a model already loaded by load_model and copies it, the
-// root-to-body chain and S (nullable) into the by-value launch parameter: 0, or the TB_ERR_* code (message set).
-int load_frame(const double *host, const DynModel &m, const int nv, const double *S, DynFrame *f, const char *what) {
+// root-to-body chain and S (nullable) into the by-value launch parameter: 0, or the TB_ERR_* code (message set).  `ref`
+// replaces the frame's reference-frame field (-1: as given), for entries whose result is always in one frame's axes.
+int load_frame(const double *host, const DynModel &m, const int nv, const double *S, const int ref, DynFrame *f,
+               const char *what) {
   const double body = host[0];
   if (!(body >= -1.0 && body < (double)nv && body == std::floor(body))) {
     set_error("%s: frame body %g must be an integer in [-1, %d)", what, body, nv);
     return TB_ERR_ARG;
   }
-  const double ref = host[13];
-  if (ref != TBD_WORLD && ref != TBD_LOCAL && ref != TBD_LOCAL_WORLD_ALIGNED) {
-    set_error("%s: unknown reference frame %g", what, ref);
+  const double r = ref >= 0 ? (double)ref : host[13];
+  if (r != TBD_WORLD && r != TBD_LOCAL && r != TBD_LOCAL_WORLD_ALIGNED) {
+    set_error("%s: unknown reference frame %g", what, r);
     return TB_ERR_ARG;
   }
   for (int j = 0; j < 12; ++j)
@@ -812,12 +814,51 @@ int load_frame(const double *host, const DynModel &m, const int nv, const double
     f->S[j] = S ? S[j] : 0.0;
     if (!std::isfinite(f->S[j])) { set_error("%s: S is not finite", what); return TB_ERR_ARG; }
   }
-  f->ref = (int)ref;
+  f->ref = (int)r;
   int n = 0;
   for (int k = (int)body; k >= 0; k = (int)m.body[k][0]) ++n;   // parents are validated: parent[k] < k
   f->n = n;
   for (int k = (int)body, i = n - 1; k >= 0; k = (int)m.body[k][0], --i) f->chain[i] = k;
   for (int i = n; i < NB; ++i) f->chain[i] = 0;
+  return 0;
+}
+
+// Frame accelerations and the inverse inertia are those of the frame origin: a quantity "at the world origin" is no
+// limit a user means, so TBD_WORLD is TB_ERR_UNSUPPORTED.
+int refuse_world(const DynFrame &f, const char *what, const char *quantity) {
+  if (f.ref != TBD_WORLD) return 0;
+  set_error("%s: the world reference frame is not supported%s (use local or local_world_aligned)", what, quantity);
+  return TB_ERR_UNSUPPORTED;
+}
+
+// The packed object (TBD_OBJECT_DOUBLES): finite, with a positive mass.
+int load_object(const double *host, DynObject *o, const char *what) {
+  for (int j = 0; j < TBD_OBJECT_DOUBLES; ++j)
+    if (!std::isfinite(host[j])) { set_error("%s: object parameters are not finite", what); return TB_ERR_ARG; }
+  if (!(host[0] > 0.0)) { set_error("%s: object mass %g must be positive", what, host[0]); return TB_ERR_ARG; }
+  o->mass = host[0];
+  for (int j = 0; j < 3; ++j) o->r[j] = host[1 + j];
+  for (int j = 0; j < 6; ++j) o->Ic[j] = host[4 + j];
+  return 0;
+}
+
+// The packed base (TBD_BASE_DOUBLES): finite, with a non-negative mass.
+int load_base(const double *host, DynBase *base, const char *what) {
+  for (int j = 0; j < TBD_BASE_DOUBLES; ++j)
+    if (!std::isfinite(host[j])) { set_error("%s: base parameters are not finite", what); return TB_ERR_ARG; }
+  if (!(host[0] >= 0.0)) { set_error("%s: base mass %g must be non-negative", what, host[0]); return TB_ERR_ARG; }
+  base->mass = host[0];
+  for (int j = 0; j < 3; ++j) base->c[j] = host[1 + j];
+  return 0;
+}
+
+// The support wrench is that of a support frame on the base, in its own axes.
+int load_support(const double *host, const DynModel &m, const int nv, DynFrame *s, const char *what) {
+  if (const int rc = load_frame(host, m, nv, nullptr, TBD_LOCAL, s, what)) return rc;
+  if (host[0] != -1.0) {
+    set_error("%s: the support must be on the base (frame body %g, expected -1)", what, host[0]);
+    return TB_ERR_ARG;
+  }
   return 0;
 }
 
@@ -856,7 +897,7 @@ extern "C" int tbd_frame_velocity(const double *model_host, int nv, const double
   DynModel m;
   if (const int rc = load_model(model_host, nv, M, &m, "tbd_frame_velocity")) return rc;
   DynFrame f;
-  if (const int rc = load_frame(frame_host, m, nv, nullptr, &f, "tbd_frame_velocity")) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, "tbd_frame_velocity")) return rc;
   frame_velocity_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qd, v);
   return launch_status("tbd_frame_velocity");
 }
@@ -871,27 +912,10 @@ extern "C" int tbd_velocity_norm_terms(const double *model_host, int nv, const d
   DynModel m;
   if (const int rc = load_model(model_host, nv, M, &m, "tbd_velocity_norm_terms")) return rc;
   DynFrame f;
-  if (const int rc = load_frame(frame_host, m, nv, S_host, &f, "tbd_velocity_norm_terms")) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, S_host, -1, &f, "tbd_velocity_norm_terms")) return rc;
   velocity_norm_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qs, b);
   return launch_status("tbd_velocity_norm_terms");
 }
-
-namespace {
-// load_model and load_frame, then refuse TBD_WORLD: a classical acceleration "at the world origin" is no limit a user
-// means.
-int load_accel(const double *model_host, const int nv, const double *frame_host, const int M, tb::DynModel *m,
-               tb::DynFrame *f, const char *what) {
-  using namespace tb;
-  if (const int rc = load_model(model_host, nv, M, m, what)) return rc;
-  if (const int rc = load_frame(frame_host, *m, nv, nullptr, f, what)) return rc;
-  if (f->ref == TBD_WORLD) {
-    set_error("%s: the world reference frame is not supported for accelerations (use local or local_world_aligned)",
-              what);
-    return TB_ERR_UNSUPPORTED;
-  }
-  return 0;
-}
-}  // namespace
 
 extern "C" int tbd_frame_acceleration(const double *model_host, int nv, const double *frame_host, int M,
                                       const double *q, const double *qd, const double *qdd, double *acc, void *stream) {
@@ -902,7 +926,9 @@ extern "C" int tbd_frame_acceleration(const double *model_host, int nv, const do
   }
   DynModel m;
   DynFrame f;
-  if (const int rc = load_accel(model_host, nv, frame_host, M, &m, &f, "tbd_frame_acceleration")) return rc;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_frame_acceleration")) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, "tbd_frame_acceleration")) return rc;
+  if (const int rc = refuse_world(f, "tbd_frame_acceleration", " for accelerations")) return rc;
   frame_acceleration_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qd, qdd, acc);
   return launch_status("tbd_frame_acceleration");
 }
@@ -921,34 +947,16 @@ extern "C" int tbd_acceleration_terms(const double *model_host, int nv, const do
   }
   DynModel m;
   DynFrame f;
-  if (const int rc = load_accel(model_host, nv, frame_host, M, &m, &f, "tbd_acceleration_terms")) return rc;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_acceleration_terms")) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, "tbd_acceleration_terms")) return rc;
+  if (const int rc = refuse_world(f, "tbd_acceleration_terms", " for accelerations")) return rc;
   const int k = __builtin_popcount((unsigned)components);
   acceleration_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, components, k, M, q, qs, qss,
                                                                               a, b);
   return launch_status("tbd_acceleration_terms");
 }
 
-namespace {
-// load_model and load_frame with the frame's reference-frame field ignored (a contact wrench is always in the frame's
-// own axes), then the object: finite, with a positive mass.
-int load_contact(const double *model_host, const int nv, const double *frame_host, const double *object_host,
-                 const int M, tb::DynModel *m, tb::DynFrame *f, tb::DynObject *o, const char *what) {
-  using namespace tb;
-  if (const int rc = load_model(model_host, nv, M, m, what)) return rc;
-  double frame[TBD_FRAME_DOUBLES];
-  for (int j = 0; j < TBD_FRAME_DOUBLES; ++j) frame[j] = frame_host[j];
-  frame[13] = TBD_LOCAL;
-  if (const int rc = load_frame(frame, *m, nv, nullptr, f, what)) return rc;
-  for (int j = 0; j < TBD_OBJECT_DOUBLES; ++j)
-    if (!std::isfinite(object_host[j])) { set_error("%s: object parameters are not finite", what); return TB_ERR_ARG; }
-  if (!(object_host[0] > 0.0)) { set_error("%s: object mass %g must be positive", what, object_host[0]); return TB_ERR_ARG; }
-  o->mass = object_host[0];
-  for (int j = 0; j < 3; ++j) o->r[j] = object_host[1 + j];
-  for (int j = 0; j < 6; ++j) o->Ic[j] = object_host[4 + j];
-  return 0;
-}
-}  // namespace
-
+// The contact wrench is always in the contact frame's own axes: its reference-frame field is ignored.
 extern "C" int tbd_contact_wrench(const double *model_host, int nv, const double *frame_host, const double *object_host,
                                   int M, const double *q, const double *qd, const double *qdd, double *w,
                                   void *stream) {
@@ -960,7 +968,9 @@ extern "C" int tbd_contact_wrench(const double *model_host, int nv, const double
   DynModel m;
   DynFrame f;
   DynObject o;
-  if (const int rc = load_contact(model_host, nv, frame_host, object_host, M, &m, &f, &o, "tbd_contact_wrench")) return rc;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_contact_wrench")) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL, &f, "tbd_contact_wrench")) return rc;
+  if (const int rc = load_object(object_host, &o, "tbd_contact_wrench")) return rc;
   contact_wrench_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, o, nv, M, q, qd, qdd, w);
   return launch_status("tbd_contact_wrench");
 }
@@ -976,24 +986,12 @@ extern "C" int tbd_contact_wrench_terms(const double *model_host, int nv, const 
   DynModel m;
   DynFrame f;
   DynObject o;
-  if (const int rc = load_contact(model_host, nv, frame_host, object_host, M, &m, &f, &o, "tbd_contact_wrench_terms"))
-    return rc;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_contact_wrench_terms")) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL, &f, "tbd_contact_wrench_terms")) return rc;
+  if (const int rc = load_object(object_host, &o, "tbd_contact_wrench_terms")) return rc;
   contact_wrench_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, o, nv, M, q, qs, qss, a, b, c);
   return launch_status("tbd_contact_wrench_terms");
 }
-
-namespace {
-// load_model, then load_frame with the reference-frame field set to `ref` (or as given when ref < 0).
-int load_energy(const double *model_host, const int nv, const double *frame_host, const int M, const int ref,
-                tb::DynModel *m, tb::DynFrame *f, const char *what) {
-  using namespace tb;
-  if (const int rc = load_model(model_host, nv, M, m, what)) return rc;
-  double frame[TBD_FRAME_DOUBLES];
-  for (int j = 0; j < TBD_FRAME_DOUBLES; ++j) frame[j] = frame_host[j];
-  if (ref >= 0) frame[13] = ref;
-  return load_frame(frame, *m, nv, nullptr, f, what);
-}
-}  // namespace
 
 extern "C" int tbd_frame_inverse_inertia(const double *model_host, int nv, const double *frame_host, int M,
                                          const double *q, double *Linv, void *stream) {
@@ -1001,15 +999,14 @@ extern "C" int tbd_frame_inverse_inertia(const double *model_host, int nv, const
   if (!model_host || !frame_host || !q || !Linv) { set_error("tbd_frame_inverse_inertia: null pointer"); return TB_ERR_ARG; }
   DynModel m;
   DynFrame f;
-  if (const int rc = load_energy(model_host, nv, frame_host, M, -1, &m, &f, "tbd_frame_inverse_inertia")) return rc;
-  if (f.ref == TBD_WORLD) {
-    set_error("tbd_frame_inverse_inertia: the world reference frame is not supported (use local or local_world_aligned)");
-    return TB_ERR_UNSUPPORTED;
-  }
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_frame_inverse_inertia")) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, "tbd_frame_inverse_inertia")) return rc;
+  if (const int rc = refuse_world(f, "tbd_frame_inverse_inertia", "")) return rc;
   frame_inverse_inertia_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, Linv);
   return launch_status("tbd_frame_inverse_inertia");
 }
 
+// The collision energy needs the world linear velocity: the frame is read as TBD_LOCAL_WORLD_ALIGNED.
 extern "C" int tbd_collision_energy_terms(const double *model_host, int nv, const double *frame_host, double human_mass,
                                           int M, const double *q, const double *qs, double *b, void *stream) {
   using namespace tb;
@@ -1023,36 +1020,12 @@ extern "C" int tbd_collision_energy_terms(const double *model_host, int nv, cons
   }
   DynModel m;
   DynFrame f;
-  if (const int rc = load_energy(model_host, nv, frame_host, M, TBD_LOCAL_WORLD_ALIGNED, &m, &f,
-                                 "tbd_collision_energy_terms"))
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_collision_energy_terms")) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL_WORLD_ALIGNED, &f, "tbd_collision_energy_terms"))
     return rc;
   collision_energy_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, human_mass, M, q, qs, b);
   return launch_status("tbd_collision_energy_terms");
 }
-
-namespace {
-// load_model and load_frame with the frame's reference-frame field ignored (the support wrench is always in the
-// support's own axes); the support must be on the base.  Then the base: finite, with a non-negative mass.
-int load_support(const double *model_host, const int nv, const double *frame_host, const double *base_host,
-                 const int M, tb::DynModel *m, tb::DynFrame *s, tb::DynBase *base, const char *what) {
-  using namespace tb;
-  if (const int rc = load_model(model_host, nv, M, m, what)) return rc;
-  double frame[TBD_FRAME_DOUBLES];
-  for (int j = 0; j < TBD_FRAME_DOUBLES; ++j) frame[j] = frame_host[j];
-  frame[13] = TBD_LOCAL;
-  if (const int rc = load_frame(frame, *m, nv, nullptr, s, what)) return rc;
-  if (frame[0] != -1.0) {
-    set_error("%s: the support must be on the base (frame body %g, expected -1)", what, frame[0]);
-    return TB_ERR_ARG;
-  }
-  for (int j = 0; j < TBD_BASE_DOUBLES; ++j)
-    if (!std::isfinite(base_host[j])) { set_error("%s: base parameters are not finite", what); return TB_ERR_ARG; }
-  if (!(base_host[0] >= 0.0)) { set_error("%s: base mass %g must be non-negative", what, base_host[0]); return TB_ERR_ARG; }
-  base->mass = base_host[0];
-  for (int j = 0; j < 3; ++j) base->c[j] = base_host[1 + j];
-  return 0;
-}
-}  // namespace
 
 extern "C" int tbd_support_wrench(const double *model_host, int nv, const double *frame_host, const double *base_host,
                                   int M, const double *q, const double *qd, const double *qdd, double *w,
@@ -1065,7 +1038,9 @@ extern "C" int tbd_support_wrench(const double *model_host, int nv, const double
   DynModel m;
   DynFrame s;
   DynBase base;
-  if (const int rc = load_support(model_host, nv, frame_host, base_host, M, &m, &s, &base, "tbd_support_wrench")) return rc;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_support_wrench")) return rc;
+  if (const int rc = load_support(frame_host, m, nv, &s, "tbd_support_wrench")) return rc;
+  if (const int rc = load_base(base_host, &base, "tbd_support_wrench")) return rc;
   support_wrench_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, s, base, nv, M, q, qd, qdd, w);
   return launch_status("tbd_support_wrench");
 }
@@ -1081,8 +1056,9 @@ extern "C" int tbd_support_wrench_terms(const double *model_host, int nv, const 
   DynModel m;
   DynFrame s;
   DynBase base;
-  if (const int rc = load_support(model_host, nv, frame_host, base_host, M, &m, &s, &base, "tbd_support_wrench_terms"))
-    return rc;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_support_wrench_terms")) return rc;
+  if (const int rc = load_support(frame_host, m, nv, &s, "tbd_support_wrench_terms")) return rc;
+  if (const int rc = load_base(base_host, &base, "tbd_support_wrench_terms")) return rc;
   support_wrench_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, s, base, nv, M, q, qs, qss, a, b, c);
   return launch_status("tbd_support_wrench_terms");
 }

@@ -177,9 +177,6 @@ class RigidBodyModel(object):
         return [self.joint_names[k] for k in range(self.nv) if empty[k]]
 
     # ---- evaluation on the GPU ----------------------------------------------------------------------------------
-    def _model_ptr(self):
-        return ctypes.c_void_p(self.packed.ctypes.data)
-
     def _prepare(self, torch, *xs):
         out = []
         for x in xs:
@@ -193,35 +190,18 @@ class RigidBodyModel(object):
     def __call__(self, q, qd, qdd):
         """Joint torques tau = M(q) qdd + h(q, qd) + g(q).  CUDA tensors (M, nv) -> (M, nv), one tbd_rnea launch on the
         current stream; numpy (nv,) or (M, nv) -> numpy, through a device round trip."""
-        torch = _lib.require_cuda()
-        if isinstance(q, torch.Tensor) and q.is_cuda:
-            q, qd, qdd = self._prepare(torch, q, qd, qdd)
-            tau = torch.empty_like(q)
-            with torch.cuda.device(q.device):
-                _lib.check(_lib_dyn.load().tbd_rnea(self._model_ptr(), self.nv, q.shape[0], _lib.ptr(q), _lib.ptr(qd),
-                                                    _lib.ptr(qdd), _lib.ptr(tau), _lib.stream_ptr()), "tbd_rnea")
-            return tau
-        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd, qdd)]
-        single = arrs[0].ndim == 1
-        dev = [torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]
-        tau = self(*dev).cpu().numpy()
-        return tau[0] if single else tau
+        if not _is_cuda(q):
+            return _round_trip(self, q, qd, qdd)
+        return _launch(self, "tbd_rnea", (), (q, qd, qdd), [(self.nv,)])
 
     def torque_terms(self, q, qs, qss, friction=None):
         """The terms of SecondOrderConstraint for CUDA tensors (M, nv), one tbd_torque_terms launch:
         c = ID(q, 0, 0), a = ID(q, 0, qs) - c, b = ID(q, qs, qss) - c, c += sign(qs) * friction (friction (nv,) or
         None).  Returns (a, b, c)."""
-        torch = _lib.require_cuda()
-        q, qs, qss = self._prepare(torch, q, qs, qss)
-        a, b, c = torch.empty_like(q), torch.empty_like(q), torch.empty_like(q)
         fric = None
         if friction is not None and np.any(np.asarray(friction) != 0):
-            fric = torch.as_tensor(np.broadcast_to(np.asarray(friction, dtype=np.float64), (self.nv,)).copy(), device=q.device)
-        with torch.cuda.device(q.device):
-            _lib.check(_lib_dyn.load().tbd_torque_terms(self._model_ptr(), self.nv, q.shape[0], _lib.ptr(q), _lib.ptr(qs),
-                                                        _lib.ptr(qss), _lib.ptr(fric), _lib.ptr(a), _lib.ptr(b),
-                                                        _lib.ptr(c), _lib.stream_ptr()), "tbd_torque_terms")
-        return a, b, c
+            fric = np.broadcast_to(np.asarray(friction, dtype=np.float64), (self.nv,)).copy()
+        return _launch(self, "tbd_torque_terms", (), (q, qs, qss), [(self.nv,)] * 3, extra=(fric,))
 
     # ---- URDF ---------------------------------------------------------------------------------------------------
     @classmethod
@@ -367,49 +347,29 @@ class RigidBodyFrame(object):
     def nv(self):
         return self.model.nv
 
-    def _frame_ptr(self):
-        return ctypes.c_void_p(self.packed.ctypes.data)
-
     def __call__(self, q, qd):
         """Frame velocities.  CUDA tensors (M, nv) -> (M, 6), one tbd_frame_velocity launch on the current stream;
         numpy (nv,) -> (6,) or (M, nv) -> (M, 6), through a device round trip."""
-        torch = _lib.require_cuda()
-        m = self.model
-        if isinstance(q, torch.Tensor) and q.is_cuda:
-            q, qd = m._prepare(torch, q, qd)
-            v = torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device)
-            with torch.cuda.device(q.device):
-                _lib.check(_lib_dyn.load().tbd_frame_velocity(m._model_ptr(), m.nv, self._frame_ptr(), q.shape[0],
-                                                              _lib.ptr(q), _lib.ptr(qd), _lib.ptr(v), _lib.stream_ptr()),
-                           "tbd_frame_velocity")
-            return v
-        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd)]
-        single = arrs[0].ndim == 1
-        v = self(*[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
-        return v[0] if single else v
+        if not _is_cuda(q):
+            return _round_trip(self, q, qd)
+        return _launch(self.model, "tbd_frame_velocity", (self.packed,), (q, qd), [(6,)])
 
     def velocity_norm_terms(self, q, qs, S):
         """b = v^T (S v), v the frame velocity at (q, qs = q'), for CUDA tensors (M, nv) -> (M,): one
         tbd_velocity_norm_terms launch.  S: (6, 6)."""
-        torch = _lib.require_cuda()
-        m = self.model
-        q, qs = m._prepare(torch, q, qs)
         S = np.ascontiguousarray(S, dtype=np.float64)
         if S.shape != (6, 6):
             raise ValueError("S matrix should be of size 6x6.")
-        b = torch.empty(q.shape[0], dtype=torch.float64, device=q.device)
-        with torch.cuda.device(q.device):
-            _lib.check(_lib_dyn.load().tbd_velocity_norm_terms(m._model_ptr(), m.nv, self._frame_ptr(),
-                                                               ctypes.c_void_p(S.ctypes.data), q.shape[0], _lib.ptr(q),
-                                                               _lib.ptr(qs), _lib.ptr(b), _lib.stream_ptr()),
-                       "tbd_velocity_norm_terms")
-        return b
+        return _launch(self.model, "tbd_velocity_norm_terms", (self.packed, S), (q, qs), [()])
+
+    def _refuse_world(self, quantity):
+        """ValueError for a "world" frame where `quantity` is one of the frame origin."""
+        if self.reference_frame == "world":
+            raise ValueError("RigidBodyFrame %r: %s; the \"world\" reference frame is not supported (use \"local\" or "
+                             "\"local_world_aligned\")" % (self.name, quantity))
 
     def _check_acceleration(self):
-        if self.reference_frame == "world":
-            raise ValueError("RigidBodyFrame %r: frame accelerations are classical accelerations of the frame origin; "
-                             "the \"world\" reference frame is not supported (use \"local\" or \"local_world_aligned\")"
-                             % self.name)
+        self._refuse_world("frame accelerations are classical accelerations of the frame origin")
 
     def acceleration(self, q, qd, qdd):
         """Classical frame accelerations [linear(3); angular(3)] (pinocchio's getFrameClassicalAcceleration, no
@@ -417,21 +377,9 @@ class RigidBodyFrame(object):
         (M, nv) -> (M, 6), one tbd_frame_acceleration launch on the current stream; numpy (nv,) -> (6,) or (M, nv) ->
         (M, 6), through a device round trip.  On one numpy point it is an `inv_dyn` of SecondOrderConstraint."""
         self._check_acceleration()
-        torch = _lib.require_cuda()
-        m = self.model
-        if isinstance(q, torch.Tensor) and q.is_cuda:
-            q, qd, qdd = m._prepare(torch, q, qd, qdd)
-            acc = torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device)
-            with torch.cuda.device(q.device):
-                _lib.check(_lib_dyn.load().tbd_frame_acceleration(m._model_ptr(), m.nv, self._frame_ptr(), q.shape[0],
-                                                                  _lib.ptr(q), _lib.ptr(qd), _lib.ptr(qdd),
-                                                                  _lib.ptr(acc), _lib.stream_ptr()),
-                           "tbd_frame_acceleration")
-            return acc
-        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd, qdd)]
-        single = arrs[0].ndim == 1
-        acc = self.acceleration(*[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
-        return acc[0] if single else acc
+        if not _is_cuda(q):
+            return _round_trip(self.acceleration, q, qd, qdd)
+        return _launch(self.model, "tbd_frame_acceleration", (self.packed,), (q, qd, qdd), [(6,)])
 
     def acceleration_terms(self, q, qs, qss, components):
         """a = acc(q, 0, qs), b = acc(q, qs, qss) for CUDA tensors (M, nv), restricted to `components` (indices into
@@ -439,18 +387,8 @@ class RigidBodyFrame(object):
         Returns (a, b), each (M, k)."""
         self._check_acceleration()
         comps = component_indices(components)
-        torch = _lib.require_cuda()
-        m = self.model
-        q, qs, qss = m._prepare(torch, q, qs, qss)
-        a = torch.empty((q.shape[0], len(comps)), dtype=torch.float64, device=q.device)
-        b = torch.empty_like(a)
         mask = sum(1 << j for j in comps)
-        with torch.cuda.device(q.device):
-            _lib.check(_lib_dyn.load().tbd_acceleration_terms(m._model_ptr(), m.nv, self._frame_ptr(), mask, q.shape[0],
-                                                              _lib.ptr(q), _lib.ptr(qs), _lib.ptr(qss), _lib.ptr(a),
-                                                              _lib.ptr(b), _lib.stream_ptr()),
-                       "tbd_acceleration_terms")
-        return a, b
+        return _launch(self.model, "tbd_acceleration_terms", (self.packed, mask), (q, qs, qss), [(len(comps),)] * 2)
 
     def contact_wrench(self, obj, q, qd, qdd):
         """The wrench [f; tau] this frame, as a contact frame, exerts on an object it carries, at its origin in its own
@@ -458,38 +396,15 @@ class RigidBodyFrame(object):
         ContactStabilityConstraint).  CUDA tensors (M, nv) -> (M, 6), one tbd_contact_wrench launch on the current
         stream; numpy (nv,) -> (6,) or (M, nv) -> (M, 6), through a device round trip."""
         obj = _packed_object(obj)
-        torch = _lib.require_cuda()
-        m = self.model
-        if isinstance(q, torch.Tensor) and q.is_cuda:
-            q, qd, qdd = m._prepare(torch, q, qd, qdd)
-            w = torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device)
-            with torch.cuda.device(q.device):
-                _lib.check(_lib_dyn.load().tbd_contact_wrench(m._model_ptr(), m.nv, self._frame_ptr(),
-                                                              ctypes.c_void_p(obj.ctypes.data), q.shape[0], _lib.ptr(q),
-                                                              _lib.ptr(qd), _lib.ptr(qdd), _lib.ptr(w),
-                                                              _lib.stream_ptr()),
-                           "tbd_contact_wrench")
-            return w
-        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd, qdd)]
-        single = arrs[0].ndim == 1
-        w = self.contact_wrench(obj, *[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
-        return w[0] if single else w
+        if not _is_cuda(q):
+            return _round_trip(lambda *x: self.contact_wrench(obj, *x), q, qd, qdd)
+        return _launch(self.model, "tbd_contact_wrench", (self.packed, obj), (q, qd, qdd), [(6,)])
 
     def contact_wrench_terms(self, obj, q, qs, qss):
         """c = w(q, 0, 0), a = w(q, 0, qs) - c, b = w(q, qs, qss) - c of the contact wrench (contact_wrench) for CUDA
         tensors (M, nv): one tbd_contact_wrench_terms launch.  Returns (a, b, c), each (M, 6)."""
         obj = _packed_object(obj)
-        torch = _lib.require_cuda()
-        m = self.model
-        q, qs, qss = m._prepare(torch, q, qs, qss)
-        a, b, c = (torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device) for _ in range(3))
-        with torch.cuda.device(q.device):
-            _lib.check(_lib_dyn.load().tbd_contact_wrench_terms(m._model_ptr(), m.nv, self._frame_ptr(),
-                                                                ctypes.c_void_p(obj.ctypes.data), q.shape[0],
-                                                                _lib.ptr(q), _lib.ptr(qs), _lib.ptr(qss), _lib.ptr(a),
-                                                                _lib.ptr(b), _lib.ptr(c), _lib.stream_ptr()),
-                       "tbd_contact_wrench_terms")
-        return a, b, c
+        return _launch(self.model, "tbd_contact_wrench_terms", (self.packed, obj), (q, qs, qss), [(6,)] * 3)
 
     def inverse_inertia(self, q):
         """Lambda_v^-1 = J_v M(q)^-1 J_v^T of the frame origin: the inverse operational-space inertia for linear motion
@@ -497,44 +412,24 @@ class RigidBodyFrame(object):
         direction u.  "local_world_aligned": world axes; "local": R_f^T Lambda_v^-1 R_f; "world" raises ValueError.
         NaN where M(q) is singular.  CUDA tensors (M, nv) -> (M, 3, 3), one tbd_frame_inverse_inertia launch on the
         current stream; numpy (nv,) -> (3, 3) or (M, nv) -> (M, 3, 3), through a device round trip."""
-        if self.reference_frame == "world":
-            raise ValueError("RigidBodyFrame %r: the inverse inertia is that of the frame origin; the \"world\" "
-                             "reference frame is not supported (use \"local\" or \"local_world_aligned\")" % self.name)
-        torch = _lib.require_cuda()
-        m = self.model
-        if isinstance(q, torch.Tensor) and q.is_cuda:
-            q, = m._prepare(torch, q)
-            L = torch.empty((q.shape[0], 3, 3), dtype=torch.float64, device=q.device)
-            with torch.cuda.device(q.device):
-                _lib.check(_lib_dyn.load().tbd_frame_inverse_inertia(m._model_ptr(), m.nv, self._frame_ptr(),
-                                                                     q.shape[0], _lib.ptr(q), _lib.ptr(L),
-                                                                     _lib.stream_ptr()),
-                           "tbd_frame_inverse_inertia")
-            return L
-        q = np.asarray(q, dtype=np.float64)
-        L = self.inverse_inertia(torch.as_tensor(np.atleast_2d(q), device="cuda")).cpu().numpy()
-        return L[0] if q.ndim == 1 else L
+        self._refuse_world("the inverse inertia is that of the frame origin")
+        if not _is_cuda(q):
+            return _round_trip(self.inverse_inertia, q)
+        return _launch(self.model, "tbd_frame_inverse_inertia", (self.packed,), (q,), [(3, 3)])
 
     def collision_energy_terms(self, q, qs, human_mass):
         """b = 1/2 |v|^4 / (|v|^2 / m_H + v^T Lambda_v^-1 v), v the world linear velocity of the frame origin at
         (q, qs = q'), m_H = human_mass (> 0, inf allowed): the collision energy E = b s'^2 of
         CollisionEnergyConstraint, for CUDA tensors (M, nv) -> (M,): one tbd_collision_energy_terms launch.  The
         reference frame is ignored."""
-        torch = _lib.require_cuda()
-        m = self.model
-        q, qs = m._prepare(torch, q, qs)
-        b = torch.empty(q.shape[0], dtype=torch.float64, device=q.device)
-        with torch.cuda.device(q.device):
-            _lib.check(_lib_dyn.load().tbd_collision_energy_terms(m._model_ptr(), m.nv, self._frame_ptr(),
-                                                                  float(human_mass), q.shape[0], _lib.ptr(q),
-                                                                  _lib.ptr(qs), _lib.ptr(b), _lib.stream_ptr()),
-                       "tbd_collision_energy_terms")
-        return b
+        return _launch(self.model, "tbd_collision_energy_terms", (self.packed, float(human_mass)), (q, qs), [()])
 
-    def _check_support(self):
+    def _support_base(self, base):
+        """The packed base of a support frame, which must be on the base: the model's when `base` is None."""
         if self.body != -1:
             raise ValueError("RigidBodyFrame %r: the support must be on the base (frame body %d, expected -1)"
                              % (self.name, self.body))
+        return self.model.packed_base() if base is None else _packed_base(base)
 
     def support_wrench(self, base, q, qd, qdd):
         """The wrench [f; tau] the support exerts on the whole robot, at this frame's origin in its axes (the reference
@@ -543,41 +438,48 @@ class RigidBodyFrame(object):
         base_com).  CUDA tensors (M, nv) -> (M, 6), one tbd_support_wrench launch on the current stream; numpy (nv,) ->
         (6,) or (M, nv) -> (M, 6), through a device round trip: on one numpy point an `inv_dyn` of
         SecondOrderConstraint."""
-        self._check_support()
-        base = self.model.packed_base() if base is None else _packed_base(base)
-        torch = _lib.require_cuda()
-        m = self.model
-        if isinstance(q, torch.Tensor) and q.is_cuda:
-            q, qd, qdd = m._prepare(torch, q, qd, qdd)
-            w = torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device)
-            with torch.cuda.device(q.device):
-                _lib.check(_lib_dyn.load().tbd_support_wrench(m._model_ptr(), m.nv, self._frame_ptr(),
-                                                              ctypes.c_void_p(base.ctypes.data), q.shape[0],
-                                                              _lib.ptr(q), _lib.ptr(qd), _lib.ptr(qdd), _lib.ptr(w),
-                                                              _lib.stream_ptr()),
-                           "tbd_support_wrench")
-            return w
-        arrs = [np.asarray(x, dtype=np.float64) for x in (q, qd, qdd)]
-        single = arrs[0].ndim == 1
-        w = self.support_wrench(base, *[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
-        return w[0] if single else w
+        base = self._support_base(base)
+        if not _is_cuda(q):
+            return _round_trip(lambda *x: self.support_wrench(base, *x), q, qd, qdd)
+        return _launch(self.model, "tbd_support_wrench", (self.packed, base), (q, qd, qdd), [(6,)])
 
     def support_wrench_terms(self, base, q, qs, qss):
         """c = w(q, 0, 0), a = w(q, 0, qs) - c, b = w(q, qs, qss) - c of the support wrench (support_wrench) for CUDA
         tensors (M, nv): one tbd_support_wrench_terms launch.  Returns (a, b, c), each (M, 6)."""
-        self._check_support()
-        base = self.model.packed_base() if base is None else _packed_base(base)
-        torch = _lib.require_cuda()
-        m = self.model
-        q, qs, qss = m._prepare(torch, q, qs, qss)
-        a, b, c = (torch.empty((q.shape[0], 6), dtype=torch.float64, device=q.device) for _ in range(3))
-        with torch.cuda.device(q.device):
-            _lib.check(_lib_dyn.load().tbd_support_wrench_terms(m._model_ptr(), m.nv, self._frame_ptr(),
-                                                                ctypes.c_void_p(base.ctypes.data), q.shape[0],
-                                                                _lib.ptr(q), _lib.ptr(qs), _lib.ptr(qss), _lib.ptr(a),
-                                                                _lib.ptr(b), _lib.ptr(c), _lib.stream_ptr()),
-                       "tbd_support_wrench_terms")
-        return a, b, c
+        base = self._support_base(base)
+        return _launch(self.model, "tbd_support_wrench_terms", (self.packed, base), (q, qs, qss), [(6,)] * 3)
+
+
+def _is_cuda(x):
+    """Whether x is a CUDA tensor; there is no CPU route, so a CUDA device is required either way."""
+    torch = _lib.require_cuda()
+    return isinstance(x, torch.Tensor) and x.is_cuda
+
+
+def _round_trip(fn, *xs):
+    """fn, which takes CUDA tensors (M, nv), on numpy inputs: (nv,) -> one point, (M, nv) -> (M, ...)."""
+    torch = _lib.require_cuda()
+    arrs = [np.asarray(x, dtype=np.float64) for x in xs]
+    out = fn(*[torch.as_tensor(np.atleast_2d(x), device="cuda") for x in arrs]).cpu().numpy()
+    return out[0] if arrs[0].ndim == 1 else out
+
+
+def _launch(model, name, params, inputs, out_shapes, extra=()):
+    """One launch of the dyn entry `name` on the current stream; every entry takes (model, nv, *params, M, *inputs,
+    *extra, *outputs, stream).  params: host numpy arrays (passed by pointer) and scalars; inputs: (M, nv) CUDA tensors;
+    extra: host vectors copied to their device, or None for a null pointer; outputs: new float64 tensors (M,) + shape
+    for each of `out_shapes`.  Returns the output, or the tuple of outputs."""
+    torch = _lib.require_cuda()
+    inputs = model._prepare(torch, *inputs)
+    q = inputs[0]
+    extra = [None if x is None else torch.as_tensor(x, device=q.device) for x in extra]
+    outs = [torch.empty((q.shape[0],) + tuple(s), dtype=torch.float64, device=q.device) for s in out_shapes]
+    host = [ctypes.c_void_p(p.ctypes.data) if isinstance(p, np.ndarray) else p for p in params]
+    with torch.cuda.device(q.device):
+        _lib.check(getattr(_lib_dyn.load(), name)(ctypes.c_void_p(model.packed.ctypes.data), model.nv, *host,
+                                                  q.shape[0], *[_lib.ptr(x) for x in inputs + extra],
+                                                  *[_lib.ptr(o) for o in outs], _lib.stream_ptr()), name)
+    return outs[0] if len(outs) == 1 else tuple(outs)
 
 
 def _inertia3(I6):
