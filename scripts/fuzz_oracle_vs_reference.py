@@ -5,7 +5,11 @@ UNMODIFIED reference build (oracle/_ref) on randomly SHAPED problems — far mor
 and interpolation, active velocity bounds, non-zero boundary velocities (admissible or not), near-degenerate paths.
 Any mismatch is printed with the seed that reproduces it.
 
-usage: python scripts/fuzz_oracle_vs_reference.py [--minutes M] [--seed S]      (needs oracle/_ref, see oracle/build_ref.sh)"""
+With --long the problems are long paths instead (tests/problems.py: random_long_problem): 13..1000 knots on uniform, uneven
+and 5-decade spacings, 2..2*nseg gridpoints; only the solve, grid-proposal, TOPPRAsd and reachable-set checks run there.
+
+usage: python scripts/fuzz_oracle_vs_reference.py [--minutes M] [--seed S] [--long] [--problems N]
+       (needs oracle/_ref, see oracle/build_ref.sh; --problems stops after N problems, whatever --minutes says)"""
 import argparse
 import os
 import sys
@@ -363,19 +367,26 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--minutes", type=float, default=5.0)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--long", action="store_true", help="long paths (random_long_problem)")
+    ap.add_argument("--problems", type=int, default=None)
     args = ap.parse_args()
+    if args.long:
+        from problems import random_long_problem
     from oracle.ref_loader import load_reference
     use(load_reference())
     t_end = time.time() + 60 * args.minutes
     seed, bad, hist = args.seed, [], {}
-    while time.time() < t_end:
+    while time.time() < t_end and (args.problems is None or seed - args.seed < args.problems):
         rng = np.random.RandomState(seed)
-        p = random_problem(rng)
+        p = random_long_problem(rng) if args.long else random_problem(rng)
         try:
             st = check_solve(p)
             hist[st] = hist.get(st, 0) + 1
             check_frows(p, rng)
             check_sd_and_reachable(p, rng)
+            if args.long:
+                seed += 1
+                continue
             check_torque(p, rng)
             check_parametrizers(p, rng)
             check_ubound(p, rng)

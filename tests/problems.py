@@ -165,3 +165,57 @@ def random_shaped_problem(rng):
     while float(sd1) ** 2 != float(sd1) * float(sd1):
         sd1 = float(np.nextafter(sd1, 1.0))
     return dict(ss=ss, way=way, vlim=vlim, alim=alim, grid=grid, bc=str(bc), interp=interp_scheme, sd0=sd0, sd1=sd1)
+
+
+# ---- long paths (tests/test_long_paths.py, tests/golden/make_golden_long.py) ------------------------------------------------
+LONG_SPACINGS = ("uniform", "uneven", "decades")
+
+
+def long_breaks(rng, n, spacing):
+    """n strictly increasing breakpoints from 0: equal steps, steps in [0.05, 1.05), or steps spread over 5 decades
+    (1e-5 .. 1: the tridiagonal solve of the spline fit then interchanges rows often)."""
+    if spacing == "uniform":
+        return np.linspace(0.0, 0.5 * (n - 1), n)
+    step = 0.05 + rng.rand(n - 1) if spacing == "uneven" else 10 ** rng.uniform(-5, 0, n - 1)
+    return np.r_[0.0, np.cumsum(step)]
+
+
+def long_waypoints(rng, ss, dof):
+    """A random walk whose steps scale with sqrt(knot spacing): the derivatives stay moderate on dense knots."""
+    return rng.randn(1, dof) + np.r_[np.zeros((1, dof)), np.cumsum(rng.randn(len(ss) - 1, dof)
+                                                                   * np.sqrt(np.diff(ss))[:, None], axis=0)]
+
+
+def long_spline_data(n, spacing, seed, dof=1):
+    """The breakpoints and waypoints of one spline fit of tests/golden/long_paths.npz (regenerated, not stored)."""
+    rng = np.random.RandomState(seed)
+    ss = long_breaks(rng, n, spacing)
+    return ss, long_waypoints(rng, ss, dof)
+
+
+def random_long_problem(rng):
+    """One randomly shaped vel+acc problem on a LONG path (used by scripts/fuzz_oracle_vs_reference.py --long): dof 1..14,
+    13..1000 knots on uniform, uneven or 5-decade spacings, 2..2*nseg gridpoints, every boundary condition of the fit
+    except periodic, both discretisations, velocity-limited paths now and then, zero or small boundary velocities."""
+    dof = int(rng.choice([1, 2, 3, 6, 7, 7, 10, 14]))
+    n = int(rng.choice([13, 16, 17, 48, 49, 114, 115, 200, 400, 1000])) if rng.rand() < 0.4 else int(rng.randint(13, 1001))
+    ss = long_breaks(rng, n, LONG_SPACINGS[rng.randint(3)])
+    way = long_waypoints(rng, ss, dof)
+    vl = 0.5 + rng.rand(dof) if rng.rand() < 0.3 else 10 + 20 * rng.rand(dof)
+    al = 10 + 2 * rng.rand(dof)
+    vlim, alim = np.stack((-vl, vl), axis=1), np.stack((-al, al), axis=1)
+    G = int(rng.randint(2, 2 * (n - 1) + 1))
+    grid = np.linspace(0, ss[-1], G)
+    if G > 3 and rng.rand() < 0.3:
+        inner = np.sort(rng.uniform(0, ss[-1], G - 2))
+        if np.all(np.diff(np.r_[0.0, inner, ss[-1]]) > 0):
+            grid = np.r_[0.0, inner, ss[-1]]
+    bc = str(rng.choice(["not-a-knot", "clamped", "natural"]))
+    interp_scheme = int(rng.rand() < 0.7)
+    sd0 = 0.0 if rng.rand() < 0.7 else 10 ** rng.uniform(-3, 0)
+    sd1 = 0.0 if rng.rand() < 0.7 else 10 ** rng.uniform(-3, 0)
+    while float(sd0) ** 2 != float(sd0) * float(sd0):      # pow(x, 2.0) rounding of the reference: DESIGN.md section 2
+        sd0 = float(np.nextafter(sd0, 1.0))
+    while float(sd1) ** 2 != float(sd1) * float(sd1):
+        sd1 = float(np.nextafter(sd1, 1.0))
+    return dict(ss=ss, way=way, vlim=vlim, alim=alim, grid=grid, bc=bc, interp=interp_scheme, sd0=sd0, sd1=sd1)
