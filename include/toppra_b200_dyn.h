@@ -59,6 +59,9 @@ extern "C" {
 #define TBD_LOCAL_WORLD_ALIGNED 2
 #define TBD_OBJECT_DOUBLES 10
 #define TBD_BASE_DOUBLES 4
+#define TBD_POINT_DOUBLES (TBD_FRAME_DOUBLES + 1)
+#define TBD_MAX_POINTS 16
+#define TBD_MAX_HUMANS 16
 
 int tbd_version(void);
 
@@ -192,6 +195,46 @@ int tbd_support_wrench(const double *model_host, int nv, const double *frame_hos
 int tbd_support_wrench_terms(const double *model_host, int nv, const double *frame_host, const double *base_host,
                              int M, const double *q, const double *qs, const double *qss, double *a, double *b,
                              double *c, void *stream);
+
+/* Speed and separation monitoring (ISO/TS 15066 5.5.4; toppra_b200.constraint.SeparationMonitoringConstraint): the
+ * surface separation and the approach speed of P robot points and H human spheres, for M points, one thread per point.
+ * points_host is a HOST array of P x TBD_POINT_DOUBLES doubles: a packed frame (TBD_FRAME_DOUBLES) followed by the
+ * point's radius r_p >= 0.  The point is the sphere about the frame's origin; the frame's reference-frame field (+13)
+ * is ignored.  humans is a DEVICE array [NH][H][4] of spheres (c_h(3), r_h) in base coordinates; point m reads set
+ * m / points_per_path, or set 0 when points_per_path is 0.  One walk of the tree gives every point's world position x_p
+ * and linear velocity v (the linear part of tbd_frame_velocity for a TBD_LOCAL_WORLD_ALIGNED frame at the point), then
+ * for each pair, p-major then h, each sum left to right:
+ *   e = c_h - x_p;  l = sqrt(e.e);  d = l - r_p - r_h;  w = (e.v) / l, or sqrt(v.v) where l == 0
+ * d is the surface separation and w the speed at which the point approaches the sphere's centre.
+ *   q, qd [M][nv]; d, w [M][P][H].  TB_ERR_UNSUPPORTED for P or H outside 1..16 (TBD_MAX_POINTS, TBD_MAX_HUMANS);
+ *   TB_ERR_ARG for a null pointer, a radius r_p that is not finite or is negative, NH < 1, points_per_path < 0 or a
+ *   points_per_path that reads past set NH - 1, and the model and frame checks of tbd_frame_velocity.  The human spheres
+ *   are device data and are not checked. */
+int tbd_separation(const double *model_host, int nv, const double *points_host, int P, int H, int NH,
+                   int points_per_path, int M, const double *q, const double *qd, const double *humans, double *d,
+                   double *w, void *stream);
+
+/* The row of SeparationMonitoringConstraint at (q, qs = q'): with the reaction time T_r >= 0, the stopping deceleration
+ * a_s > 0, the human speed v_h >= 0 and the clearance C >= 0 (all finite), the separation distance of the standard,
+ * S_p = v_h (T_r + T_s) + v_r T_r + v_r^2 / (2 a_s) + C with T_s = v_r / a_s, stays below d for robot speeds up to
+ *   vmax = 0 where D <= 0, else 2 a_s D / (sqrt(k^2 + 2 a_s D) + k),   D = d - C - v_h T_r,  k = a_s T_r + v_h
+ * and the limit w s' <= vmax binds where w > 0 as w^2 s'^2 <= vmax^2.  Per point, one row a = 0, b, c:
+ *   b = w*^2, c = 0 - vmax*^2     for the pair * among those with w > 0 that minimises vmax^2 / w^2 (the first in
+ *                                 pair order on ties);
+ *   b = 0, c = -1                 where no pair has w > 0 (an inactive row);
+ *   b = c = NaN                   where any pair's d or w is NaN.
+ * Bit-identical to tbd_separation with qd = qs followed by these float64 operations, in this order, on host scalars
+ * vhTr = v_h * T_r, twoa = 2 * a_s, k = a_s * T_r + v_h, kk = k * k:
+ *   per pair:  D = d - C;  D = D - vhTr;  num = twoa * D;  vmax = D <= 0 ? 0 : num / (sqrt(kk + num) + k);
+ *              w2 = w * w;  v2 = vmax * vmax;
+ *              the pair replaces the best (bw2, bv2) when w > 0 and (no best yet or v2 * bw2 < bv2 * w2)
+ *   per point: b = bw2, c = 0 - bv2.
+ *   q, qs [M][nv]; b, c [M].  TB_ERR_ARG for a parameter out of range (NaN included); otherwise the checks of
+ *   tbd_separation. */
+int tbd_separation_terms(const double *model_host, int nv, const double *points_host, int P, int H, int NH,
+                         int points_per_path, double reaction_time, double stopping_deceleration, double human_speed,
+                         double clearance, int M, const double *q, const double *qs, const double *humans, double *b,
+                         double *c, void *stream);
 
 #ifdef __cplusplus
 }

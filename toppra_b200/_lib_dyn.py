@@ -30,6 +30,10 @@ _PROTOS = {
     "tbd_support_wrench": ([_c_dp, _int, _c_dp, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
     "tbd_support_wrench_terms": ([_c_dp, _int, _c_dp, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream],
                                  _int),
+    "tbd_separation": ([_c_dp, _int, _c_dp, _int, _int, _int, _int, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream],
+                       _int),
+    "tbd_separation_terms": ([_c_dp, _int, _c_dp, _int, _int, _int, _int, ctypes.c_double, ctypes.c_double,
+                              ctypes.c_double, ctypes.c_double, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
 }
 
 _dlib = None

@@ -10,11 +10,12 @@ from .cartesian_acceleration import CartesianAccelerationConstraint
 from .contact_stability import ContactStabilityConstraint, contact_wrench_cone
 from .collision_energy import CollisionEnergyConstraint
 from .support_stability import SupportStabilityConstraint, support_polygon_rows
+from .separation_monitoring import SeparationMonitoringConstraint
 from .conic_constraint import ConicConstraint, RobustLinearConstraint
 
 __all__ = ["ConstraintType", "DiscretizationType", "Constraint", "LinearConstraint",
            "canlinear_colloc_to_interpolate", "JointAccelerationConstraint", "JointVelocityConstraint", "JointVelocityConstraintVarying",
            "SecondOrderConstraint", "JointTorqueConstraint", "CartesianVelocityNorm", "CartesianAccelerationConstraint",
            "ContactStabilityConstraint", "contact_wrench_cone", "CollisionEnergyConstraint",
-           "SupportStabilityConstraint", "support_polygon_rows", "RecordContext", "ConicConstraint",
-           "RobustLinearConstraint"]
+           "SupportStabilityConstraint", "support_polygon_rows", "SeparationMonitoringConstraint", "RecordContext",
+           "ConicConstraint", "RobustLinearConstraint"]

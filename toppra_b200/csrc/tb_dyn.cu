@@ -30,6 +30,12 @@
 // Both run frame_inverse_inertia: the composite-rigid-body mass matrix of the whole tree in per-thread local arrays,
 // its Cholesky factor and a forward substitution; the terms kernel adds frame_velocity.
 //
+//   separation_kernel        d, w = surface separation and approach speed of P robot points and H human spheres at
+//                            (q, qd), one thread per point;
+//   separation_terms_kernel  the row b, c of SeparationMonitoringConstraint at (q, q') from the same pairs.
+// Both run point_states, one walk of the tree's bodies with their world placements and velocities in per-thread local
+// arrays, then separation_pair for every pair.
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -753,6 +759,140 @@ support_wrench_terms_kernel(const __grid_constant__ DynModel m, const __grid_con
   for (int j = 0; j < 6; ++j) b[r + j] = y[j] - y0[j];
 }
 
+// The robot points of speed and separation monitoring (include/toppra_b200_dyn.h), passed by value: each point's body
+// (-1 = the base), the origin p of its frame in body coordinates and its radius.  Bodies [0, top) cover every point's
+// chain (parents come first), so the walk stops there.
+struct DynPoints {
+  double p[TBD_MAX_POINTS][3], r[TBD_MAX_POINTS];
+  int body[TBD_MAX_POINTS];
+  int n, top;
+};
+
+// World position x and linear velocity v of every point at (q, qd): one walk of the tree's bodies [0, top) with each
+// body's world placement (Rw, pw), angular velocity w and origin velocity vo in per-thread local arrays.  The per-body
+// operations are those of frame_velocity on a chain, so v is bit-identical to the linear part of tbd_frame_velocity
+// for a TBD_LOCAL_WORLD_ALIGNED frame at the point.
+__device__ __forceinline__ void point_states(const DynModel &m, const DynPoints &pts, const double *__restrict__ q,
+                                             const double *__restrict__ qd, double (*x)[3], double (*v)[3]) {
+  double Rw[NB][9], pw[NB][3], w[NB][3], vo[NB][3];
+  for (int k = 0; k < pts.top; ++k) {
+    const double *bd = m.body[k];
+    const int par = (int)bd[0];
+    double Rp[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0}, pp[3] = {0.0, 0.0, 0.0};
+    double wp[3] = {0.0, 0.0, 0.0}, vp[3] = {0.0, 0.0, 0.0};
+    if (par >= 0) {
+      for (int j = 0; j < 9; ++j) Rp[j] = Rw[par][j];
+      for (int j = 0; j < 3; ++j) { pp[j] = pw[par][j]; wp[j] = w[par][j]; vp[j] = vo[par][j]; }
+    }
+    double R[9], p[3], d[3], t[3];
+    const double qk = q[k];
+    TB_BODY_TRANSFORM(bd, qk, R, p);
+    mul3(Rp, p, d);                     // origin of body k relative to its parent's, world coordinates
+    cross3(wp, d, t);
+    for (int j = 0; j < 3; ++j) { pw[k][j] = pp[j] + d[j]; vo[k][j] = vp[j] + t[j]; }
+    for (int r = 0; r < 3; ++r)
+      for (int c = 0; c < 3; ++c) Rw[k][3 * r + c] = Rp[3 * r] * R[c] + Rp[3 * r + 1] * R[3 + c] + Rp[3 * r + 2] * R[6 + c];
+    double s[3];
+    mul3(Rw[k], bd + 2, s);             // joint axis, world coordinates
+    const double qdk = qd[k];
+    if (bd[1] == TBD_REVOLUTE) {
+      for (int j = 0; j < 3; ++j) { w[k][j] = wp[j] + s[j] * qdk; }
+    } else {
+      for (int j = 0; j < 3; ++j) { w[k][j] = wp[j]; vo[k][j] = vo[k][j] + s[j] * qdk; }
+    }
+  }
+  for (int i = 0; i < pts.n; ++i) {
+    const int k = pts.body[i];
+    if (k < 0) {
+      for (int j = 0; j < 3; ++j) { x[i][j] = pts.p[i][j]; v[i][j] = 0.0; }
+      continue;
+    }
+    double d[3], t[3];
+    mul3(Rw[k], pts.p[i], d);           // point relative to the body origin, world coordinates
+    cross3(w[k], d, t);
+    for (int j = 0; j < 3; ++j) { x[i][j] = pw[k][j] + d[j]; v[i][j] = vo[k][j] + t[j]; }
+  }
+}
+
+// Surface separation dd and approach speed ww of the point (x, v, radius rp) and the human sphere hs = (c, r):
+//   e = c - x;  l = sqrt(e.e);  dd = l - rp - r;  ww = (e.v) / l, or |v| where l == 0
+// each sum left to right.
+__device__ __forceinline__ void separation_pair(const double *x, const double *v, const double rp, const double *hs,
+                                                double &dd, double &ww) {
+  const double e[3] = {hs[0] - x[0], hs[1] - x[1], hs[2] - x[2]};
+  const double l = sqrt(e[0] * e[0] + e[1] * e[1] + e[2] * e[2]);
+  dd = l - rp - hs[3];
+  ww = l == 0.0 ? sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]) : (e[0] * v[0] + e[1] * v[1] + e[2] * v[2]) / l;
+}
+
+// The human-sphere set of point pt: [H][4] doubles of set pt / points_per_path (set 0 when points_per_path is 0).
+__device__ __forceinline__ const double *human_set(const double *humans, const int H, const int points_per_path,
+                                                   const long pt) {
+  const long set = points_per_path > 0 ? pt / points_per_path : 0;
+  return humans + (size_t)set * H * 4;
+}
+
+__global__ void __launch_bounds__(THREADS)
+separation_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynPoints pts, const int nv, const int H,
+                  const int points_per_path, const int M, const double *__restrict__ q, const double *__restrict__ qd,
+                  const double *__restrict__ humans, double *__restrict__ dist, double *__restrict__ speed) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double x[TBD_MAX_POINTS][3], v[TBD_MAX_POINTS][3];
+  point_states(m, pts, q + o, qd + o, x, v);
+  const double *hs = human_set(humans, H, points_per_path, pt);
+  for (int i = 0; i < pts.n; ++i)
+    for (int h = 0; h < H; ++h) {
+      double dd, ww;
+      separation_pair(x[i], v[i], pts.r[i], hs + 4 * h, dd, ww);
+      const size_t r = ((size_t)pt * pts.n + i) * H + h;
+      dist[r] = dd;
+      speed[r] = ww;
+    }
+}
+
+// The row of SeparationMonitoringConstraint at (q, qs = q'), from the pairs of separation_kernel at qd = qs: per pair
+//   D = dd - C - vhTr;  num = twoa * D;  vmax = D <= 0 ? 0 : num / (sqrt(kk + num) + k)
+// with twoa = 2 a_s, vhTr = v_h T_r, k = a_s T_r + v_h, kk = k k; among the pairs with ww > 0 (p-major, then h) the
+// first one minimising vmax^2 / ww^2 by cross-multiplication (v2 * bw2 < bv2 * w2, v2 = vmax vmax, w2 = ww ww) gives
+// b = bw2, c = 0 - bv2; no such pair gives b = 0, c = -1; a NaN dd or ww of any pair gives b = c = NaN.
+__global__ void __launch_bounds__(THREADS)
+separation_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynPoints pts, const int nv,
+                        const int H, const int points_per_path, const double clearance, const double vhTr,
+                        const double twoa, const double k, const double kk, const int M, const double *__restrict__ q,
+                        const double *__restrict__ qs, const double *__restrict__ humans, double *__restrict__ b,
+                        double *__restrict__ c) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double x[TBD_MAX_POINTS][3], v[TBD_MAX_POINTS][3];
+  point_states(m, pts, q + o, qs + o, x, v);
+  const double *hs = human_set(humans, H, points_per_path, pt);
+  double bw2 = 0.0, bv2 = 0.0;
+  bool found = false, bad = false;
+  for (int i = 0; i < pts.n; ++i)
+    for (int h = 0; h < H; ++h) {
+      double dd, ww;
+      separation_pair(x[i], v[i], pts.r[i], hs + 4 * h, dd, ww);
+      const double D = dd - clearance - vhTr;
+      const double num = twoa * D;
+      const double vmax = D <= 0.0 ? 0.0 : num / (sqrt(kk + num) + k);
+      bad = bad || isnan(ww) || isnan(vmax);
+      if (ww > 0.0) {
+        const double w2 = ww * ww, v2 = vmax * vmax;
+        if (!found || v2 * bw2 < bv2 * w2) { bw2 = w2; bv2 = v2; found = true; }
+      }
+    }
+  if (bad) {
+    b[pt] = nan("");
+    c[pt] = nan("");
+  } else {
+    b[pt] = found ? bw2 : 0.0;
+    c[pt] = found ? 0.0 - bv2 : -1.0;
+  }
+}
+
 int launch_status(const char *what) {
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -858,6 +998,39 @@ int load_support(const double *host, const DynModel &m, const int nv, DynFrame *
   if (host[0] != -1.0) {
     set_error("%s: the support must be on the base (frame body %g, expected -1)", what, host[0]);
     return TB_ERR_ARG;
+  }
+  return 0;
+}
+
+// The packed points (P x TBD_POINT_DOUBLES: a packed frame and a radius), the human-sphere sets and their assignment to
+// points, for a model already loaded by load_model: 0, or the TB_ERR_* code (message set).  The frames' reference-frame
+// field is ignored.
+int load_points(const double *host, const int P, const int H, const int NH, const int points_per_path, const int M,
+                const DynModel &m, const int nv, DynPoints *pts, const char *what) {
+  if (P < 1 || P > TBD_MAX_POINTS) { set_error("%s: P=%d points outside 1..%d", what, P, TBD_MAX_POINTS); return TB_ERR_UNSUPPORTED; }
+  if (H < 1 || H > TBD_MAX_HUMANS) { set_error("%s: H=%d human spheres outside 1..%d", what, H, TBD_MAX_HUMANS); return TB_ERR_UNSUPPORTED; }
+  if (NH < 1) { set_error("%s: NH=%d human-sphere sets must be positive", what, NH); return TB_ERR_ARG; }
+  if (points_per_path < 0 || (points_per_path > 0 && (M - 1) / points_per_path >= NH)) {
+    set_error("%s: points_per_path=%d with M=%d reads past the NH=%d human-sphere sets", what, points_per_path, M, NH);
+    return TB_ERR_ARG;
+  }
+  pts->n = P;
+  pts->top = 0;
+  for (int i = 0; i < TBD_MAX_POINTS; ++i) {
+    pts->body[i] = -1;
+    pts->r[i] = 0.0;
+    for (int j = 0; j < 3; ++j) pts->p[i][j] = 0.0;
+  }
+  for (int i = 0; i < P; ++i) {
+    const double *ph = host + (size_t)TBD_POINT_DOUBLES * i;
+    DynFrame f;
+    if (const int rc = load_frame(ph, m, nv, nullptr, TBD_LOCAL_WORLD_ALIGNED, &f, what)) return rc;
+    const double r = ph[TBD_FRAME_DOUBLES];
+    if (!std::isfinite(r) || r < 0.0) { set_error("%s: point %d: radius %g must be finite and >= 0", what, i, r); return TB_ERR_ARG; }
+    pts->body[i] = (int)ph[0];
+    pts->r[i] = r;
+    for (int j = 0; j < 3; ++j) pts->p[i][j] = f.p[j];
+    if (pts->body[i] + 1 > pts->top) pts->top = pts->body[i] + 1;
   }
   return 0;
 }
@@ -1061,4 +1234,49 @@ extern "C" int tbd_support_wrench_terms(const double *model_host, int nv, const 
   if (const int rc = load_base(base_host, &base, "tbd_support_wrench_terms")) return rc;
   support_wrench_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, s, base, nv, M, q, qs, qss, a, b, c);
   return launch_status("tbd_support_wrench_terms");
+}
+
+extern "C" int tbd_separation(const double *model_host, int nv, const double *points_host, int P, int H, int NH,
+                              int points_per_path, int M, const double *q, const double *qd, const double *humans,
+                              double *d, double *w, void *stream) {
+  using namespace tb;
+  if (!model_host || !points_host || !q || !qd || !humans || !d || !w) {
+    set_error("tbd_separation: null pointer");
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynPoints pts;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_separation")) return rc;
+  if (const int rc = load_points(points_host, P, H, NH, points_per_path, M, m, nv, &pts, "tbd_separation")) return rc;
+  separation_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, pts, nv, H, points_per_path, M, q, qd, humans,
+                                                                     d, w);
+  return launch_status("tbd_separation");
+}
+
+extern "C" int tbd_separation_terms(const double *model_host, int nv, const double *points_host, int P, int H, int NH,
+                                    int points_per_path, double reaction_time, double stopping_deceleration,
+                                    double human_speed, double clearance, int M, const double *q, const double *qs,
+                                    const double *humans, double *b, double *c, void *stream) {
+  using namespace tb;
+  if (!model_host || !points_host || !q || !qs || !humans || !b || !c) {
+    set_error("tbd_separation_terms: null pointer");
+    return TB_ERR_ARG;
+  }
+  if (!(std::isfinite(reaction_time) && reaction_time >= 0.0 && std::isfinite(stopping_deceleration) &&
+        stopping_deceleration > 0.0 && std::isfinite(human_speed) && human_speed >= 0.0 && std::isfinite(clearance) &&
+        clearance >= 0.0)) {
+    set_error("tbd_separation_terms: reaction_time %g, human_speed %g and clearance %g must be finite and >= 0, "
+              "stopping_deceleration %g finite and > 0", reaction_time, human_speed, clearance, stopping_deceleration);
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  DynPoints pts;
+  if (const int rc = load_model(model_host, nv, M, &m, "tbd_separation_terms")) return rc;
+  if (const int rc = load_points(points_host, P, H, NH, points_per_path, M, m, nv, &pts, "tbd_separation_terms"))
+    return rc;
+  const double vhTr = human_speed * reaction_time, twoa = 2.0 * stopping_deceleration;
+  const double k = stopping_deceleration * reaction_time + human_speed, kk = k * k;
+  separation_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, pts, nv, H, points_per_path, clearance,
+                                                                           vhTr, twoa, k, kk, M, q, qs, humans, b, c);
+  return launch_status("tbd_separation_terms");
 }

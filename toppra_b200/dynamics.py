@@ -20,7 +20,9 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     loaded = model.with_payload("flange", m, com, I)          # a rigidly held payload folded into the flange's body
     floor = model.frame("base_footprint")                     # a support frame on the base (z: the support normal)
     w = floor.support_wrench(None, q, qd, qdd)                # (M, 6) the support's wrench on the whole robot, one launch
-    pc = SupportStabilityConstraint(floor, half_lengths=(X, Y), friction=mu)  # the robot must not tip over or slide"""
+    pc = SupportStabilityConstraint(floor, half_lengths=(X, Y), friction=mu)  # the robot must not tip over or slide
+    pc = SeparationMonitoringConstraint([(tcp, 0.05)], humans, T_r, a_s)  # speed and separation monitoring
+    d, w = model.separation(pack_points([(tcp, 0.05)])[1], humans, q, qd)  # (M, P, H) separations, approach speeds"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -202,6 +204,29 @@ class RigidBodyModel(object):
         if friction is not None and np.any(np.asarray(friction) != 0):
             fric = np.broadcast_to(np.asarray(friction, dtype=np.float64), (self.nv,)).copy()
         return _launch(self, "tbd_torque_terms", (), (q, qs, qss), [(self.nv,)] * 3, extra=(fric,))
+
+    def separation(self, points, humans, q, qd, points_per_path=0):
+        """Surface separation d and approach speed w of robot points and human spheres at the state (q, qd), for CUDA
+        tensors (M, nv): one tbd_separation launch.  points: packed (P, TBD_POINT_DOUBLES) (pack_points); humans:
+        (H, 4) or (NH, H, 4) spheres (centre, radius) in base coordinates, point m reading set m // points_per_path
+        (set 0 when points_per_path is 0).  With e = c_h - x_p, l = |e|: d = l - r_p - r_h, w = e.v / l (|v| where
+        l == 0), v the point's linear velocity.  Returns (d, w), each (M, P, H)."""
+        P, hum = _check_packed_points(points), _human_sets(humans, q)
+        NH, H = hum.shape[:2]
+        return _launch(self, "tbd_separation", (points, P, H, NH, int(points_per_path)), (q, qd), [(P, H)] * 2,
+                       extra=(hum,))
+
+    def separation_terms(self, points, humans, reaction_time, stopping_deceleration, human_speed, clearance, q, qs,
+                         points_per_path=0):
+        """The row (b, c) of SeparationMonitoringConstraint at (q, qs = q') for CUDA tensors (M, nv): one
+        tbd_separation_terms launch; the arguments are those of `separation` and the four scalars of the limit
+        (include/toppra_b200_dyn.h).  b = w*^2, c = 0 - vmax*^2 of the binding pair, or b = 0, c = -1 where no pair
+        approaches.  Returns (b, c), each (M,)."""
+        P, hum = _check_packed_points(points), _human_sets(humans, q)
+        NH, H = hum.shape[:2]
+        return _launch(self, "tbd_separation_terms",
+                       (points, P, H, NH, int(points_per_path), float(reaction_time), float(stopping_deceleration),
+                        float(human_speed), float(clearance)), (q, qs), [(), ()], extra=(hum,))
 
     # ---- URDF ---------------------------------------------------------------------------------------------------
     @classmethod
@@ -541,6 +566,53 @@ def _packed_base(base):
     if base.shape != (BASE_DOUBLES,):
         raise ValueError("packed base: expected %d doubles (m_b, c_b), got shape %s" % (BASE_DOUBLES, base.shape))
     return base
+
+
+FRAME_DOUBLES = 14
+POINT_DOUBLES = FRAME_DOUBLES + 1
+MAX_POINTS = MAX_HUMANS = 16
+
+
+def pack_points(points):
+    """The robot points of speed and separation monitoring: a sequence of (RigidBodyFrame, radius) of one model, the
+    sphere of that radius about the frame's origin.  Returns (model, packed (P, TBD_POINT_DOUBLES)): each row the
+    frame's packed doubles and the radius.  ValueError for anything else, frames of different models, a radius that is
+    not finite or is negative, or P outside 1..16."""
+    try:
+        items = [(f, r) for f, r in points]
+    except (TypeError, ValueError):
+        raise ValueError("points: expected a sequence of (RigidBodyFrame, radius)")
+    if not 1 <= len(items) <= MAX_POINTS:
+        raise ValueError("points: %d points, supported 1..%d" % (len(items), MAX_POINTS))
+    if not all(isinstance(f, RigidBodyFrame) and np.ndim(r) == 0 for f, r in items):
+        raise ValueError("points: expected a sequence of (RigidBodyFrame, radius)")
+    model = items[0][0].model
+    if any(f.model is not model for f, _ in items):
+        raise ValueError("points: every frame must belong to the same RigidBodyModel")
+    radii = np.array([float(r) for _, r in items])
+    if not (np.isfinite(radii).all() and (radii >= 0).all()):
+        raise ValueError("points: radii must be finite and >= 0; got %s" % radii.tolist())
+    packed = np.concatenate([np.stack([f.packed for f, _ in items]), radii[:, None]], axis=1)
+    return model, np.ascontiguousarray(packed)
+
+
+def _check_packed_points(points):
+    """P of packed points (P, TBD_POINT_DOUBLES), a contiguous float64 array: the library reads exactly that."""
+    if not (isinstance(points, np.ndarray) and points.dtype == np.float64 and points.flags.c_contiguous
+            and points.ndim == 2 and points.shape[1] == POINT_DOUBLES):
+        raise ValueError("packed points: expected a contiguous float64 (P, %d) array (pack_points)" % POINT_DOUBLES)
+    return points.shape[0]
+
+
+def _human_sets(humans, q):
+    """Human spheres (H, 4) or (NH, H, 4) as a contiguous float64 CUDA tensor (NH, H, 4) on q's device."""
+    torch = _lib.require_cuda()
+    h = torch.as_tensor(humans, dtype=torch.float64, device=q.device if _is_cuda(q) else "cuda")
+    if h.dim() == 2:
+        h = h.unsqueeze(0)
+    if h.dim() != 3 or h.shape[2] != 4 or h.shape[0] < 1:
+        raise ValueError("humans: expected (H, 4) or (NH, H, 4) spheres (centre, radius); got %s" % (tuple(h.shape),))
+    return h.contiguous()
 
 
 def component_indices(components):
