@@ -86,6 +86,12 @@ __device__ __forceinline__ void mul3t(const double *R, const double *x, double *
   o[2] = R[2] * x[0] + R[5] * x[1] + R[8] * x[2];
 }
 
+// O = A B (row-major 3x3), each entry summed left to right
+__device__ __forceinline__ void mul33(const double *A, const double *B, double *O) {
+  for (int r = 0; r < 3; ++r)
+    for (int c = 0; c < 3; ++c) O[3 * r + c] = A[3 * r] * B[c] + A[3 * r + 1] * B[3 + c] + A[3 * r + 2] * B[6 + c];
+}
+
 // o = I x with I = (Ixx, Ixy, Ixz, Iyy, Iyz, Izz)
 __device__ __forceinline__ void mul_inertia(const double *I, const double *x, double *o) {
   o[0] = I[0] * x[0] + I[1] * x[1] + I[2] * x[2];
@@ -267,8 +273,7 @@ __device__ __forceinline__ void frame_velocity(const DynModel &m, const DynFrame
     mul3(Rw, p, d);                     // origin of body k relative to its parent's, world coordinates
     cross3(w, d, t);
     for (int j = 0; j < 3; ++j) { pw[j] = pw[j] + d[j]; vo[j] = vo[j] + t[j]; }
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) Rn[3 * r + c] = Rw[3 * r] * R[c] + Rw[3 * r + 1] * R[3 + c] + Rw[3 * r + 2] * R[6 + c];
+    mul33(Rw, R, Rn);
     for (int j = 0; j < 9; ++j) Rw[j] = Rn[j];
     double s[3];
     mul3(Rw, bd + 2, s);                // joint axis, world coordinates
@@ -285,8 +290,7 @@ __device__ __forceinline__ void frame_velocity(const DynModel &m, const DynFrame
   for (int j = 0; j < 3; ++j) pd[j] = vo[j] + t[j];
   if (f.ref == TBD_LOCAL) {
     double Rf[9];
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) Rf[3 * r + c] = Rw[3 * r] * f.R[c] + Rw[3 * r + 1] * f.R[3 + c] + Rw[3 * r + 2] * f.R[6 + c];
+    mul33(Rw, f.R, Rf);
     mul3t(Rf, pd, v);
     mul3t(Rf, w, v + 3);
   } else if (f.ref == TBD_WORLD) {
@@ -364,8 +368,7 @@ __device__ __forceinline__ void frame_acceleration(const DynModel &m, const DynF
       cross3(w[s], t2, t3);
       for (int j = 0; j < 3; ++j) ao[s][j] = ao[s][j] + t1[j] + t3[j];
     }
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) Rn[3 * r + c] = Rw[3 * r] * R[c] + Rw[3 * r + 1] * R[3 + c] + Rw[3 * r + 2] * R[6 + c];
+    mul33(Rw, R, Rn);
     for (int j = 0; j < 9; ++j) Rw[j] = Rn[j];
     double sx[3];
     mul3(Rw, bd + 2, sx);               // joint axis, world coordinates
@@ -384,9 +387,7 @@ __device__ __forceinline__ void frame_acceleration(const DynModel &m, const DynF
   }
   double d[3], Rf[9];
   mul3(Rw, f.p, d);                     // frame origin relative to the body origin, world coordinates
-  if (ROT || f.ref == TBD_LOCAL)
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) Rf[3 * r + c] = Rw[3 * r] * f.R[c] + Rw[3 * r + 1] * f.R[3 + c] + Rw[3 * r + 2] * f.R[6 + c];
+  if (ROT || f.ref == TBD_LOCAL) mul33(Rw, f.R, Rf);
   for (int s = 0; s < NS; ++s) {
     double t1[3], t2[3], t3[3], af[3];
     cross3(dw[s], d, t1);
@@ -518,8 +519,7 @@ __device__ bool frame_inverse_inertia(const DynModel &m, const DynFrame &f, cons
     double d[3], Rn[9];
     mul3(Rw, p, d);
     for (int j = 0; j < 3; ++j) pw[j] = pw[j] + d[j];
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) Rn[3 * r + c] = Rw[3 * r] * R[c] + Rw[3 * r + 1] * R[3 + c] + Rw[3 * r + 2] * R[6 + c];
+    mul33(Rw, R, Rn);
     for (int j = 0; j < 9; ++j) Rw[j] = Rn[j];
     mul3(Rw, m.body[k] + 2, s[i]);
     for (int j = 0; j < 3; ++j) o[i][j] = pw[j];
@@ -560,10 +560,9 @@ __device__ bool frame_inverse_inertia(const DynModel &m, const DynFrame &f, cons
     double hr[3], A[9], B[9];
     mul3(R, e + 1, hr);
     const double I3[9] = {e[4], e[5], e[6], e[5], e[7], e[8], e[6], e[8], e[9]};
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) A[3 * r + c] = R[3 * r] * I3[c] + R[3 * r + 1] * I3[3 + c] + R[3 * r + 2] * I3[6 + c];
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) B[3 * r + c] = A[3 * r] * R[3 * c] + A[3 * r + 1] * R[3 * c + 1] + A[3 * r + 2] * R[3 * c + 2];
+    const double Rt[9] = {R[0], R[3], R[6], R[1], R[4], R[7], R[2], R[5], R[8]};
+    mul33(R, I3, A);
+    mul33(A, Rt, B);
     const double pp = p[0] * p[0] + p[1] * p[1] + p[2] * p[2];
     const double ph = p[0] * hr[0] + p[1] * hr[1] + p[2] * hr[2];
     const double diag = e[0] * pp + 2.0 * ph;
@@ -643,12 +642,10 @@ __device__ bool frame_inverse_inertia(const DynModel &m, const DynFrame &f, cons
     }
   if (f.ref == TBD_LOCAL) {
     double Rf[9], T[9];
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) Rf[3 * r + c] = Rw[3 * r] * f.R[c] + Rw[3 * r + 1] * f.R[3 + c] + Rw[3 * r + 2] * f.R[6 + c];
-    for (int r = 0; r < 3; ++r)                                        // T = W R_f
-      for (int c = 0; c < 3; ++c) T[3 * r + c] = W[3 * r] * Rf[c] + W[3 * r + 1] * Rf[3 + c] + W[3 * r + 2] * Rf[6 + c];
-    for (int r = 0; r < 3; ++r)                                        // R_f^T T
-      for (int c = 0; c < 3; ++c) Linv[3 * r + c] = Rf[r] * T[c] + Rf[3 + r] * T[3 + c] + Rf[6 + r] * T[6 + c];
+    mul33(Rw, f.R, Rf);
+    mul33(W, Rf, T);
+    const double Rft[9] = {Rf[0], Rf[3], Rf[6], Rf[1], Rf[4], Rf[7], Rf[2], Rf[5], Rf[8]};
+    mul33(Rft, T, Linv);                                               // R_f^T W R_f
   } else {
     for (int j = 0; j < 9; ++j) Linv[j] = W[j];
   }
@@ -790,8 +787,7 @@ __device__ __forceinline__ void point_states(const DynModel &m, const DynPoints 
     mul3(Rp, p, d);                     // origin of body k relative to its parent's, world coordinates
     cross3(wp, d, t);
     for (int j = 0; j < 3; ++j) { pw[k][j] = pp[j] + d[j]; vo[k][j] = vp[j] + t[j]; }
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) Rw[k][3 * r + c] = Rp[3 * r] * R[c] + Rp[3 * r + 1] * R[3 + c] + Rp[3 * r + 2] * R[6 + c];
+    mul33(Rp, R, Rw[k]);
     double s[3];
     mul3(Rw[k], bd + 2, s);             // joint axis, world coordinates
     const double qdk = qd[k];
@@ -1037,96 +1033,99 @@ int load_points(const double *host, const int P, const int H, const int NH, cons
 
 unsigned blocks(const int M) { return (unsigned)((M + THREADS - 1) / THREADS); }
 
+// 0 if no pointer is null, else "<what>: null pointer" and TB_ERR_ARG.
+template <class... P>
+int nonnull(const char *what, const P *...ptrs) {
+  if ((... && ptrs)) return 0;
+  set_error("%s: null pointer", what);
+  return TB_ERR_ARG;
+}
+
+// One thread per point on `stream`, then the launch status of entry `what`.
+template <class... K, class... A>
+int launch(const char *what, void (*kernel)(K...), const int M, void *stream, const A &...args) {
+  kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(args...);
+  return launch_status(what);
+}
+
 }  // namespace
 }  // namespace tb
+
+// Each entry checks its pointers, its scalars and the packed model and parameters (loaders), in that order, and
+// launches; __func__ names the entry in every error message.
 
 extern "C" int tbd_version(void) { return TBD_VERSION; }
 
 extern "C" int tbd_rnea(const double *model_host, int nv, int M, const double *q, const double *qd, const double *qdd,
                         double *tau, void *stream) {
   using namespace tb;
-  if (!model_host || !q || !qd || !qdd || !tau) { set_error("tbd_rnea: null pointer"); return TB_ERR_ARG; }
+  if (const int rc = nonnull(__func__, model_host, q, qd, qdd, tau)) return rc;
   DynModel m;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_rnea")) return rc;
-  rnea_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, nv, M, q, qd, qdd, tau);
-  return launch_status("tbd_rnea");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  return launch(__func__, rnea_kernel, M, stream, m, nv, M, q, qd, qdd, tau);
 }
 
+// friction may be null (no friction).
 extern "C" int tbd_torque_terms(const double *model_host, int nv, int M, const double *q, const double *qs,
                                 const double *qss, const double *friction, double *a, double *b, double *c,
                                 void *stream) {
   using namespace tb;
-  if (!model_host || !q || !qs || !qss || !a || !b || !c) { set_error("tbd_torque_terms: null pointer"); return TB_ERR_ARG; }
+  if (const int rc = nonnull(__func__, model_host, q, qs, qss, a, b, c)) return rc;
   DynModel m;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_torque_terms")) return rc;
-  torque_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, nv, M, q, qs, qss, friction, a, b, c);
-  return launch_status("tbd_torque_terms");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  return launch(__func__, torque_terms_kernel, M, stream, m, nv, M, q, qs, qss, friction, a, b, c);
 }
 
 extern "C" int tbd_frame_velocity(const double *model_host, int nv, const double *frame_host, int M, const double *q,
                                   const double *qd, double *v, void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !q || !qd || !v) { set_error("tbd_frame_velocity: null pointer"); return TB_ERR_ARG; }
+  if (const int rc = nonnull(__func__, model_host, frame_host, q, qd, v)) return rc;
   DynModel m;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_frame_velocity")) return rc;
   DynFrame f;
-  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, "tbd_frame_velocity")) return rc;
-  frame_velocity_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qd, v);
-  return launch_status("tbd_frame_velocity");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, __func__)) return rc;
+  return launch(__func__, frame_velocity_kernel, M, stream, m, f, nv, M, q, qd, v);
 }
 
 extern "C" int tbd_velocity_norm_terms(const double *model_host, int nv, const double *frame_host, const double *S_host,
                                        int M, const double *q, const double *qs, double *b, void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !S_host || !q || !qs || !b) {
-    set_error("tbd_velocity_norm_terms: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, frame_host, S_host, q, qs, b)) return rc;
   DynModel m;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_velocity_norm_terms")) return rc;
   DynFrame f;
-  if (const int rc = load_frame(frame_host, m, nv, S_host, -1, &f, "tbd_velocity_norm_terms")) return rc;
-  velocity_norm_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qs, b);
-  return launch_status("tbd_velocity_norm_terms");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, S_host, -1, &f, __func__)) return rc;
+  return launch(__func__, velocity_norm_terms_kernel, M, stream, m, f, nv, M, q, qs, b);
 }
 
 extern "C" int tbd_frame_acceleration(const double *model_host, int nv, const double *frame_host, int M,
                                       const double *q, const double *qd, const double *qdd, double *acc, void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !q || !qd || !qdd || !acc) {
-    set_error("tbd_frame_acceleration: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, frame_host, q, qd, qdd, acc)) return rc;
   DynModel m;
   DynFrame f;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_frame_acceleration")) return rc;
-  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, "tbd_frame_acceleration")) return rc;
-  if (const int rc = refuse_world(f, "tbd_frame_acceleration", " for accelerations")) return rc;
-  frame_acceleration_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, qd, qdd, acc);
-  return launch_status("tbd_frame_acceleration");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, __func__)) return rc;
+  if (const int rc = refuse_world(f, __func__, " for accelerations")) return rc;
+  return launch(__func__, frame_acceleration_kernel, M, stream, m, f, nv, M, q, qd, qdd, acc);
 }
 
 extern "C" int tbd_acceleration_terms(const double *model_host, int nv, const double *frame_host, int components, int M,
                                       const double *q, const double *qs, const double *qss, double *a, double *b,
                                       void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !q || !qs || !qss || !a || !b) {
-    set_error("tbd_acceleration_terms: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, frame_host, q, qs, qss, a, b)) return rc;
   if (components < 1 || components > 63) {
-    set_error("tbd_acceleration_terms: components=%d must be a bit mask in 1..63", components);
+    set_error("%s: components=%d must be a bit mask in 1..63", __func__, components);
     return TB_ERR_ARG;
   }
   DynModel m;
   DynFrame f;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_acceleration_terms")) return rc;
-  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, "tbd_acceleration_terms")) return rc;
-  if (const int rc = refuse_world(f, "tbd_acceleration_terms", " for accelerations")) return rc;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, __func__)) return rc;
+  if (const int rc = refuse_world(f, __func__, " for accelerations")) return rc;
   const int k = __builtin_popcount((unsigned)components);
-  acceleration_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, components, k, M, q, qs, qss,
-                                                                              a, b);
-  return launch_status("tbd_acceleration_terms");
+  return launch(__func__, acceleration_terms_kernel, M, stream, m, f, nv, components, k, M, q, qs, qss, a, b);
 }
 
 // The contact wrench is always in the contact frame's own axes: its reference-frame field is ignored.
@@ -1134,123 +1133,96 @@ extern "C" int tbd_contact_wrench(const double *model_host, int nv, const double
                                   int M, const double *q, const double *qd, const double *qdd, double *w,
                                   void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !object_host || !q || !qd || !qdd || !w) {
-    set_error("tbd_contact_wrench: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, frame_host, object_host, q, qd, qdd, w)) return rc;
   DynModel m;
   DynFrame f;
   DynObject o;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_contact_wrench")) return rc;
-  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL, &f, "tbd_contact_wrench")) return rc;
-  if (const int rc = load_object(object_host, &o, "tbd_contact_wrench")) return rc;
-  contact_wrench_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, o, nv, M, q, qd, qdd, w);
-  return launch_status("tbd_contact_wrench");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL, &f, __func__)) return rc;
+  if (const int rc = load_object(object_host, &o, __func__)) return rc;
+  return launch(__func__, contact_wrench_kernel, M, stream, m, f, o, nv, M, q, qd, qdd, w);
 }
 
 extern "C" int tbd_contact_wrench_terms(const double *model_host, int nv, const double *frame_host,
                                         const double *object_host, int M, const double *q, const double *qs,
                                         const double *qss, double *a, double *b, double *c, void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !object_host || !q || !qs || !qss || !a || !b || !c) {
-    set_error("tbd_contact_wrench_terms: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, frame_host, object_host, q, qs, qss, a, b, c)) return rc;
   DynModel m;
   DynFrame f;
   DynObject o;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_contact_wrench_terms")) return rc;
-  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL, &f, "tbd_contact_wrench_terms")) return rc;
-  if (const int rc = load_object(object_host, &o, "tbd_contact_wrench_terms")) return rc;
-  contact_wrench_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, o, nv, M, q, qs, qss, a, b, c);
-  return launch_status("tbd_contact_wrench_terms");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL, &f, __func__)) return rc;
+  if (const int rc = load_object(object_host, &o, __func__)) return rc;
+  return launch(__func__, contact_wrench_terms_kernel, M, stream, m, f, o, nv, M, q, qs, qss, a, b, c);
 }
 
 extern "C" int tbd_frame_inverse_inertia(const double *model_host, int nv, const double *frame_host, int M,
                                          const double *q, double *Linv, void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !q || !Linv) { set_error("tbd_frame_inverse_inertia: null pointer"); return TB_ERR_ARG; }
+  if (const int rc = nonnull(__func__, model_host, frame_host, q, Linv)) return rc;
   DynModel m;
   DynFrame f;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_frame_inverse_inertia")) return rc;
-  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, "tbd_frame_inverse_inertia")) return rc;
-  if (const int rc = refuse_world(f, "tbd_frame_inverse_inertia", "")) return rc;
-  frame_inverse_inertia_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, M, q, Linv);
-  return launch_status("tbd_frame_inverse_inertia");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, -1, &f, __func__)) return rc;
+  if (const int rc = refuse_world(f, __func__, "")) return rc;
+  return launch(__func__, frame_inverse_inertia_kernel, M, stream, m, f, nv, M, q, Linv);
 }
 
 // The collision energy needs the world linear velocity: the frame is read as TBD_LOCAL_WORLD_ALIGNED.
 extern "C" int tbd_collision_energy_terms(const double *model_host, int nv, const double *frame_host, double human_mass,
                                           int M, const double *q, const double *qs, double *b, void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !q || !qs || !b) {
-    set_error("tbd_collision_energy_terms: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, frame_host, q, qs, b)) return rc;
   if (!(human_mass > 0.0)) {
-    set_error("tbd_collision_energy_terms: human_mass %g must be positive (inf allowed)", human_mass);
+    set_error("%s: human_mass %g must be positive (inf allowed)", __func__, human_mass);
     return TB_ERR_ARG;
   }
   DynModel m;
   DynFrame f;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_collision_energy_terms")) return rc;
-  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL_WORLD_ALIGNED, &f, "tbd_collision_energy_terms"))
-    return rc;
-  collision_energy_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, f, nv, human_mass, M, q, qs, b);
-  return launch_status("tbd_collision_energy_terms");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_frame(frame_host, m, nv, nullptr, TBD_LOCAL_WORLD_ALIGNED, &f, __func__)) return rc;
+  return launch(__func__, collision_energy_terms_kernel, M, stream, m, f, nv, human_mass, M, q, qs, b);
 }
 
 extern "C" int tbd_support_wrench(const double *model_host, int nv, const double *frame_host, const double *base_host,
                                   int M, const double *q, const double *qd, const double *qdd, double *w,
                                   void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !base_host || !q || !qd || !qdd || !w) {
-    set_error("tbd_support_wrench: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, frame_host, base_host, q, qd, qdd, w)) return rc;
   DynModel m;
   DynFrame s;
   DynBase base;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_support_wrench")) return rc;
-  if (const int rc = load_support(frame_host, m, nv, &s, "tbd_support_wrench")) return rc;
-  if (const int rc = load_base(base_host, &base, "tbd_support_wrench")) return rc;
-  support_wrench_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, s, base, nv, M, q, qd, qdd, w);
-  return launch_status("tbd_support_wrench");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_support(frame_host, m, nv, &s, __func__)) return rc;
+  if (const int rc = load_base(base_host, &base, __func__)) return rc;
+  return launch(__func__, support_wrench_kernel, M, stream, m, s, base, nv, M, q, qd, qdd, w);
 }
 
 extern "C" int tbd_support_wrench_terms(const double *model_host, int nv, const double *frame_host,
                                         const double *base_host, int M, const double *q, const double *qs,
                                         const double *qss, double *a, double *b, double *c, void *stream) {
   using namespace tb;
-  if (!model_host || !frame_host || !base_host || !q || !qs || !qss || !a || !b || !c) {
-    set_error("tbd_support_wrench_terms: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, frame_host, base_host, q, qs, qss, a, b, c)) return rc;
   DynModel m;
   DynFrame s;
   DynBase base;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_support_wrench_terms")) return rc;
-  if (const int rc = load_support(frame_host, m, nv, &s, "tbd_support_wrench_terms")) return rc;
-  if (const int rc = load_base(base_host, &base, "tbd_support_wrench_terms")) return rc;
-  support_wrench_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, s, base, nv, M, q, qs, qss, a, b, c);
-  return launch_status("tbd_support_wrench_terms");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_support(frame_host, m, nv, &s, __func__)) return rc;
+  if (const int rc = load_base(base_host, &base, __func__)) return rc;
+  return launch(__func__, support_wrench_terms_kernel, M, stream, m, s, base, nv, M, q, qs, qss, a, b, c);
 }
 
 extern "C" int tbd_separation(const double *model_host, int nv, const double *points_host, int P, int H, int NH,
                               int points_per_path, int M, const double *q, const double *qd, const double *humans,
                               double *d, double *w, void *stream) {
   using namespace tb;
-  if (!model_host || !points_host || !q || !qd || !humans || !d || !w) {
-    set_error("tbd_separation: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, points_host, q, qd, humans, d, w)) return rc;
   DynModel m;
   DynPoints pts;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_separation")) return rc;
-  if (const int rc = load_points(points_host, P, H, NH, points_per_path, M, m, nv, &pts, "tbd_separation")) return rc;
-  separation_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, pts, nv, H, points_per_path, M, q, qd, humans,
-                                                                     d, w);
-  return launch_status("tbd_separation");
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_points(points_host, P, H, NH, points_per_path, M, m, nv, &pts, __func__)) return rc;
+  return launch(__func__, separation_kernel, M, stream, m, pts, nv, H, points_per_path, M, q, qd, humans, d, w);
 }
 
 extern "C" int tbd_separation_terms(const double *model_host, int nv, const double *points_host, int P, int H, int NH,
@@ -1258,25 +1230,21 @@ extern "C" int tbd_separation_terms(const double *model_host, int nv, const doub
                                     double human_speed, double clearance, int M, const double *q, const double *qs,
                                     const double *humans, double *b, double *c, void *stream) {
   using namespace tb;
-  if (!model_host || !points_host || !q || !qs || !humans || !b || !c) {
-    set_error("tbd_separation_terms: null pointer");
-    return TB_ERR_ARG;
-  }
+  if (const int rc = nonnull(__func__, model_host, points_host, q, qs, humans, b, c)) return rc;
   if (!(std::isfinite(reaction_time) && reaction_time >= 0.0 && std::isfinite(stopping_deceleration) &&
         stopping_deceleration > 0.0 && std::isfinite(human_speed) && human_speed >= 0.0 && std::isfinite(clearance) &&
         clearance >= 0.0)) {
-    set_error("tbd_separation_terms: reaction_time %g, human_speed %g and clearance %g must be finite and >= 0, "
-              "stopping_deceleration %g finite and > 0", reaction_time, human_speed, clearance, stopping_deceleration);
+    set_error("%s: reaction_time %g, human_speed %g and clearance %g must be finite and >= 0, "
+              "stopping_deceleration %g finite and > 0", __func__, reaction_time, human_speed, clearance,
+              stopping_deceleration);
     return TB_ERR_ARG;
   }
   DynModel m;
   DynPoints pts;
-  if (const int rc = load_model(model_host, nv, M, &m, "tbd_separation_terms")) return rc;
-  if (const int rc = load_points(points_host, P, H, NH, points_per_path, M, m, nv, &pts, "tbd_separation_terms"))
-    return rc;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_points(points_host, P, H, NH, points_per_path, M, m, nv, &pts, __func__)) return rc;
   const double vhTr = human_speed * reaction_time, twoa = 2.0 * stopping_deceleration;
   const double k = stopping_deceleration * reaction_time + human_speed, kk = k * k;
-  separation_terms_kernel<<<blocks(M), THREADS, 0, (cudaStream_t)stream>>>(m, pts, nv, H, points_per_path, clearance,
-                                                                           vhTr, twoa, k, kk, M, q, qs, humans, b, c);
-  return launch_status("tbd_separation_terms");
+  return launch(__func__, separation_terms_kernel, M, stream, m, pts, nv, H, points_per_path, clearance, vhTr, twoa, k,
+                kk, M, q, qs, humans, b, c);
 }
