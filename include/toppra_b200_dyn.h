@@ -62,6 +62,7 @@ extern "C" {
 #define TBD_POINT_DOUBLES (TBD_FRAME_DOUBLES + 1)
 #define TBD_MAX_POINTS 16
 #define TBD_MAX_HUMANS 16
+#define TBD_DRIVE_DOUBLES(nv) ((nv) * (nv) + 2 * (nv))
 
 int tbd_version(void);
 
@@ -235,6 +236,45 @@ int tbd_separation_terms(const double *model_host, int nv, const double *points_
                          int points_per_path, double reaction_time, double stopping_deceleration, double human_speed,
                          double clearance, int M, const double *q, const double *qs, const double *humans, double *b,
                          double *c, void *stream);
+
+/* Geared drives (toppra_b200.Drives; MotorTorqueConstraint, MotorSpeedConstraint): each joint is driven by motors
+ * through a constant transmission.  Motor positions are theta = T q with T an invertible nv x nv matrix (a gear
+ * ratio n_k on the diagonal; off-diagonal entries couple joints, as in a coupled wrist).  Both sides exchange the same
+ * power, so the joint torques tau_j load the motors with T^-T tau_j, and each motor also accelerates its rotor of
+ * inertia I_r (rotor gyroscopic terms neglected, as in pinocchio's armature).  drive_host is a HOST array of
+ * TBD_DRIVE_DOUBLES(nv) doubles:
+ *
+ *   [0, nv*nv)            T, row-major
+ *   [nv*nv, nv*nv + nv)   I_r: rotor inertia of each motor, finite and >= 0
+ *   [nv*nv + nv, ...)     f: Coulomb friction torque of each motor, finite and >= 0
+ *
+ * Every entry refuses (TB_ERR_ARG) a T with a non-finite entry and a singular T: the entry inverts T on the host in fp64
+ * by Gauss-Jordan elimination with partial pivoting and refuses a zero pivot or a non-finite inverse.  T and T^-T travel
+ * to the kernel by value next to the model.  Every matrix-vector sum below is taken left to right.
+ *
+ * tau_m = w(q, qd, qdd) = T^-T ID(q, qd, qdd) + I_r o (T qdd): the motor torques at M points, one thread per point
+ * (the RNEA of tbd_rnea, then the motor map, in that order: (T^-T tau)_i + I_r,i (T qdd)_i).
+ *   q, qd, qdd, tau_m [M][nv].  TB_ERR_ARG for a null pointer, a bad drive and the model checks of tbd_rnea. */
+int tbd_drive_torque(const double *model_host, int nv, const double *drive_host, int M, const double *q,
+                     const double *qd, const double *qdd, double *tau_m, void *stream);
+
+/* The three terms of SecondOrderConstraint with the motor torques as inverse dynamics, in one launch; the joint
+ * transforms are computed once per point and shared by the three passes:
+ *   c = w(q, 0, 0);  a = w(q, 0, qs) - c;  b = w(q, qs, qss) - c;  c = c + f o sign(T qs)
+ * Bit-identical to three tbd_drive_torque launches followed by those element-wise operations (sign: 0 at +-0 and NaN).
+ * With T = I, I_r = 0 and f the joint friction it equals tbd_torque_terms.
+ *   q, qs, qss, a, b, c [M][nv].  The checks of tbd_drive_torque. */
+int tbd_drive_torque_terms(const double *model_host, int nv, const double *drive_host, int M, const double *q,
+                           const double *qs, const double *qss, double *a, double *b, double *c, void *stream);
+
+/* The motor-speed row at qs = q': |theta'_i| s' <= omega_i for every motor i is x = s'^2 times
+ *   b = max_i ((T qs)_i / omega_i)^2 <= 1
+ * one row a = 0, b, c = -1 per point with the feasible set of the nv rows.  Per motor: v = (T qs)_i, r = v / omega_i,
+ * r * r; the maximum propagates NaN (a NaN in qs gives a NaN b).  omega_i = inf contributes 0 (for a finite v).
+ *   speed_limit: HOST array of nv doubles omega_i > 0 (inf allowed); qs [M][nv]; b [M].  TB_ERR_UNSUPPORTED for nv
+ *   outside 1..16; TB_ERR_ARG for a null pointer, M <= 0, an omega_i that is not > 0 (NaN included) and a bad drive. */
+int tbd_drive_speed_terms(int nv, const double *drive_host, const double *speed_limit, int M, const double *qs,
+                          double *b, void *stream);
 
 #ifdef __cplusplus
 }

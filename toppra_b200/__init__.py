@@ -17,7 +17,8 @@ from . import constraint
 from . import solverwrapper
 from . import algorithm
 from .batch import BatchResult, BatchTOPPRA, BatchTOPPRAsd, solve_batch
-from .dynamics import RigidBodyFrame, RigidBodyModel
+from .dynamics import Drives, RigidBodyFrame, RigidBodyModel
+from .constraint import MotorSpeedConstraint, MotorTorqueConstraint
 from .utils import setup_logging
 
 __version__ = "0.1.0"
@@ -26,4 +27,5 @@ logging.getLogger("toppra_b200").addHandler(logging.NullHandler())
 
 __all__ = ["AbstractGeometricPath", "BatchSplineInterpolator", "BatchPiecewisePolyPath", "PiecewisePolyPath", "PPolyPath", "PolynomialPath", "SimplePath", "SplineInterpolator", "UnivariateSplineInterpolator", "propose_gridpoints",
            "ParametrizeConstAccel", "ParametrizeSpline", "BatchParametrizeConstAccel", "BatchParametrizeSpline", "constraint", "solverwrapper", "algorithm", "BatchResult",
-           "BatchTOPPRA", "BatchTOPPRAsd", "solve_batch", "RigidBodyFrame", "RigidBodyModel", "constants", "exceptions", "setup_logging"]
+           "BatchTOPPRA", "BatchTOPPRAsd", "solve_batch", "RigidBodyFrame", "RigidBodyModel", "Drives",
+           "MotorTorqueConstraint", "MotorSpeedConstraint", "constants", "exceptions", "setup_logging"]

@@ -11,6 +11,8 @@ from .contact_stability import ContactStabilityConstraint, contact_wrench_cone
 from .collision_energy import CollisionEnergyConstraint
 from .support_stability import SupportStabilityConstraint, support_polygon_rows
 from .separation_monitoring import SeparationMonitoringConstraint
+from .motor_limits import MotorSpeedConstraint, MotorTorqueConstraint
+from ..dynamics import Drives
 from .conic_constraint import ConicConstraint, RobustLinearConstraint
 
 __all__ = ["ConstraintType", "DiscretizationType", "Constraint", "LinearConstraint",
@@ -18,4 +20,5 @@ __all__ = ["ConstraintType", "DiscretizationType", "Constraint", "LinearConstrai
            "SecondOrderConstraint", "JointTorqueConstraint", "CartesianVelocityNorm", "CartesianAccelerationConstraint",
            "ContactStabilityConstraint", "contact_wrench_cone", "CollisionEnergyConstraint",
            "SupportStabilityConstraint", "support_polygon_rows", "SeparationMonitoringConstraint", "RecordContext",
+           "Drives", "MotorTorqueConstraint", "MotorSpeedConstraint",
            "ConicConstraint", "RobustLinearConstraint"]

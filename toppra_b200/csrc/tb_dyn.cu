@@ -36,6 +36,11 @@
 // Both run point_states, one walk of the tree's bodies with their world placements and velocities in per-thread local
 // arrays, then separation_pair for every pair.
 //
+//   drive_torque_kernel        tau_m = T^-T ID(q, qd, qdd) + I_r o (T qdd), the motor torques of geared drives;
+//   drive_torque_terms_kernel  the terms of MotorTorqueConstraint from the same motor map after each of the three passes;
+//   drive_speed_terms_kernel   b = max_i ((T q')_i / omega_i)^2, the row of MotorSpeedConstraint (no model).
+// The torque kernels run joint_transforms and rnea_pass as rnea_kernel does, then motor_torque.
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -889,6 +894,86 @@ separation_terms_kernel(const __grid_constant__ DynModel m, const __grid_constan
   }
 }
 
+// Geared drives (include/toppra_b200_dyn.h), passed by value next to the model: the transmission T and T^-T (row-major,
+// entries [0, nv) of each), the rotor inertias, the motor friction and, for tbd_drive_speed_terms, the speed limits.
+struct DynDrive {
+  double T[NB][NB], Tit[NB][NB], Ir[NB], f[NB], omega[NB];
+};
+
+// tm = T^-T tau + I_r o (T qdd): per motor i, both sums left to right, then (T^-T tau)_i + I_r,i (T qdd)_i.
+__device__ __forceinline__ void motor_torque(const DynDrive &d, const int nv, const double *tau, const double *qdd,
+                                             double *tm) {
+  for (int i = 0; i < nv; ++i) {
+    double s = d.Tit[i][0] * tau[0], t = d.T[i][0] * qdd[0];
+    for (int j = 1; j < nv; ++j) { s = s + d.Tit[i][j] * tau[j]; t = t + d.T[i][j] * qdd[j]; }
+    tm[i] = s + d.Ir[i] * t;
+  }
+}
+
+// (T x)_i, summed left to right.
+__device__ __forceinline__ double motor_row(const DynDrive &d, const int nv, const int i, const double *x) {
+  double v = d.T[i][0] * x[0];
+  for (int j = 1; j < nv; ++j) v = v + d.T[i][j] * x[j];
+  return v;
+}
+
+__global__ void __launch_bounds__(THREADS)
+drive_torque_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynDrive d, const int nv, const int M,
+                    const double *__restrict__ q, const double *__restrict__ qd, const double *__restrict__ qdd,
+                    double *__restrict__ tau_m) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double X[NB][12], st[NB][12], f[NB][6], t[NB];
+  joint_transforms(m, nv, q + o, X);
+  rnea_pass(m, nv, X, qd + o, qdd + o, st, f, t);
+  motor_torque(d, nv, t, qdd + o, tau_m + o);
+}
+
+// c = w(q, 0, 0), a = w(q, 0, q') - c, b = w(q, q', q'') - c, c += f o sign(T q'): the terms of MotorTorqueConstraint;
+// the joint transforms (and their sincos) are computed once per point and shared by the three passes.
+__global__ void __launch_bounds__(THREADS)
+drive_torque_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynDrive d, const int nv,
+                          const int M, const double *__restrict__ q, const double *__restrict__ qs,
+                          const double *__restrict__ qss, double *__restrict__ a, double *__restrict__ b,
+                          double *__restrict__ c) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double X[NB][12], st[NB][12], f[NB][6], zero[NB], t[NB], wc[NB], w[NB];
+  for (int k = 0; k < nv; ++k) zero[k] = 0.0;
+  joint_transforms(m, nv, q + o, X);
+  rnea_pass(m, nv, X, zero, zero, st, f, t);
+  motor_torque(d, nv, t, zero, wc);
+  rnea_pass(m, nv, X, zero, qs + o, st, f, t);
+  motor_torque(d, nv, t, qs + o, w);
+  for (int k = 0; k < nv; ++k) a[o + k] = w[k] - wc[k];
+  rnea_pass(m, nv, X, qs + o, qss + o, st, f, t);
+  motor_torque(d, nv, t, qss + o, w);
+  for (int k = 0; k < nv; ++k) b[o + k] = w[k] - wc[k];
+  for (int k = 0; k < nv; ++k) {
+    const double x = motor_row(d, nv, k, qs + o);
+    const double sgn = (double)((0.0 < x) - (x < 0.0));   // torch.sign: 0 at +-0 and NaN
+    c[o + k] = wc[k] + sgn * d.f[k];
+  }
+}
+
+// b = max_i ((T q')_i / omega_i)^2, the maximum propagating NaN: the motor-speed row of MotorSpeedConstraint.
+__global__ void __launch_bounds__(THREADS)
+drive_speed_terms_kernel(const __grid_constant__ DynDrive d, const int nv, const int M, const double *__restrict__ qs,
+                         double *__restrict__ b) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const double *x = qs + (size_t)pt * nv;
+  double mx = 0.0;
+  for (int i = 0; i < nv; ++i) {
+    const double r = motor_row(d, nv, i, x) / d.omega[i];
+    const double r2 = r * r;
+    if (!isnan(mx) && (i == 0 || r2 > mx || isnan(r2))) mx = r2;
+  }
+  b[pt] = mx;
+}
+
 int launch_status(const char *what) {
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
@@ -898,10 +983,16 @@ int launch_status(const char *what) {
   return 0;
 }
 
-// Validates the packed model and copies it into the by-value launch parameter: 0, or the TB_ERR_* code (message set).
-int load_model(const double *host, const int nv, const int M, DynModel *m, const char *what) {
+// The point count and the number of bodies (or motors): 0, or the TB_ERR_* code (message set).
+int check_sizes(const int nv, const int M, const char *what) {
   if (M <= 0) { set_error("%s: M=%d must be positive", what, M); return TB_ERR_ARG; }
   if (nv < 1 || nv > NB) { set_error("%s: nv=%d outside 1..%d", what, nv, NB); return TB_ERR_UNSUPPORTED; }
+  return 0;
+}
+
+// Validates the packed model and copies it into the by-value launch parameter: 0, or the TB_ERR_* code (message set).
+int load_model(const double *host, const int nv, const int M, DynModel *m, const char *what) {
+  if (const int rc = check_sizes(nv, M, what)) return rc;
   for (int i = 0; i < 3; ++i) m->g[i] = host[i];
   for (int k = 0; k < NB; ++k)
     for (int j = 0; j < TBD_BODY_DOUBLES; ++j) m->body[k][j] = k < nv ? host[3 + TBD_BODY_DOUBLES * k + j] : 0.0;
@@ -1028,6 +1119,59 @@ int load_points(const double *host, const int P, const int H, const int NH, cons
     for (int j = 0; j < 3; ++j) pts->p[i][j] = f.p[j];
     if (pts->body[i] + 1 > pts->top) pts->top = pts->body[i] + 1;
   }
+  return 0;
+}
+
+// Validates the packed drive (TBD_DRIVE_DOUBLES(nv)) of nv motors, already checked to be in 1..NB, and copies T, T^-T,
+// I_r, f and the speed limits omega (nullable: entries without them) into the by-value launch parameter: 0, or
+// TB_ERR_ARG (message set).  T^-1 by Gauss-Jordan elimination with partial pivoting on [T | I], in fp64.
+int load_drive(const double *host, const int nv, const double *omega, DynDrive *d, const char *what) {
+  *d = DynDrive{};
+  const double *Ir = host + nv * nv, *fr = Ir + nv;
+  for (int j = 0; j < nv * nv; ++j)
+    if (!std::isfinite(host[j])) { set_error("%s: transmission T is not finite", what); return TB_ERR_ARG; }
+  for (int i = 0; i < nv; ++i) {
+    if (!(std::isfinite(Ir[i]) && Ir[i] >= 0.0)) {
+      set_error("%s: motor %d: rotor inertia %g must be finite and >= 0", what, i, Ir[i]);
+      return TB_ERR_ARG;
+    }
+    if (!(std::isfinite(fr[i]) && fr[i] >= 0.0)) {
+      set_error("%s: motor %d: friction %g must be finite and >= 0", what, i, fr[i]);
+      return TB_ERR_ARG;
+    }
+    if (omega && !(omega[i] > 0.0)) {
+      set_error("%s: motor %d: speed limit %g must be > 0 (inf allowed)", what, i, omega[i]);
+      return TB_ERR_ARG;
+    }
+    d->Ir[i] = Ir[i];
+    d->f[i] = fr[i];
+    d->omega[i] = omega ? omega[i] : 0.0;
+  }
+  double A[NB][2 * NB];
+  for (int i = 0; i < nv; ++i)
+    for (int j = 0; j < nv; ++j) {
+      d->T[i][j] = A[i][j] = host[nv * i + j];
+      A[i][nv + j] = i == j ? 1.0 : 0.0;
+    }
+  for (int c = 0; c < nv; ++c) {
+    int p = c;
+    for (int r = c + 1; r < nv; ++r)
+      if (std::fabs(A[r][c]) > std::fabs(A[p][c])) p = r;
+    if (!(A[p][c] != 0.0)) { set_error("%s: transmission T is singular (zero pivot in column %d)", what, c); return TB_ERR_ARG; }
+    for (int j = 0; j < 2 * nv; ++j) { const double x = A[c][j]; A[c][j] = A[p][j]; A[p][j] = x; }
+    const double piv = A[c][c];
+    for (int j = 0; j < 2 * nv; ++j) A[c][j] = A[c][j] / piv;
+    for (int r = 0; r < nv; ++r) {
+      if (r == c) continue;
+      const double e = A[r][c];
+      for (int j = 0; j < 2 * nv; ++j) A[r][j] = A[r][j] - e * A[c][j];
+    }
+  }
+  for (int i = 0; i < nv; ++i)
+    for (int j = 0; j < nv; ++j) {
+      if (!std::isfinite(A[i][nv + j])) { set_error("%s: the inverse of transmission T is not finite", what); return TB_ERR_ARG; }
+      d->Tit[j][i] = A[i][nv + j];
+    }
   return 0;
 }
 
@@ -1247,4 +1391,38 @@ extern "C" int tbd_separation_terms(const double *model_host, int nv, const doub
   const double k = stopping_deceleration * reaction_time + human_speed, kk = k * k;
   return launch(__func__, separation_terms_kernel, M, stream, m, pts, nv, H, points_per_path, clearance, vhTr, twoa, k,
                 kk, M, q, qs, humans, b, c);
+}
+
+extern "C" int tbd_drive_torque(const double *model_host, int nv, const double *drive_host, int M, const double *q,
+                                const double *qd, const double *qdd, double *tau_m, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, drive_host, q, qd, qdd, tau_m)) return rc;
+  DynModel m;
+  DynDrive d;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_drive(drive_host, nv, nullptr, &d, __func__)) return rc;
+  return launch(__func__, drive_torque_kernel, M, stream, m, d, nv, M, q, qd, qdd, tau_m);
+}
+
+extern "C" int tbd_drive_torque_terms(const double *model_host, int nv, const double *drive_host, int M,
+                                      const double *q, const double *qs, const double *qss, double *a, double *b,
+                                      double *c, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, drive_host, q, qs, qss, a, b, c)) return rc;
+  DynModel m;
+  DynDrive d;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_drive(drive_host, nv, nullptr, &d, __func__)) return rc;
+  return launch(__func__, drive_torque_terms_kernel, M, stream, m, d, nv, M, q, qs, qss, a, b, c);
+}
+
+// No model: the speed row needs only the transmission.
+extern "C" int tbd_drive_speed_terms(int nv, const double *drive_host, const double *speed_limit, int M,
+                                     const double *qs, double *b, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, drive_host, speed_limit, qs, b)) return rc;
+  if (const int rc = check_sizes(nv, M, __func__)) return rc;
+  DynDrive d;
+  if (const int rc = load_drive(drive_host, nv, speed_limit, &d, __func__)) return rc;
+  return launch(__func__, drive_speed_terms_kernel, M, stream, d, nv, M, qs, b);
 }

@@ -22,7 +22,11 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     w = floor.support_wrench(None, q, qd, qdd)                # (M, 6) the support's wrench on the whole robot, one launch
     pc = SupportStabilityConstraint(floor, half_lengths=(X, Y), friction=mu)  # the robot must not tip over or slide
     pc = SeparationMonitoringConstraint([(tcp, 0.05)], humans, T_r, a_s)  # speed and separation monitoring
-    d, w = model.separation(pack_points([(tcp, 0.05)])[1], humans, q, qd)  # (M, P, H) separations, approach speeds"""
+    d, w = model.separation(pack_points([(tcp, 0.05)])[1], humans, q, qd)  # (M, P, H) separations, approach speeds
+    drives = Drives(model, gear_ratio=n, rotor_inertia=I_r)   # geared motors (or transmission=T for coupled joints)
+    tau_m = drives.torque(q, qd, qdd)                         # (M, nv) motor torques, one launch
+    pc = MotorTorqueConstraint(drives, motor_limits)          # torque limits on the motor side
+    pc = MotorSpeedConstraint(drives, omega_max)              # motor speed limits"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -473,6 +477,77 @@ class RigidBodyFrame(object):
         tensors (M, nv): one tbd_support_wrench_terms launch.  Returns (a, b, c), each (M, 6)."""
         base = self._support_base(base)
         return _launch(self.model, "tbd_support_wrench_terms", (self.packed, base), (q, qs, qss), [(6,)] * 3)
+
+
+class Drives(object):
+    """The geared drives of a RigidBodyModel: motor positions theta = T q with a constant invertible transmission T.
+    Pass exactly one of `gear_ratio` (nv,), for T = diag(gear_ratio), or `transmission` (nv, nv), whose off-diagonal
+    entries couple joints (a coupled wrist).  rotor_inertia: I_r of each motor, a float or (nv,); friction: Coulomb
+    friction torque of each motor, a float or (nv,).
+
+    The motor torques are w(q, qd, qdd) = T^-T ID(q, qd, qdd) + I_r o (T qdd): the joint torques seen through the
+    transmission plus the torque that accelerates each rotor (the joint-side inertia n^2 I_r of a gear ratio n; rotor
+    gyroscopic terms neglected).  `packed` is the host array of include/toppra_b200_dyn.h (T row-major, I_r, f).  The
+    library checks the values (T finite and invertible, I_r and f finite and >= 0) at every launch."""
+
+    def __init__(self, model, gear_ratio=None, transmission=None, rotor_inertia=0.0, friction=0.0):
+        if not isinstance(model, RigidBodyModel):
+            raise ValueError("Drives needs a RigidBodyModel")
+        nv = model.nv
+        if (gear_ratio is None) == (transmission is None):
+            raise ValueError("Drives: pass exactly one of gear_ratio (nv,) or transmission (nv, nv)")
+        if gear_ratio is not None:
+            n = np.asarray(gear_ratio, dtype=np.float64)
+            if n.shape != (nv,):
+                raise ValueError("Drives: gear_ratio has shape %s; expected (%d,)" % (n.shape, nv))
+            T = np.diag(n)
+        else:
+            T = np.asarray(transmission, dtype=np.float64)
+            if T.shape != (nv, nv):
+                raise ValueError("Drives: transmission has shape %s; expected (%d, %d)" % (T.shape, nv, nv))
+        per_motor = []
+        for name, x in (("rotor_inertia", rotor_inertia), ("friction", friction)):
+            x = np.asarray(x, dtype=np.float64)
+            if x.shape not in ((), (nv,)):
+                raise ValueError("Drives: %s has shape %s; expected a float or (%d,)" % (name, x.shape, nv))
+            per_motor.append(np.broadcast_to(x, (nv,)))
+        self.model = model
+        self.transmission = T.copy()
+        self.rotor_inertia, self.friction = (x.copy() for x in per_motor)
+        self.packed = np.concatenate((T.reshape(-1), per_motor[0], per_motor[1]))
+
+    @property
+    def nv(self):
+        return self.model.nv
+
+    def torque(self, q, qd, qdd):
+        """Motor torques w(q, qd, qdd).  CUDA tensors (M, nv) -> (M, nv), one tbd_drive_torque launch on the current
+        stream; numpy (nv,) or (M, nv) -> numpy, through a device round trip."""
+        if not _is_cuda(q):
+            return _round_trip(self.torque, q, qd, qdd)
+        return _launch(self.model, "tbd_drive_torque", (self.packed,), (q, qd, qdd), [(self.nv,)])
+
+    def torque_terms(self, q, qs, qss):
+        """c = w(q, 0, 0), a = w(q, 0, qs) - c, b = w(q, qs, qss) - c, c += f o sign(T qs) for CUDA tensors (M, nv):
+        one tbd_drive_torque_terms launch.  Returns (a, b, c), each (M, nv)."""
+        return _launch(self.model, "tbd_drive_torque_terms", (self.packed,), (q, qs, qss), [(self.nv,)] * 3)
+
+    def speed_terms(self, qs, speed_limit):
+        """b = max_i ((T qs)_i / omega_i)^2 with omega = speed_limit (nv,) in motor rad/s (inf: no limit), for CUDA
+        tensors (M, nv) -> (M,): one tbd_drive_speed_terms launch.  b s'^2 <= 1 is every motor speed within its
+        limit; NaN in qs gives NaN."""
+        omega = np.ascontiguousarray(speed_limit, dtype=np.float64)
+        if omega.shape != (self.nv,):
+            raise ValueError("Drives: speed_limit has shape %s; expected (%d,)" % (omega.shape, self.nv))
+        torch = _lib.require_cuda()
+        (qs,) = self.model._prepare(torch, qs)
+        b = torch.empty(qs.shape[0], dtype=torch.float64, device=qs.device)
+        with torch.cuda.device(qs.device):
+            _lib.check(_lib_dyn.load().tbd_drive_speed_terms(self.nv, ctypes.c_void_p(self.packed.ctypes.data),
+                                                             ctypes.c_void_p(omega.ctypes.data), qs.shape[0],
+                                                             _lib.ptr(qs), _lib.ptr(b), _lib.stream_ptr()),
+                       "tbd_drive_speed_terms")
+        return b
 
 
 def _is_cuda(x):
