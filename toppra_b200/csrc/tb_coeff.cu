@@ -9,28 +9,18 @@
 //   seidelWrapper.__init__ row assembly (F.a, F.b, F.c - g)        toppra/solverwrapper/cy_seidel_solverwrapper.pyx:474-520
 //
 // Bound: HBM write bandwidth (3R+2 doubles per path and gridpoint; the PPoly input is 4*nseg*dof doubles
-// per path).  One CTA per (path, chunk of CH gridpoints): q', q'' of the chunk (+1 gridpoint for the
+// per path).  One CTA per (path, chunk of VELACC_CH gridpoints): q', q'' of the chunk (+1 gridpoint for the
 // interpolation lift) are evaluated once into shared memory, then every thread writes consecutive doubles of
-// the record stream, so the stores are fully coalesced.
-#include "tb_common.cuh"
+// the record stream, so the stores are fully coalesced.  The record builder is in tb_records.cuh.
+#include "tb_records.cuh"
 
 namespace tb {
 namespace {
 
-constexpr int COEFF_THREADS = 128;
-constexpr int CH = 32;  // gridpoints per CTA
-
-__device__ __forceinline__ int R_total_or1(int R_total) { return R_total > 0 ? R_total : 1; }
-
-// Shared-memory plan of one CTA (dof = d, VS = 6d + 3 doubles per gridpoint, CH gridpoints per CTA):
+// The record builder of tb_records.cuh with q', q'' from the spline.  K1's own shared memory, between sgrid and tab:
+//   sx_s [nseg+1]       breakpoints
 //   dco  [nseg][d][5]   derivative coefficients of the path's PPoly: q' = (3c0, 2c1, c2), q'' = (6c0, 2c1)
-//   raw  [(CH+1)][2d]   q'(s_i), q''(s_i) of the chunk (+1 gridpoint for the lift)
-//   cand [CH][2d]       velocity-bound candidates vlim/q' per joint (upper, lower)
-//   vec  [CH][VS]       per gridpoint: q' | a+ | q'' | b+ | -amax | +amin | xlo | xhi | 0
-//   tab  [W]            per record column: offset into vec (bit 15 = negate, 0x7fff = column not owned)
-// Phase 2: every thread owns one 16-byte column pair and walks down the gridpoints:
-//   rec[ci][col] = +-vec[ci][tab[col]]  -> two shared loads + one coalesced 16-byte store per iteration.
-__global__ void __launch_bounds__(COEFF_THREADS)
+__global__ void __launch_bounds__(VELACC_THREADS)
 coeff_velacc_kernel(const double *__restrict__ ppoly, const double *__restrict__ breaks, const int breaks_shared,
                     const int nseg, const int dof, const double *__restrict__ grid, const int grid_shared, const int G,
                     const double *__restrict__ vlim, const double *__restrict__ alim, const int lim_shared,
@@ -39,19 +29,19 @@ coeff_velacc_kernel(const double *__restrict__ ppoly, const double *__restrict__
   extern __shared__ double sm[];
   const int VS = 6 * dof + 3;
   double *raw = sm;                                  // [(CH+1)][2*dof]
-  double *cand = raw + (CH + 1) * 2 * dof;           // [CH][2*dof]
-  double *vec = cand + CH * 2 * dof;                 // [CH][VS]
-  double *sgrid = vec + CH * VS;                     // [CH+1]
+  double *cand = raw + (VELACC_CH + 1) * 2 * dof;    // [CH][2*dof]
+  double *vec = cand + VELACC_CH * 2 * dof;          // [CH][VS]
+  double *sgrid = vec + VELACC_CH * VS;              // [CH+1]
   // long splines (many waypoints): breakpoints and coefficients stay in global memory (L1/L2)
-  double *sx_s = sgrid + CH + 1;                     // [nseg+1] breakpoints
+  double *sx_s = sgrid + VELACC_CH + 1;              // [nseg+1] breakpoints
   double *dco = sx_s + (pp_in_smem ? nseg + 1 : 0);  // [nseg][dof][5]
   unsigned short *tab = reinterpret_cast<unsigned short *>(dco + (pp_in_smem ? nseg * dof * 5 : 0));  // [W]
   const long path = blockIdx.x / nchunks;
   const int chunk = blockIdx.x % nchunks;
-  const int i0 = chunk * CH;
+  const int i0 = chunk * VELACC_CH;
   const int N = G - 1;
-  const int npts = min(CH, G - i0);          // gridpoints written by this CTA
-  const int nev = min(CH + 1, G - i0);       // gridpoints evaluated (one extra for the lift)
+  const int npts = min(VELACC_CH, G - i0);     // gridpoints written by this CTA
+  const int nev = min(VELACC_CH + 1, G - i0);  // gridpoints evaluated (one extra for the lift)
   const double *c = ppoly + path * 4 * nseg * dof;
   const double *x = breaks + (breaks_shared ? 0 : path * (nseg + 1));
   const double *gp = grid + (grid_shared ? 0 : path * G);
@@ -61,38 +51,21 @@ coeff_velacc_kernel(const double *__restrict__ ppoly, const double *__restrict__
   const int Racc = al ? (interp ? 4 : 2) * dof : 0;
 
   // ---- phase 0: gridpoints, breakpoints, derivative coefficients, column table ----
-  for (int ci = tid; ci < nev; ci += COEFF_THREADS) sgrid[ci] = gp[i0 + ci];
+  for (int ci = tid; ci < nev; ci += VELACC_THREADS) sgrid[ci] = gp[i0 + ci];
   const double *sx = pp_in_smem ? sx_s : x;
-  for (int q = tid; pp_in_smem && q <= nseg; q += COEFF_THREADS) sx_s[q] = x[q];
-  for (int q = tid; pp_in_smem && q < nseg * dof; q += COEFF_THREADS) {
+  for (int q = tid; pp_in_smem && q <= nseg; q += VELACC_THREADS) sx_s[q] = x[q];
+  for (int q = tid; pp_in_smem && q < nseg * dof; q += VELACC_THREADS) {
     // scipy PPoly.derivative: c'[j] = c[j] * (k - j); cspldd = cspld.derivative() (interpolator.py:419-421)
     const double c0 = c[q], c1 = c[nseg * dof + q], c2 = c[2 * nseg * dof + q];
     const double d0 = c0 * 3.0, d1 = c1 * 2.0, d2 = c2 * 1.0;
     double *o = dco + q * 5;
     o[0] = d0; o[1] = d1; o[2] = d2; o[3] = d0 * 2.0; o[4] = d1 * 1.0;
   }
-  for (int w = tid; w < W; w += COEFF_THREADS) {
-    unsigned short code = 0x7fff;  // not owned by this call: leave untouched
-    const int kind = w / R_total_or1(R_total), r = w - kind * R_total - row0;
-    if (kind < 3 && R_total > 0 && r >= 0 && r < Racc) {
-      const int blk = r / dof, k = r - blk * dof;
-      const int neg = blk & 1, second = blk >> 1;
-      if (kind == 0) code = (unsigned short)((second ? dof + k : k) | (neg << 15));
-      else if (kind == 1) code = (unsigned short)((second ? 3 * dof + k : 2 * dof + k) | (neg << 15));
-      else code = (unsigned short)(neg ? 5 * dof + k : 4 * dof + k);
-    } else if (w >= 3 * R_total) {
-      // xlo | xhi | padding zeros; records with a u-bound pair (W >= 3R+4, TB_SCAN_UBOUND) keep those two slots
-      const bool ub_slot = (W >= 3 * R_total + 4) && (w == 3 * R_total + 2 || w == 3 * R_total + 3);
-      if (write_xbound && !ub_slot)
-        code = (unsigned short)(w == 3 * R_total ? 6 * dof : (w == 3 * R_total + 1 ? 6 * dof + 1 : 6 * dof + 2));
-    }
-    tab[w] = code;
-  }
+  velacc_column_table(tab, tid, W, R_total, row0, Racc, dof, write_xbound);
   __syncthreads();
 
   // ---- phase 1: q', q'' at the chunk's gridpoints (+ per-joint velocity-bound candidates) ----
-  const double inf_d = __longlong_as_double(0x7ff0000000000000LL);
-  for (int idx = tid; idx < nev * dof; idx += COEFF_THREADS) {
+  for (int idx = tid; idx < nev * dof; idx += VELACC_THREADS) {
     const int ci = idx / dof, k = idx - ci * dof;
     const double s = sgrid[ci];
     const int seg = find_interval(sx, nseg, s);
@@ -118,105 +91,12 @@ coeff_velacc_kernel(const double *__restrict__ ppoly, const double *__restrict__
       v2 = 0.0 + o[4];
       v2 = v2 + o[3] * ds;
     }
-    raw[ci * 2 * dof + k] = v1;
-    raw[ci * 2 * dof + dof + k] = v2;
-    if (vl && write_xbound && ci < npts) {
-      // _CythonUtils.pyx:44-50: q' > 0: (vmax/q', vmin/q'); q' < 0: (vmin/q', vmax/q'); q' == 0 (or NaN): no update
-      const bool posq = v1 > 0, negq = v1 < 0;
-      const double qd = (posq || negq) ? v1 : 1.0;
-      const double r1 = vl[k * 2 + 1] / qd, r0 = vl[k * 2 + 0] / qd;
-      cand[ci * 2 * dof + k] = posq ? r1 : (negq ? r0 : inf_d);          // candidate for sdmax
-      cand[ci * 2 * dof + dof + k] = posq ? r0 : (negq ? r1 : -inf_d);   // candidate for sdmin
-    }
+    velacc_store_sample(raw, cand, vl, ci, k, dof, npts, v1, v2, write_xbound);
   }
   __syncthreads();
 
-  // ---- phase 1b: per-gridpoint value vectors ----
-  double *rec0 = records + (path * G + i0) * (long)W;
-  for (int idx = tid; idx < npts * dof; idx += COEFF_THREADS) {
-    const int ci = idx / dof, k = idx - ci * dof;
-    const int gi = i0 + ci;
-    double *v = vec + ci * VS;
-    const double a = raw[ci * 2 * dof + k], b = raw[ci * 2 * dof + dof + k];
-    double ap = a, bp = b;  // last gridpoint duplicates itself, linear_constraint.py:171,175
-    if (gi < N) {
-      const double delta = sgrid[ci + 1] - sgrid[ci];
-      ap = raw[(ci + 1) * 2 * dof + k] + (2 * delta) * raw[(ci + 1) * 2 * dof + dof + k];  // linear_constraint.py:170
-      bp = raw[(ci + 1) * 2 * dof + dof + k];
-    }
-    v[k] = a; v[dof + k] = ap; v[2 * dof + k] = b; v[3 * dof + k] = bp;
-    if (al) {
-      v[4 * dof + k] = 0.0 - al[k * 2 + 1];       // F.c - g with c = 0, g = [amax; -amin]
-      v[5 * dof + k] = 0.0 - (-al[k * 2 + 0]);
-    }
-    if (k == 0 && write_xbound) {
-      // velocity bound of this gridpoint: fp32 running min/max over the joints exactly like _CythonUtils.pyx:41-58
-      double xlo = VAR_MIN, xhi = VAR_MAX;  // seidelWrapper low_arr/high_arr init, pyx:477-478
-      if (vl) {
-        // The reference keeps the running min/max in C floats: s <- (float)min(cand_k, (double)s), k = 0..dof-1,
-        // s_0 = 1e8f (_CythonUtils.pyx:41-50).  Round-to-nearest is monotone and idempotent, so that chain equals
-        // (float)min(1e8, min_k cand_k) (likewise for the max): reduce in fp64, round once.
-        double mhi = JVEL_MAXSD, mlo = -JVEL_MAXSD;
-        for (int kk = 0; kk < dof; ++kk) {
-          const double hi = cand[ci * 2 * dof + kk], lo = cand[ci * 2 * dof + dof + kk];
-          mhi = (hi <= mhi) ? hi : mhi;
-          mlo = (lo >= mlo) ? lo : mlo;
-        }
-        const float sdmax = __double2float_rn(mhi), sdmin = __double2float_rn(mlo);
-        const float up = __fmul_rn(sdmax, sdmax);                          // powf(sdmax, 2) in fp32
-        const double lo_d = ((double)sdmin >= 0.0) ? (double)sdmin : 0.0;  // float64_max(sdmin, 0.)
-        xlo = lo_d * lo_d;
-        xhi = (double)up;
-        if (write_xbound != 2) {
-          // pyx:517-520: low = max(VAR_MIN, xbound_lo), high = min(VAR_MAX, xbound_hi)
-          xlo = fmax(VAR_MIN, xlo);
-          xhi = fmin(VAR_MAX, xhi);
-        }
-      }
-      if (write_xbound == 3) {  // intersect with what the record already holds
-        const double *rec = rec0 + (long)ci * W;
-        xlo = fmax(rec[3 * R_total], xlo);
-        xhi = fmin(rec[3 * R_total + 1], xhi);
-      }
-      v[6 * dof] = xlo; v[6 * dof + 1] = xhi; v[6 * dof + 2] = 0.0;
-    }
-  }
-  __syncthreads();
-
-  // ---- phase 2: stream the records out; thread -> fixed 16-byte column pair, loop over gridpoints ----
-  const int Wh = W >> 1;
-  const int ngrp = COEFF_THREADS / Wh;  // gridpoints written per sweep (threads beyond ngrp * Wh idle)
-  const int g = tid / Wh, j = tid - g * Wh;
-  if (ngrp > 0 && g < ngrp) {
-    const unsigned short c0 = tab[2 * j], c1 = tab[2 * j + 1];
-    const int o0 = c0 & 0x7fff, o1 = c1 & 0x7fff;
-    const bool n0 = (c0 & 0x8000) != 0, n1 = (c1 & 0x8000) != 0;
-    const bool own0 = c0 != 0x7fff, own1 = c1 != 0x7fff;
-    double *dst = rec0 + (long)g * W + 2 * j;
-    const double *v = vec + g * VS;
-    if (own0 && own1) {
-      for (int ci = g; ci < npts; ci += ngrp, dst += (long)ngrp * W, v += ngrp * VS) {
-        double2 o;
-        o.x = n0 ? -v[o0] : v[o0];
-        o.y = n1 ? -v[o1] : v[o1];
-        __stcs(reinterpret_cast<double2 *>(dst), o);  // streaming store: written once, read later by K2
-      }
-    } else if (own0 || own1) {
-      for (int ci = g; ci < npts; ci += ngrp, dst += (long)ngrp * W, v += ngrp * VS) {
-        if (own0) dst[0] = n0 ? -v[o0] : v[o0];
-        if (own1) dst[1] = n1 ? -v[o1] : v[o1];
-      }
-    }
-  } else if (ngrp == 0) {  // records wider than 2 * COEFF_THREADS columns: column loop per gridpoint
-    for (int ci = 0; ci < npts; ++ci)
-      for (int w = tid; w < W; w += COEFF_THREADS) {
-        const unsigned short cw = tab[w];
-        if (cw != 0x7fff) {
-          const double t = vec[ci * VS + (cw & 0x7fff)];
-          rec0[(long)ci * W + w] = (cw & 0x8000) ? -t : t;
-        }
-      }
-  }
+  VELACC_WRITE_RECORDS(raw, cand, vec, sgrid, tab, al, vl, records, path, G, i0, N, npts, dof, VS, W, R_total,
+                       write_xbound, tid);
 }
 
 // Generic CanonicalLinear row assembly (seidelWrapper.__init__ pyx:483-510 +
@@ -289,27 +169,8 @@ __global__ void xbound_varying_kernel(const double *__restrict__ ppoly, const do
     const double *vl = per_grid ? vlim_grid + ((vlim_shared ? 0 : p * G) + gi) * (long)dof * 2
                                 : vlim_grid + (vlim_shared ? 0 : p) * (long)dof * 2;
     const int seg = find_interval(x, nseg, s);
-    float sdmin = -(float)JVEL_MAXSD, sdmax = (float)JVEL_MAXSD;
-    for (int k = 0; k < dof && seg >= 0; ++k) {
-      const double q = ppoly_eval1(c, nseg, dof, seg, k, s - x[seg], 1);
-      if (q > 0) {
-        const double hi = vl[k * 2 + 1] / q, lo = vl[k * 2 + 0] / q;
-        sdmax = __double2float_rn(hi <= (double)sdmax ? hi : (double)sdmax);
-        sdmin = __double2float_rn(lo >= (double)sdmin ? lo : (double)sdmin);
-      } else if (q < 0) {
-        const double hi = vl[k * 2 + 0] / q, lo = vl[k * 2 + 1] / q;
-        sdmax = __double2float_rn(hi <= (double)sdmax ? hi : (double)sdmax);
-        sdmin = __double2float_rn(lo >= (double)sdmin ? lo : (double)sdmin);
-      }
-    }
-    const float up = __fmul_rn(sdmax, sdmax);
-    const double lo_d = ((double)sdmin >= 0.0) ? (double)sdmin : 0.0;
-    double xlo = lo_d * lo_d, xhi = (double)up;
-    double *rec = records + idx * W;
-    if (mode != 2) { xlo = fmax(VAR_MIN, xlo); xhi = fmin(VAR_MAX, xhi); }
-    if (mode == 3) { xlo = fmax(rec[3 * R_total], xlo); xhi = fmin(rec[3 * R_total + 1], xhi); }
-    rec[3 * R_total] = xlo;
-    rec[3 * R_total + 1] = xhi;
+    velocity_xbound([&](const int k) { return ppoly_eval1(c, nseg, dof, seg, k, s - x[seg], 1); }, seg >= 0, dof, vl,
+                    records + idx * W, R_total, mode);
   }
 }
 
@@ -479,25 +340,15 @@ extern "C" int tb_coeff_velacc(const double *ppoly, const double *breaks, int br
     set_error("tb_coeff_velacc: bad argument");
     return TB_ERR_ARG;
   }
-  const int Racc = alim ? (interp ? 4 : 2) * dof : 0;
-  if (row0 < 0 || row0 + Racc > R_total || W < 3 * R_total + 2) {
-    set_error("tb_coeff_velacc: rows [%d,%d) do not fit R_total=%d / W=%d", row0, row0 + Racc, R_total, W);
-    return TB_ERR_ARG;
-  }
-  if (R_total > MAX_ROWS) { set_error("tb_coeff_velacc: R=%d > %d", R_total, MAX_ROWS); return TB_ERR_UNSUPPORTED; }
-  if (6 * dof + 3 >= 0x7fff) { set_error("tb_coeff_velacc: dof=%d too large", dof); return TB_ERR_UNSUPPORTED; }
-  const int nchunks = (G + CH - 1) / CH;
+  const int nchunks = (G + VELACC_CH - 1) / VELACC_CH;
   const long blocks = (long)B * nchunks;
-  if (blocks > 0x7fffffffL) { set_error("tb_coeff_velacc: batch too large for one launch"); return TB_ERR_UNSUPPORTED; }
+  if (const int rc = velacc_check("tb_coeff_velacc", alim ? (interp ? 4 : 2) * dof : 0, dof, W, R_total, row0, blocks))
+    return rc;
   const size_t pp_doubles = (size_t)nseg + 1 + (size_t)nseg * dof * 5;
   const int pp_in_smem = pp_doubles * sizeof(double) <= 32 * 1024;
-  const size_t smem = (size_t)((CH + 1) * dof * 2 + CH * dof * 2 + CH * (6 * dof + 3) + CH + 1 +
-                               (pp_in_smem ? pp_doubles : 0)) * sizeof(double) + (size_t)W * sizeof(unsigned short) + 16;
-  if (smem > 48 * 1024) {
-    cudaError_t e = cudaFuncSetAttribute(coeff_velacc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { set_error("tb_coeff_velacc: dof=%d too large for shared memory", dof); return TB_ERR_UNSUPPORTED; }
-  }
-  coeff_velacc_kernel<<<(unsigned)blocks, COEFF_THREADS, smem, (cudaStream_t)stream>>>(
+  const size_t smem = velacc_smem("tb_coeff_velacc", coeff_velacc_kernel, dof, W, pp_in_smem ? pp_doubles : 0);
+  if (!smem) return TB_ERR_UNSUPPORTED;
+  coeff_velacc_kernel<<<(unsigned)blocks, VELACC_THREADS, smem, (cudaStream_t)stream>>>(
       ppoly, breaks, breaks_shared, nseg, dof, grid, grid_shared, G, vlim, alim, lim_shared, interp, records, W,
       R_total, row0, write_xbound, nchunks, pp_in_smem);
   return check_launch("tb_coeff_velacc");
@@ -520,8 +371,7 @@ extern "C" int tb_rows_canlinear(const double *a, const double *b, const double 
   }
   const long total = (long)B * G * nrows;
   const int threads = 256;
-  long blocks = (total + threads - 1) / threads;
-  if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
+  const long blocks = grid_stride_blocks(total, threads, 32);
   rows_canlinear_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(a, b, c, F, g, F_mode, B, G, m, k, grid,
                                                                                grid_shared, interp, records, W,
                                                                                R_total, row0);
@@ -533,8 +383,7 @@ extern "C" int tb_init_bounds(double *records, int B, int G, int W, int R_total,
   if (!records || B <= 0 || G <= 0 || W < 3 * R_total + 2) { set_error("tb_init_bounds: bad argument"); return TB_ERR_ARG; }
   const long BG = (long)B * G;
   const int threads = 256;
-  long blocks = (BG + threads - 1) / threads;
-  if (blocks > (long)num_sms() * 32) blocks = (long)num_sms() * 32;
+  const long blocks = grid_stride_blocks(BG, threads, 32);
   init_bounds_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(records, BG, W, R_total);
   return check_launch("tb_init_bounds");
 }
@@ -550,8 +399,7 @@ extern "C" int tb_xbound_varying(const double *ppoly, const double *breaks, int 
   }
   const long total = (long)B * G;
   const int threads = 128;
-  long blocks = (total + threads - 1) / threads;
-  if (blocks > (long)num_sms() * 64) blocks = (long)num_sms() * 64;
+  const long blocks = grid_stride_blocks(total, threads, 64);
   xbound_varying_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(
       ppoly, breaks, breaks_shared, B, nseg, dof, grid, grid_shared, G, vlim_grid, vlim_shared, 1, records, W, R_total,
       write_xbound);
@@ -603,8 +451,7 @@ extern "C" int tb_xbound_velocity(const double *ppoly, const double *breaks, int
   }
   const long total = (long)B * G;
   const int threads = 128;
-  long blocks = (total + threads - 1) / threads;
-  if (blocks > (long)num_sms() * 64) blocks = (long)num_sms() * 64;
+  const long blocks = grid_stride_blocks(total, threads, 64);
   xbound_varying_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(
       ppoly, breaks, breaks_shared, B, nseg, dof, grid, grid_shared, G, vlim, lim_shared, 0, records, W, R_total,
       write_xbound);

@@ -108,4 +108,22 @@ int check_launch(const char *what);
 // multiprocessor count of the current device (132 on an H100 SXM): sizes grid-stride launches and one-wave batches
 int num_sms();
 
+// CTAs of a grid-stride launch over `total` items: one item per thread, at most per_sm CTAs per multiprocessor.
+inline long grid_stride_blocks(const long total, const int threads, const int per_sm) {
+  const long blocks = (total + threads - 1) / threads;
+  return blocks > (long)num_sms() * per_sm ? (long)num_sms() * per_sm : blocks;
+}
+
+// check_launch for the companion libraries.  Each library carries its own static CUDA runtime, and cudaGetLastError
+// sees only the launches made through it, so each companion reads its launch errors here, through the copy compiled
+// into it (static: a call is never bound to another library's copy), not through libtoppra_b200.so's check_launch.
+static inline int launch_status(const char *what) {
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("%s: launch failed: %s", what, cudaGetErrorString(e));
+    return (int)e;
+  }
+  return 0;
+}
+
 }  // namespace tb

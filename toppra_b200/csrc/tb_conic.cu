@@ -183,15 +183,6 @@ socp_stage_kernel(const double *__restrict__ g, const double *__restrict__ ra, c
   if (lane == 0) { out[2 * p] = us; out[2 * p + 1] = xs; }
 }
 
-int launch_status(const char *what) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("%s: launch failed: %s", what, cudaGetErrorString(e));
-    return (int)e;
-  }
-  return 0;
-}
-
 // Checks shared by both entries: 0, or the TB_ERR_* code (message set).
 int check_conic(const int R, const int conic_row0, const int conic_rows, const double *ell, const char *what) {
   if (R > MAX_ROWS) { set_error("%s: R=%d > %d rows", what, R, MAX_ROWS); return TB_ERR_UNSUPPORTED; }

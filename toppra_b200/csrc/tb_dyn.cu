@@ -974,15 +974,6 @@ drive_speed_terms_kernel(const __grid_constant__ DynDrive d, const int nv, const
   b[pt] = mx;
 }
 
-int launch_status(const char *what) {
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) {
-    set_error("%s: launch failed: %s", what, cudaGetErrorString(e));
-    return (int)e;
-  }
-  return 0;
-}
-
 // The point count and the number of bodies (or motors): 0, or the TB_ERR_* code (message set).
 int check_sizes(const int nv, const int M, const char *what) {
   if (M <= 0) { set_error("%s: M=%d must be positive", what, M); return TB_ERR_ARG; }

@@ -8,7 +8,7 @@
 //   ParametrizeSpline.__init__ time stamps   toppra/parametrizer.py:171-186      -> tb_spline_time_stamps
 // All three are per-path sequential recurrences whose rounding order is the reference's; the batch supplies the
 // parallelism (one warp or one thread per path).  fp64, -fmad=false.
-#include "tb_common.cuh"
+#include "tb_path.cuh"
 #include "tb_propose.cuh"
 
 namespace tb {
@@ -19,21 +19,13 @@ constexpr double PARAM_TINY = 1e-8;  // toppra/constants.py:15 (TINY), used by p
 // ---------------------------------------------------------------------------------------------------------------
 // propose_gridpoints: one warp per path, the passes of tb_propose.cuh on the cubic pieces.
 // ---------------------------------------------------------------------------------------------------------------
-struct CubicQdd {
-  __device__ __forceinline__ int kc() const { return 4; }
-  __device__ __forceinline__ double operator()(const double *c, const int nseg, const int dof, const int seg, const int k,
-                                               const double ds) const {
-    return ppoly_eval1(c, nseg, dof, seg, k, ds, 2);
-  }
-};
-
 __global__ void __launch_bounds__(32)
 propose_gridpoints_kernel(const double *__restrict__ ppoly, const double *__restrict__ breaks, const int breaks_shared,
                           const int B, const int nseg, const int dof, const double max_err, const int max_iter,
                           const double max_seg, const int min_pts, const int Gmax, double *__restrict__ grid_out,
                           double *__restrict__ scratch, int *__restrict__ glen, int *__restrict__ status) {
   propose_gridpoints_warp(ppoly, breaks, breaks_shared, B, nseg, dof, max_err, max_iter, max_seg, min_pts, Gmax, grid_out,
-                          scratch, glen, status, CubicQdd{});
+                          scratch, glen, status, CubicPath{});
 }
 
 // ---------------------------------------------------------------------------------------------------------------

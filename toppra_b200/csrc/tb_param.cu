@@ -8,7 +8,7 @@
 //   __call__ (:82-99)                  q(s) | q'(s) v | q''(s) v^2 + q'(s) u
 // tb_time_grid: one thread per path walks its grid sequentially (the running sum keeps the reference's rounding
 // order).  tb_constaccel_eval: one thread per (path, sample, joint).
-#include "tb_common.cuh"
+#include "tb_path.cuh"
 
 namespace tb {
 namespace {
@@ -38,45 +38,8 @@ __global__ void constaccel_eval_kernel(const double *__restrict__ ppoly, const d
                                        const double *__restrict__ us, const long B, const int G,
                                        const double *__restrict__ ts, const int ts_shared, const int M, const int order,
                                        double *__restrict__ out) {
-  const long total = B * M * dof;
-  for (long idx = (long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
-    const int k = (int)(idx % dof);
-    const long pm = idx / dof;
-    const int m = (int)(pm % M);
-    const long p = pm / M;
-    const double t = ts[(ts_shared ? 0 : p * M) + m];
-    const double *tg = t_grid + p * G;
-    // np.searchsorted(tg, t, side="right") - 1, then idx == len(us) -> idx - 1   (parametrizer.py:117-121)
-    int lo = 0, hi = G;  // first index with tg[j] > t
-    while (lo < hi) {
-      const int mid = (lo + hi) >> 1;
-      if (tg[mid] <= t) lo = mid + 1; else hi = mid;
-    }
-    int i = lo - 1;
-    if (i == G - 1) i = G - 2;
-    // t before the start: the reference indexes with -1, i.e. the LAST entry of each array (knot time, speed and
-    // position at the end, the last stage's acceleration: parametrizer.py:115-128)
-    const int it = i < 0 ? G - 1 : i, iu = i < 0 ? G - 2 : i;
-    const double *sg = grid + (grid_shared ? 0 : p * G);
-    const double dt = t - tg[it];
-    const double u = us[p * (G - 1) + iu];
-    const double v0 = sd[p * G + it];
-    const double v = v0 + dt * u;
-    const double s = sg[it] + dt * v0 + 0.5 * (dt * dt) * u;
-    const double *x = breaks + (breaks_shared ? 0 : p * (nseg + 1));
-    const double *c = ppoly + p * 4 * nseg * dof;
-    const int seg = find_interval(x, nseg, s);
-    double r;
-    if (seg < 0) {
-      r = __longlong_as_double(0x7ff8000000000000LL);
-    } else {
-      const double ds = s - x[seg];
-      if (order == 0) r = ppoly_eval1(c, nseg, dof, seg, k, ds, 0);
-      else if (order == 1) r = ppoly_eval1(c, nseg, dof, seg, k, ds, 1) * v;
-      else r = ppoly_eval1(c, nseg, dof, seg, k, ds, 2) * (v * v) + ppoly_eval1(c, nseg, dof, seg, k, ds, 1) * u;
-    }
-    out[idx] = r;
-  }
+  constaccel_eval(CubicPath{}, ppoly, breaks, breaks_shared, nseg, dof, grid, grid_shared, sd, t_grid, us, B, G, ts,
+                  ts_shared, M, order, out);
 }
 
 }  // namespace
@@ -105,8 +68,7 @@ extern "C" int tb_constaccel_eval(const double *ppoly, const double *breaks, int
   if (order < 0 || order > 2) { set_error("tb_constaccel_eval: order %d not in {0,1,2}", order); return TB_ERR_ARG; }
   const long total = (long)B * M * dof;
   const int threads = 256;
-  long blocks = (total + threads - 1) / threads;
-  if (blocks > (long)num_sms() * 64) blocks = (long)num_sms() * 64;
+  const long blocks = grid_stride_blocks(total, threads, 64);
   constaccel_eval_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(
       ppoly, breaks, breaks_shared, nseg, dof, grid, grid_shared, sd, t_grid, us, B, G, ts, ts_shared, M, order, out);
   return check_launch("tb_constaccel_eval");

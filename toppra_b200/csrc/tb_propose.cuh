@@ -1,5 +1,5 @@
 // tb_propose.cuh — the propose_gridpoints passes of one path on one warp, shared by tb_frows.cu (cubic paths) and
-// tb_poly.cu (order-k paths).  The two callers differ only in how they evaluate q''.
+// tb_poly.cu (order-k paths).  The two callers differ only in their path evaluator (tb_path.cuh).
 //
 // Replaces (reference) propose_gridpoints, toppra/interpolator.py:49-122.  A pass visits every segment of the current
 // (sorted) list; a segment longer than max_seg_length, or whose estimated interpolation error
@@ -11,20 +11,20 @@
 
 namespace tb {
 
-// `qdd` has kc(): the coefficients per piece, and qdd(c, nseg, dof, seg, k, ds): q_k''(x[seg] + ds) of the piece
-// coefficients c of one path.  The parameters are those of the kernels, which call this with blockIdx.x / threadIdx.x.
-template <class Qdd>
+// `path` is a path evaluator (tb_path.cuh).  The parameters are those of the kernels, which call this with
+// blockIdx.x / threadIdx.x.
+template <class Path>
 __device__ __forceinline__ void propose_gridpoints_warp(const double *__restrict__ ppoly,
                                                         const double *__restrict__ breaks, const int breaks_shared,
                                                         const int B, const int nseg, const int dof, const double max_err,
                                                         const int max_iter, const double max_seg, const int min_pts,
                                                         const int Gmax, double *__restrict__ grid_out,
                                                         double *__restrict__ scratch, int *__restrict__ glen,
-                                                        int *__restrict__ status, const Qdd qdd) {
+                                                        int *__restrict__ status, const Path path) {
   const int p = blockIdx.x, lane = threadIdx.x;
   if (p >= B) return;
   const double *x = breaks + (breaks_shared ? 0 : (size_t)p * (nseg + 1));
-  const double *c = ppoly + (size_t)p * qdd.kc() * nseg * dof;
+  const double *c = ppoly + (size_t)p * path.kc() * nseg * dof;
   double *cur = grid_out + (size_t)p * Gmax, *nxt = scratch + (size_t)p * Gmax;
   int n = 2, st = 0;
   if (lane == 0) { cur[0] = x[0]; cur[1] = x[nseg]; }   // path.path_interval
@@ -52,7 +52,8 @@ __device__ __forceinline__ void propose_gridpoints_warp(const double *__restrict
           double worst = -1.0;
           bool isnan_any = false;
           for (int k = 0; k < dof; ++k) {
-            const double e = fabs((0.5 * qdd(c, nseg, dof, seg < 0 ? 0 : seg, k, mid - x[seg < 0 ? 0 : seg])) * d2);
+            const double e =
+                fabs((0.5 * path.eval(c, nseg, dof, seg < 0 ? 0 : seg, k, mid - x[seg < 0 ? 0 : seg], 2)) * d2);
             isnan_any = isnan_any || (e != e);
             worst = (e > worst) ? e : worst;
           }

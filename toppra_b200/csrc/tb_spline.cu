@@ -9,7 +9,7 @@
 //   * evaluation = PPoly.derivative(nu) coefficients (c*3, c*2, ...) + power accumulation of evaluate_poly1.
 // One thread per (path, dof) for the fit (n is small: 5 knots in the BASELINE configs), one thread per
 // output element for the evaluation.  fp64, -fmad=false: bit-identical to scipy on x86-64.
-#include "tb_common.cuh"
+#include "tb_path.cuh"
 
 namespace tb {
 
@@ -21,20 +21,7 @@ __global__ void ppoly_eval_kernel(const double *__restrict__ ppoly, const double
                                   const int breaks_shared, const long B, const int nseg, const int dof,
                                   const double *__restrict__ s, const int s_shared, const int G, const int order,
                                   double *__restrict__ out) {
-  const long total = B * G * dof;
-  for (long idx = (long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
-    const int k = (int)(idx % dof);
-    const long pg = idx / dof;
-    const int gi = (int)(pg % G);
-    const long p = pg / G;
-    const double *x = breaks + (breaks_shared ? 0 : p * (nseg + 1));
-    const double sv = s[(s_shared ? 0 : p * G) + gi];
-    const int seg = find_interval(x, nseg, sv);
-    double r;
-    if (seg < 0) r = __longlong_as_double(0x7ff8000000000000LL);
-    else r = ppoly_eval1(ppoly + p * 4 * nseg * dof, nseg, dof, seg, k, sv - x[seg], order);
-    out[idx] = r;
-  }
+  path_eval(CubicPath{}, ppoly, breaks, breaks_shared, B, nseg, dof, s, s_shared, G, order, out);
 }
 
 // LAPACK dgtsv elimination (partial pivoting) + back substitution, single right-hand side.
@@ -234,8 +221,7 @@ extern "C" int tb_ppoly_eval(const double *ppoly, const double *breaks, int brea
   if (order < 0 || order > 2) { set_error("tb_ppoly_eval: order %d not in {0,1,2}", order); return TB_ERR_ARG; }
   const long total = (long)B * G * dof;
   const int threads = 256;
-  long blocks = (total + threads - 1) / threads;
-  if (blocks > (long)num_sms() * 64) blocks = (long)num_sms() * 64;
+  const long blocks = grid_stride_blocks(total, threads, 64);
   ppoly_eval_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(ppoly, breaks, breaks_shared, B, nseg, dof, s,
                                                                            s_shared, G, order, out);
   return check_launch("tb_ppoly_eval");

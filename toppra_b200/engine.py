@@ -171,6 +171,27 @@ def check_path_vector(t, B, what):
         raise ValueError("%s must have shape (%d,); got %s" % (what, B, tuple(t.shape)))
 
 
+def velacc_limits(vlim, alim, B, dof):
+    """(vlim, alim, shared) for the records of coeff_velacc / rows_velacc_sampled: each limit array (dof, 2) or
+    (B, dof, 2), either may be None.  When one is per path, the other is expanded to (B, dof, 2) and shared is False."""
+    lims = [t for t in (vlim, alim) if t is not None]
+    for t in lims:  # raw pointers go to the kernels: a short limit array would be read out of bounds on the device
+        if t.dim() not in (2, 3) or tuple(t.shape[-2:]) != (dof, 2) or (t.dim() == 3 and t.shape[0] != B):
+            raise ValueError("limits must have shape (dof, 2) or (B, dof, 2) with B = %d, dof = %d; got %s"
+                             % (B, dof, tuple(t.shape)))
+    shared = all(t.dim() == 2 for t in lims)
+    if not shared:
+        vlim = None if vlim is None else (vlim if vlim.dim() == 3 else vlim.expand(B, dof, 2).contiguous())
+        alim = None if alim is None else (alim if alim.dim() == 3 else alim.expand(B, dof, 2).contiguous())
+    return vlim, alim, shared
+
+
+def check_vlim_grid(vlim_grid, B, G, dof):
+    """Per-gridpoint velocity limits: (G, dof, 2) shared by the batch or (B, G, dof, 2)."""
+    if tuple(vlim_grid.shape[-3:]) != (G, dof, 2) or vlim_grid.dim() not in (3, 4) or (vlim_grid.dim() == 4 and vlim_grid.shape[0] != B):
+        raise ValueError("varying velocity limits must have shape (G, dof, 2) or (B, G, dof, 2); got %s" % (tuple(vlim_grid.shape),))
+
+
 def coeff_velacc(ppoly, breaks, grid, vlim, alim, interp, records, R_total, row0=0, write_xbound=1):
     """K1.  vlim/alim: [dof,2] or [B,dof,2] device tensors (either may be None, not both).  Order-k paths: q' and q''
     at the gridpoints (tbp_ppoly_eval), then the records from those samples (rows_velacc_sampled)."""
@@ -178,20 +199,12 @@ def coeff_velacc(ppoly, breaks, grid, vlim, alim, interp, records, R_total, row0
     B, _, nseg, dof = ppoly.shape
     G = grid.shape[-1]
     W = records.shape[-1]
-    lims = [t for t in (vlim, alim) if t is not None]
-    for t in lims:  # raw pointers go to the kernels: a short limit array would be read out of bounds on the device
-        if t.dim() not in (2, 3) or tuple(t.shape[-2:]) != (dof, 2) or (t.dim() == 3 and t.shape[0] != B):
-            raise ValueError("limits must have shape (dof, 2) or (B, dof, 2) with B = %d, dof = %d; got %s"
-                             % (B, dof, tuple(t.shape)))
+    vlim, alim, shared = velacc_limits(vlim, alim, B, dof)
     check_grid_shapes(B, breaks, nseg + 1, grid, G)
     if not is_cubic(ppoly):
         qd, qdd = ppoly_eval(ppoly, breaks, grid, 1), ppoly_eval(ppoly, breaks, grid, 2)
         rows_velacc_sampled(qd, qdd, grid, vlim, alim, interp, records, R_total, row0, write_xbound)
         return
-    shared = all(t.dim() == 2 for t in lims)
-    if not shared:
-        vlim = None if vlim is None else (vlim if vlim.dim() == 3 else vlim.expand(B, dof, 2).contiguous())
-        alim = None if alim is None else (alim if alim.dim() == 3 else alim.expand(B, dof, 2).contiguous())
     with torch.cuda.device(records.device):
         rc = _lib.load().tb_coeff_velacc(_lib.ptr(ppoly), _lib.ptr(breaks), 1 if breaks.dim() == 1 else 0, B, nseg, dof,
                                          _lib.ptr(grid), 1 if grid.dim() == 1 else 0, G, _lib.ptr(vlim),
@@ -210,15 +223,7 @@ def rows_velacc_sampled(qd, qdd, grid, vlim, alim, interp, records, R_total, row
     check_grid(grid, B, G)
     if tuple(records.shape[:2]) != (B, G):
         raise ValueError("records must have shape (%d, %d, W); got %s" % (B, G, tuple(records.shape)))
-    lims = [t for t in (vlim, alim) if t is not None]
-    for t in lims:
-        if t.dim() not in (2, 3) or tuple(t.shape[-2:]) != (dof, 2) or (t.dim() == 3 and t.shape[0] != B):
-            raise ValueError("limits must have shape (dof, 2) or (B, dof, 2) with B = %d, dof = %d; got %s"
-                             % (B, dof, tuple(t.shape)))
-    shared = all(t.dim() == 2 for t in lims)
-    if not shared:
-        vlim = None if vlim is None else (vlim if vlim.dim() == 3 else vlim.expand(B, dof, 2).contiguous())
-        alim = None if alim is None else (alim if alim.dim() == 3 else alim.expand(B, dof, 2).contiguous())
+    vlim, alim, shared = velacc_limits(vlim, alim, B, dof)
     with torch.cuda.device(records.device):
         rc = _lib_poly.load().tbp_rows_velacc_sampled(_lib.ptr(qd), _lib.ptr(qdd), B, dof, _lib.ptr(grid),
                                                       1 if grid.dim() == 1 else 0, G, _lib.ptr(vlim), _lib.ptr(alim),
@@ -750,8 +755,7 @@ def xbound_varying(ppoly, breaks, grid, vlim_grid, records, R_total, write_xboun
     G = grid.shape[-1]
     W = records.shape[-1]
     check_grid_shapes(B, breaks, nseg + 1, grid, G)
-    if tuple(vlim_grid.shape[-3:]) != (G, dof, 2) or vlim_grid.dim() not in (3, 4) or (vlim_grid.dim() == 4 and vlim_grid.shape[0] != B):
-        raise ValueError("varying velocity limits must have shape (G, dof, 2) or (B, G, dof, 2); got %s" % (tuple(vlim_grid.shape),))
+    check_vlim_grid(vlim_grid, B, G, dof)
     if not is_cubic(ppoly):
         xbound_varying_sampled(ppoly_eval(ppoly, breaks, grid, 1), vlim_grid, records, R_total, write_xbound)
         return
@@ -768,8 +772,7 @@ def xbound_varying_sampled(qd, vlim_grid, records, R_total, write_xbound):
     torch = torch_mod()
     B, G, dof = qd.shape
     W = records.shape[-1]
-    if tuple(vlim_grid.shape[-3:]) != (G, dof, 2) or vlim_grid.dim() not in (3, 4) or (vlim_grid.dim() == 4 and vlim_grid.shape[0] != B):
-        raise ValueError("varying velocity limits must have shape (G, dof, 2) or (B, G, dof, 2); got %s" % (tuple(vlim_grid.shape),))
+    check_vlim_grid(vlim_grid, B, G, dof)
     if tuple(records.shape[:2]) != (B, G):
         raise ValueError("records must have shape (%d, %d, W); got %s" % (B, G, tuple(records.shape)))
     with torch.cuda.device(records.device):
