@@ -62,6 +62,9 @@ extern "C" {
 #define TBD_POINT_DOUBLES (TBD_FRAME_DOUBLES + 1)
 #define TBD_MAX_POINTS 16
 #define TBD_MAX_HUMANS 16
+#define TBD_CAPSULE_DOUBLES (2 * TBD_FRAME_DOUBLES + 1)
+#define TBD_HUMAN_CAPSULE_DOUBLES 7
+#define TBD_CAPSULE_PARALLEL 1e-12
 #define TBD_DRIVE_DOUBLES(nv) ((nv) * (nv) + 2 * (nv))
 
 int tbd_version(void);
@@ -236,6 +239,55 @@ int tbd_separation_terms(const double *model_host, int nv, const double *points_
                          int points_per_path, double reaction_time, double stopping_deceleration, double human_speed,
                          double clearance, int M, const double *q, const double *qs, const double *humans, double *b,
                          double *c, void *stream);
+
+/* Speed and separation monitoring with capsules: P robot capsules and H human capsules, for M points, one thread per
+ * point.  capsules_host is a HOST array of P x TBD_CAPSULE_DOUBLES doubles: packed frame a, packed frame b (each
+ * TBD_FRAME_DOUBLES, reference-frame fields ignored) and the radius r_p >= 0.  The robot capsule is the set of points
+ * within r_p of the segment between the two frame origins; the frames may lie on different bodies.  With x_a, v_a and
+ * x_b, v_b the world positions and linear velocities of the two origins (the walk of tbd_separation), the point at
+ * parameter t is p(t) = x_a + t (x_b - x_a) and its velocity v(t) = v_a + t (v_b - v_a), exact for two moving points.
+ * humans is a DEVICE array [NH][H][TBD_HUMAN_CAPSULE_DOUBLES] of capsules (c0(3), c1(3), r_h) in base coordinates, the
+ * points within r_h of the segment c0 -> c1, h(tau) = c0 + tau (c1 - c0); sets are read as in tbd_separation.
+ *
+ * Per pair, capsule-major then h, the closest pair (t, tau) of the two segments (Ericson, Real-Time Collision
+ * Detection 5.1.9), each dot product summed left to right, clamp(x) = x < 0 ? 0 : (x > 1 ? 1 : x) (NaN passes):
+ *   d1 = x_b - x_a;  d2 = c1 - c0;  r0 = x_a - c0;  a = d1.d1;  e = d2.d2;  f = d2.r0
+ *   a == 0 and e == 0:  t = tau = 0
+ *   a == 0:             t = 0;  tau = clamp(f / e)
+ *   otherwise c = d1.r0, and
+ *   e == 0:             tau = 0;  t = clamp(-c / a)            (-c: the negation of c)
+ *   otherwise b = d1.d2;  denom = a * e - b * b;
+ *     parallel, denom <= TBD_CAPSULE_PARALLEL * a * e (evaluated left to right; an angle below about 1e-6 rad):
+ *       t0 = -c / a;  t1 = (b - c) / a;  lo = max(min(t0, t1), 0);  hi = min(max(t0, t1), 1)
+ *       lo <= hi:  the pairs (lo, clamp((b * lo + f) / e)) and (hi, clamp((b * hi + f) / e)) (below)
+ *       lo > hi:   t = 0, then the re-clamp
+ *     not parallel:  t = clamp((b * f - c * e) / denom), then the re-clamp
+ *     re-clamp:  tau = (b * t + f) / e;  tau < 0: tau = 0, t = clamp(-c / a);  tau > 1: tau = 1, t = clamp((b - c) / a)
+ * then with p = x_a + t * d1, v = v_a + t * (v_b - v_a), h = c0 + tau * d2 (per component) the operations of
+ * tbd_separation:  E = h - p;  l = sqrt(E.E);  d = l - r_p - r_h;  w = (E.v) / l, or sqrt(v.v) where l == 0.
+ * Parallel segments whose projections overlap have a segment of closest pairs, along which w is affine in t; the rate
+ * at which the distance closes is the largest w over that set (Danskin's theorem), so both ends are evaluated and
+ * d = the smaller d, w = the larger w of the two.  A capsule with frame a == frame b and a human capsule with
+ * c0 == c1 give the numbers of tbd_separation (signed zeros aside).
+ *   q, qd [M][nv]; d, w [M][P][H].  TB_ERR_UNSUPPORTED for P or H outside 1..16; TB_ERR_ARG for a null pointer, a
+ *   radius r_p that is not finite or is negative, NH < 1, points_per_path < 0 or a points_per_path that reads past set
+ *   NH - 1, and the model and frame checks of tbd_frame_velocity for both frames.  The human capsules are device data
+ *   and are not checked.  The capsules travel by value next to the model (32 endpoints, 1160 bytes), which makes the
+ *   kernel parameters 4696 bytes here and 4744 bytes in tbd_capsule_separation_terms: above the classic 4 KB, within
+ *   the 32 KB that CUDA 12.1+ allows on sm_90a. */
+int tbd_capsule_separation(const double *model_host, int nv, const double *capsules_host, int P, int H, int NH,
+                           int points_per_path, int M, const double *q, const double *qd, const double *humans,
+                           double *d, double *w, void *stream);
+
+/* The row of SeparationMonitoringConstraint at (q, qs = q') with capsules: bit-identical to tbd_capsule_separation
+ * with qd = qs followed by the float64 operations of tbd_separation_terms (the same vmax, binding pair in pair order,
+ * inactive row and NaN rule).
+ *   q, qs [M][nv]; b, c [M].  TB_ERR_ARG for a parameter out of range (NaN included); otherwise the checks of
+ *   tbd_capsule_separation. */
+int tbd_capsule_separation_terms(const double *model_host, int nv, const double *capsules_host, int P, int H, int NH,
+                                 int points_per_path, double reaction_time, double stopping_deceleration,
+                                 double human_speed, double clearance, int M, const double *q, const double *qs,
+                                 const double *humans, double *b, double *c, void *stream);
 
 /* Geared drives (toppra_b200.Drives; MotorTorqueConstraint, MotorSpeedConstraint): each joint is driven by motors
  * through a constant transmission.  Motor positions are theta = T q with T an invertible nv x nv matrix (a gear

@@ -34,6 +34,11 @@ _PROTOS = {
                        _int),
     "tbd_separation_terms": ([_c_dp, _int, _c_dp, _int, _int, _int, _int, ctypes.c_double, ctypes.c_double,
                               ctypes.c_double, ctypes.c_double, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
+    "tbd_capsule_separation": ([_c_dp, _int, _c_dp, _int, _int, _int, _int, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp,
+                                _stream], _int),
+    "tbd_capsule_separation_terms": ([_c_dp, _int, _c_dp, _int, _int, _int, _int, ctypes.c_double, ctypes.c_double,
+                                      ctypes.c_double, ctypes.c_double, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream],
+                                     _int),
     "tbd_drive_torque": ([_c_dp, _int, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
     "tbd_drive_torque_terms": ([_c_dp, _int, _c_dp, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
     "tbd_drive_speed_terms": ([_int, _c_dp, _c_dp, _int, _c_dp, _c_dp, _stream], _int),

@@ -36,6 +36,12 @@
 // Both run point_states, one walk of the tree's bodies with their world placements and velocities in per-thread local
 // arrays, then separation_pair for every pair.
 //
+//   capsule_separation_kernel        d, w of P robot capsules (segments between two frame origins) and H human
+//                                    capsules at (q, qd), one thread per point;
+//   capsule_separation_terms_kernel  the row b, c from the same pairs.
+// Both run point_states on the 2 P endpoints, then capsule_pair (the closest pair of two segments, then
+// separation_pair).  Both terms kernels select the binding pair in separation_row.
+//
 //   drive_torque_kernel        tau_m = T^-T ID(q, qd, qdd) + I_r o (T qdd), the motor torques of geared drives;
 //   drive_torque_terms_kernel  the terms of MotorTorqueConstraint from the same motor map after each of the three passes;
 //   drive_speed_terms_kernel   b = max_i ((T q')_i / omega_i)^2, the row of MotorSpeedConstraint (no model).
@@ -763,18 +769,23 @@ support_wrench_terms_kernel(const __grid_constant__ DynModel m, const __grid_con
 
 // The robot points of speed and separation monitoring (include/toppra_b200_dyn.h), passed by value: each point's body
 // (-1 = the base), the origin p of its frame in body coordinates and its radius.  Bodies [0, top) cover every point's
-// chain (parents come first), so the walk stops there.
-struct DynPoints {
-  double p[TBD_MAX_POINTS][3], r[TBD_MAX_POINTS];
-  int body[TBD_MAX_POINTS];
+// chain (parents come first), so the walk stops there.  NP points at most: the P spheres of tbd_separation, or the 2 P
+// endpoints of tbd_capsule_separation (capsule i = points 2 i and 2 i + 1, its radius in r[2 i]).
+template <int NP>
+struct DynPointSet {
+  double p[NP][3], r[NP];
+  int body[NP];
   int n, top;
 };
+struct DynPoints : DynPointSet<TBD_MAX_POINTS> {};
+struct DynCapsules : DynPointSet<2 * TBD_MAX_POINTS> {};
 
 // World position x and linear velocity v of every point at (q, qd): one walk of the tree's bodies [0, top) with each
 // body's world placement (Rw, pw), angular velocity w and origin velocity vo in per-thread local arrays.  The per-body
 // operations are those of frame_velocity on a chain, so v is bit-identical to the linear part of tbd_frame_velocity
 // for a TBD_LOCAL_WORLD_ALIGNED frame at the point.
-__device__ __forceinline__ void point_states(const DynModel &m, const DynPoints &pts, const double *__restrict__ q,
+template <int NP>
+__device__ __forceinline__ void point_states(const DynModel &m, const DynPointSet<NP> &pts, const double *__restrict__ q,
                                              const double *__restrict__ qd, double (*x)[3], double (*v)[3]) {
   double Rw[NB][9], pw[NB][3], w[NB][3], vo[NB][3];
   for (int k = 0; k < pts.top; ++k) {
@@ -826,11 +837,121 @@ __device__ __forceinline__ void separation_pair(const double *x, const double *v
   ww = l == 0.0 ? sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]) : (e[0] * v[0] + e[1] * v[1] + e[2] * v[2]) / l;
 }
 
-// The human-sphere set of point pt: [H][4] doubles of set pt / points_per_path (set 0 when points_per_path is 0).
+__device__ __forceinline__ double clamp01(const double x) { return x < 0.0 ? 0.0 : (x > 1.0 ? 1.0 : x); }
+
+// Surface separation dd and approach speed ww of the robot capsule (segment xa -> xb, endpoint velocities va, vb,
+// radius rp) and the human capsule hc = (c0, c1, r_h): the closest pair (t, tau) of the two segments (Ericson, Real-Time
+// Collision Detection 5.1.9), then separation_pair of p(t) = xa + t (xb - xa), v(t) = va + t (vb - va) and the sphere
+// (c0 + tau (c1 - c0), r_h).  Parallel segments (denom <= TBD_CAPSULE_PARALLEL a e) whose projections overlap on
+// [t_lo, t_hi] have a segment of closest pairs: both ends are evaluated, dd is the smaller and ww the larger (Danskin).
+// Operation order in include/toppra_b200_dyn.h.
+__device__ __forceinline__ void capsule_pair(const double *xa, const double *va, const double *xb, const double *vb,
+                                             const double rp, const double *hc, double &dd, double &ww) {
+  double d1[3], d2[3], r0[3];
+  for (int j = 0; j < 3; ++j) { d1[j] = xb[j] - xa[j]; d2[j] = hc[3 + j] - hc[j]; r0[j] = xa[j] - hc[j]; }
+  const double a = d1[0] * d1[0] + d1[1] * d1[1] + d1[2] * d1[2];
+  const double e = d2[0] * d2[0] + d2[1] * d2[1] + d2[2] * d2[2];
+  const double f = d2[0] * r0[0] + d2[1] * r0[1] + d2[2] * r0[2];
+  double t = 0.0, tau = 0.0, t2 = 0.0, tau2 = 0.0;
+  bool two = false;
+  if (a == 0.0) {
+    if (e != 0.0) tau = clamp01(f / e);
+  } else {
+    const double c = d1[0] * r0[0] + d1[1] * r0[1] + d1[2] * r0[2];
+    if (e == 0.0) {
+      t = clamp01(-c / a);
+    } else {
+      const double b = d1[0] * d2[0] + d1[1] * d2[1] + d1[2] * d2[2];
+      const double denom = a * e - b * b;
+      bool general = true;
+      if (denom <= TBD_CAPSULE_PARALLEL * a * e) {
+        const double t0 = -c / a, t1 = (b - c) / a;
+        const double lo = fmax(fmin(t0, t1), 0.0), hi = fmin(fmax(t0, t1), 1.0);
+        if (lo <= hi) {
+          t = lo;
+          tau = clamp01((b * lo + f) / e);
+          t2 = hi;
+          tau2 = clamp01((b * hi + f) / e);
+          two = true;
+          general = false;
+        }
+      } else {
+        t = clamp01((b * f - c * e) / denom);
+      }
+      if (general) {
+        tau = (b * t + f) / e;
+        if (tau < 0.0) {
+          tau = 0.0;
+          t = clamp01(-c / a);
+        } else if (tau > 1.0) {
+          tau = 1.0;
+          t = clamp01((b - c) / a);
+        }
+      }
+    }
+  }
+  double p[3], v[3], hs[4];
+  for (int j = 0; j < 3; ++j) {
+    p[j] = xa[j] + t * d1[j];
+    v[j] = va[j] + t * (vb[j] - va[j]);
+    hs[j] = hc[j] + tau * d2[j];
+  }
+  hs[3] = hc[6];
+  separation_pair(p, v, rp, hs, dd, ww);
+  if (two) {
+    for (int j = 0; j < 3; ++j) {
+      p[j] = xa[j] + t2 * d1[j];
+      v[j] = va[j] + t2 * (vb[j] - va[j]);
+      hs[j] = hc[j] + tau2 * d2[j];
+    }
+    double d2_, w2_;
+    separation_pair(p, v, rp, hs, d2_, w2_);
+    if (d2_ < dd) dd = d2_;
+    if (w2_ > ww) ww = w2_;
+  }
+}
+
+// The human set of point pt: [H][HD] doubles of set pt / points_per_path (set 0 when points_per_path is 0); HD = 4 for
+// spheres, TBD_HUMAN_CAPSULE_DOUBLES for capsules.
+template <int HD = 4>
 __device__ __forceinline__ const double *human_set(const double *humans, const int H, const int points_per_path,
                                                    const long pt) {
   const long set = points_per_path > 0 ? pt / points_per_path : 0;
-  return humans + (size_t)set * H * 4;
+  return humans + (size_t)set * H * HD;
+}
+
+// The row of SeparationMonitoringConstraint at point pt from the pairs pair(i, h, dd, ww), i < n, h < H, i-major: per
+// pair
+//   D = dd - C - vhTr;  num = twoa * D;  vmax = D <= 0 ? 0 : num / (sqrt(kk + num) + k)
+// with twoa = 2 a_s, vhTr = v_h T_r, k = a_s T_r + v_h, kk = k k; among the pairs with ww > 0 the first one minimising
+// vmax^2 / ww^2 by cross-multiplication (v2 * bw2 < bv2 * w2, v2 = vmax vmax, w2 = ww ww) gives b = bw2, c = 0 - bv2;
+// no such pair gives b = 0, c = -1; a NaN dd or ww of any pair gives b = c = NaN.
+template <class Pair>
+__device__ __forceinline__ void separation_row(const Pair &pair, const int n, const int H, const double clearance,
+                                               const double vhTr, const double twoa, const double k, const double kk,
+                                               const long pt, double *__restrict__ b, double *__restrict__ c) {
+  double bw2 = 0.0, bv2 = 0.0;
+  bool found = false, bad = false;
+  for (int i = 0; i < n; ++i)
+    for (int h = 0; h < H; ++h) {
+      double dd, ww;
+      pair(i, h, dd, ww);
+      const double D = dd - clearance - vhTr;
+      const double num = twoa * D;
+      const double vmax = D <= 0.0 ? 0.0 : num / (sqrt(kk + num) + k);
+      bad = bad || isnan(ww) || isnan(vmax);
+      if (ww > 0.0) {
+        const double w2 = ww * ww, v2 = vmax * vmax;
+        if (!found || v2 * bw2 < bv2 * w2) { bw2 = w2; bv2 = v2; found = true; }
+      }
+    }
+  if (bad) {
+    b[pt] = nan("");
+    c[pt] = nan("");
+  } else {
+    b[pt] = found ? bw2 : 0.0;
+    c[pt] = found ? 0.0 - bv2 : -1.0;
+  }
 }
 
 __global__ void __launch_bounds__(THREADS)
@@ -853,11 +974,8 @@ separation_kernel(const __grid_constant__ DynModel m, const __grid_constant__ Dy
     }
 }
 
-// The row of SeparationMonitoringConstraint at (q, qs = q'), from the pairs of separation_kernel at qd = qs: per pair
-//   D = dd - C - vhTr;  num = twoa * D;  vmax = D <= 0 ? 0 : num / (sqrt(kk + num) + k)
-// with twoa = 2 a_s, vhTr = v_h T_r, k = a_s T_r + v_h, kk = k k; among the pairs with ww > 0 (p-major, then h) the
-// first one minimising vmax^2 / ww^2 by cross-multiplication (v2 * bw2 < bv2 * w2, v2 = vmax vmax, w2 = ww ww) gives
-// b = bw2, c = 0 - bv2; no such pair gives b = 0, c = -1; a NaN dd or ww of any pair gives b = c = NaN.
+// The row of SeparationMonitoringConstraint at (q, qs = q'), from the pairs of separation_kernel at qd = qs
+// (separation_row).
 __global__ void __launch_bounds__(THREADS)
 separation_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynPoints pts, const int nv,
                         const int H, const int points_per_path, const double clearance, const double vhTr,
@@ -870,28 +988,52 @@ separation_terms_kernel(const __grid_constant__ DynModel m, const __grid_constan
   double x[TBD_MAX_POINTS][3], v[TBD_MAX_POINTS][3];
   point_states(m, pts, q + o, qs + o, x, v);
   const double *hs = human_set(humans, H, points_per_path, pt);
-  double bw2 = 0.0, bv2 = 0.0;
-  bool found = false, bad = false;
-  for (int i = 0; i < pts.n; ++i)
+  separation_row([&](const int i, const int h, double &dd, double &ww) {
+    separation_pair(x[i], v[i], pts.r[i], hs + 4 * h, dd, ww);
+  }, pts.n, H, clearance, vhTr, twoa, k, kk, pt, b, c);
+}
+
+// d, w of P robot capsules (the 2 P endpoints of caps) and H human capsules at (q, qd), capsule-major, then h.
+__global__ void __launch_bounds__(THREADS)
+capsule_separation_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynCapsules caps, const int nv,
+                          const int H, const int points_per_path, const int M, const double *__restrict__ q,
+                          const double *__restrict__ qd, const double *__restrict__ humans, double *__restrict__ dist,
+                          double *__restrict__ speed) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double x[2 * TBD_MAX_POINTS][3], v[2 * TBD_MAX_POINTS][3];
+  point_states(m, caps, q + o, qd + o, x, v);
+  const double *hc = human_set<TBD_HUMAN_CAPSULE_DOUBLES>(humans, H, points_per_path, pt);
+  const int P = caps.n / 2;
+  for (int i = 0; i < P; ++i)
     for (int h = 0; h < H; ++h) {
       double dd, ww;
-      separation_pair(x[i], v[i], pts.r[i], hs + 4 * h, dd, ww);
-      const double D = dd - clearance - vhTr;
-      const double num = twoa * D;
-      const double vmax = D <= 0.0 ? 0.0 : num / (sqrt(kk + num) + k);
-      bad = bad || isnan(ww) || isnan(vmax);
-      if (ww > 0.0) {
-        const double w2 = ww * ww, v2 = vmax * vmax;
-        if (!found || v2 * bw2 < bv2 * w2) { bw2 = w2; bv2 = v2; found = true; }
-      }
+      capsule_pair(x[2 * i], v[2 * i], x[2 * i + 1], v[2 * i + 1], caps.r[2 * i], hc + TBD_HUMAN_CAPSULE_DOUBLES * h,
+                   dd, ww);
+      const size_t r = ((size_t)pt * P + i) * H + h;
+      dist[r] = dd;
+      speed[r] = ww;
     }
-  if (bad) {
-    b[pt] = nan("");
-    c[pt] = nan("");
-  } else {
-    b[pt] = found ? bw2 : 0.0;
-    c[pt] = found ? 0.0 - bv2 : -1.0;
-  }
+}
+
+// The row of SeparationMonitoringConstraint at (q, qs = q') from the pairs of capsule_separation_kernel at qd = qs.
+__global__ void __launch_bounds__(THREADS)
+capsule_separation_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynCapsules caps,
+                                const int nv, const int H, const int points_per_path, const double clearance,
+                                const double vhTr, const double twoa, const double k, const double kk, const int M,
+                                const double *__restrict__ q, const double *__restrict__ qs,
+                                const double *__restrict__ humans, double *__restrict__ b, double *__restrict__ c) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double x[2 * TBD_MAX_POINTS][3], v[2 * TBD_MAX_POINTS][3];
+  point_states(m, caps, q + o, qs + o, x, v);
+  const double *hc = human_set<TBD_HUMAN_CAPSULE_DOUBLES>(humans, H, points_per_path, pt);
+  separation_row([&](const int i, const int h, double &dd, double &ww) {
+    capsule_pair(x[2 * i], v[2 * i], x[2 * i + 1], v[2 * i + 1], caps.r[2 * i], hc + TBD_HUMAN_CAPSULE_DOUBLES * h,
+                 dd, ww);
+  }, caps.n / 2, H, clearance, vhTr, twoa, k, kk, pt, b, c);
 }
 
 // Geared drives (include/toppra_b200_dyn.h), passed by value next to the model: the transmission T and T^-T (row-major,
@@ -1083,33 +1225,90 @@ int load_support(const double *host, const DynModel &m, const int nv, DynFrame *
 // The packed points (P x TBD_POINT_DOUBLES: a packed frame and a radius), the human-sphere sets and their assignment to
 // points, for a model already loaded by load_model: 0, or the TB_ERR_* code (message set).  The frames' reference-frame
 // field is ignored.
-int load_points(const double *host, const int P, const int H, const int NH, const int points_per_path, const int M,
-                const DynModel &m, const int nv, DynPoints *pts, const char *what) {
-  if (P < 1 || P > TBD_MAX_POINTS) { set_error("%s: P=%d points outside 1..%d", what, P, TBD_MAX_POINTS); return TB_ERR_UNSUPPORTED; }
-  if (H < 1 || H > TBD_MAX_HUMANS) { set_error("%s: H=%d human spheres outside 1..%d", what, H, TBD_MAX_HUMANS); return TB_ERR_UNSUPPORTED; }
-  if (NH < 1) { set_error("%s: NH=%d human-sphere sets must be positive", what, NH); return TB_ERR_ARG; }
+// The counts and the assignment of human sets shared by both separation forms: robot and human name the two sides in
+// the messages ("points" and "sphere", or "capsules" and "capsule").
+int check_separation_sets(const int P, const int H, const int NH, const int points_per_path, const int M,
+                          const char *robot, const char *human, const char *what) {
+  if (P < 1 || P > TBD_MAX_POINTS) { set_error("%s: P=%d %s outside 1..%d", what, P, robot, TBD_MAX_POINTS); return TB_ERR_UNSUPPORTED; }
+  if (H < 1 || H > TBD_MAX_HUMANS) { set_error("%s: H=%d human %ss outside 1..%d", what, H, human, TBD_MAX_HUMANS); return TB_ERR_UNSUPPORTED; }
+  if (NH < 1) { set_error("%s: NH=%d human-%s sets must be positive", what, NH, human); return TB_ERR_ARG; }
   if (points_per_path < 0 || (points_per_path > 0 && (M - 1) / points_per_path >= NH)) {
-    set_error("%s: points_per_path=%d with M=%d reads past the NH=%d human-sphere sets", what, points_per_path, M, NH);
+    set_error("%s: points_per_path=%d with M=%d reads past the NH=%d human-%s sets", what, points_per_path, M, NH, human);
     return TB_ERR_ARG;
   }
-  pts->n = P;
+  return 0;
+}
+
+// An empty point set with n points.
+template <int NP>
+void clear_points(DynPointSet<NP> *pts, const int n) {
+  pts->n = n;
   pts->top = 0;
-  for (int i = 0; i < TBD_MAX_POINTS; ++i) {
+  for (int i = 0; i < NP; ++i) {
     pts->body[i] = -1;
     pts->r[i] = 0.0;
     for (int j = 0; j < 3; ++j) pts->p[i][j] = 0.0;
   }
+}
+
+// Point i of the set: the origin of the packed frame fh (checked by load_frame), radius r.
+template <int NP>
+int put_point(const double *fh, const double r, const DynModel &m, const int nv, const int i, DynPointSet<NP> *pts,
+              const char *what) {
+  DynFrame f;
+  if (const int rc = load_frame(fh, m, nv, nullptr, TBD_LOCAL_WORLD_ALIGNED, &f, what)) return rc;
+  pts->body[i] = (int)fh[0];
+  pts->r[i] = r;
+  for (int j = 0; j < 3; ++j) pts->p[i][j] = f.p[j];
+  if (pts->body[i] + 1 > pts->top) pts->top = pts->body[i] + 1;
+  return 0;
+}
+
+int load_points(const double *host, const int P, const int H, const int NH, const int points_per_path, const int M,
+                const DynModel &m, const int nv, DynPoints *pts, const char *what) {
+  if (const int rc = check_separation_sets(P, H, NH, points_per_path, M, "points", "sphere", what)) return rc;
+  clear_points(pts, P);
   for (int i = 0; i < P; ++i) {
     const double *ph = host + (size_t)TBD_POINT_DOUBLES * i;
-    DynFrame f;
-    if (const int rc = load_frame(ph, m, nv, nullptr, TBD_LOCAL_WORLD_ALIGNED, &f, what)) return rc;
     const double r = ph[TBD_FRAME_DOUBLES];
+    if (const int rc = put_point(ph, r, m, nv, i, pts, what)) return rc;
     if (!std::isfinite(r) || r < 0.0) { set_error("%s: point %d: radius %g must be finite and >= 0", what, i, r); return TB_ERR_ARG; }
-    pts->body[i] = (int)ph[0];
-    pts->r[i] = r;
-    for (int j = 0; j < 3; ++j) pts->p[i][j] = f.p[j];
-    if (pts->body[i] + 1 > pts->top) pts->top = pts->body[i] + 1;
   }
+  return 0;
+}
+
+// The packed capsules (P x TBD_CAPSULE_DOUBLES: packed frames a and b and a radius) as the 2 P endpoints of caps, the
+// human-capsule sets and their assignment to points; the checks of load_points, frame a, frame b, then the radius.
+int load_capsules(const double *host, const int P, const int H, const int NH, const int points_per_path, const int M,
+                  const DynModel &m, const int nv, DynCapsules *caps, const char *what) {
+  if (const int rc = check_separation_sets(P, H, NH, points_per_path, M, "capsules", "capsule", what)) return rc;
+  clear_points(caps, 2 * P);
+  for (int i = 0; i < P; ++i) {
+    const double *ch = host + (size_t)TBD_CAPSULE_DOUBLES * i;
+    const double r = ch[2 * TBD_FRAME_DOUBLES];
+    if (const int rc = put_point(ch, r, m, nv, 2 * i, caps, what)) return rc;
+    if (const int rc = put_point(ch + TBD_FRAME_DOUBLES, r, m, nv, 2 * i + 1, caps, what)) return rc;
+    if (!std::isfinite(r) || r < 0.0) { set_error("%s: capsule %d: radius %g must be finite and >= 0", what, i, r); return TB_ERR_ARG; }
+  }
+  return 0;
+}
+
+// The four scalars of the limit (include/toppra_b200_dyn.h, tbd_separation_terms) and the host values the terms
+// kernels take: 0, or TB_ERR_ARG (message set).
+int load_limit(const double reaction_time, const double stopping_deceleration, const double human_speed,
+               const double clearance, double *vhTr, double *twoa, double *k, double *kk, const char *what) {
+  if (!(std::isfinite(reaction_time) && reaction_time >= 0.0 && std::isfinite(stopping_deceleration) &&
+        stopping_deceleration > 0.0 && std::isfinite(human_speed) && human_speed >= 0.0 && std::isfinite(clearance) &&
+        clearance >= 0.0)) {
+    set_error("%s: reaction_time %g, human_speed %g and clearance %g must be finite and >= 0, "
+              "stopping_deceleration %g finite and > 0", what, reaction_time, human_speed, clearance,
+              stopping_deceleration);
+    return TB_ERR_ARG;
+  }
+  *vhTr = human_speed * reaction_time;
+  *twoa = 2.0 * stopping_deceleration;
+  *k = stopping_deceleration * reaction_time + human_speed;
+  *kk = *k * *k;
   return 0;
 }
 
@@ -1366,22 +1565,48 @@ extern "C" int tbd_separation_terms(const double *model_host, int nv, const doub
                                     const double *humans, double *b, double *c, void *stream) {
   using namespace tb;
   if (const int rc = nonnull(__func__, model_host, points_host, q, qs, humans, b, c)) return rc;
-  if (!(std::isfinite(reaction_time) && reaction_time >= 0.0 && std::isfinite(stopping_deceleration) &&
-        stopping_deceleration > 0.0 && std::isfinite(human_speed) && human_speed >= 0.0 && std::isfinite(clearance) &&
-        clearance >= 0.0)) {
-    set_error("%s: reaction_time %g, human_speed %g and clearance %g must be finite and >= 0, "
-              "stopping_deceleration %g finite and > 0", __func__, reaction_time, human_speed, clearance,
-              stopping_deceleration);
-    return TB_ERR_ARG;
-  }
+  double vhTr, twoa, k, kk;
+  if (const int rc = load_limit(reaction_time, stopping_deceleration, human_speed, clearance, &vhTr, &twoa, &k, &kk,
+                                __func__))
+    return rc;
   DynModel m;
   DynPoints pts;
   if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
   if (const int rc = load_points(points_host, P, H, NH, points_per_path, M, m, nv, &pts, __func__)) return rc;
-  const double vhTr = human_speed * reaction_time, twoa = 2.0 * stopping_deceleration;
-  const double k = stopping_deceleration * reaction_time + human_speed, kk = k * k;
   return launch(__func__, separation_terms_kernel, M, stream, m, pts, nv, H, points_per_path, clearance, vhTr, twoa, k,
                 kk, M, q, qs, humans, b, c);
+}
+
+extern "C" int tbd_capsule_separation(const double *model_host, int nv, const double *capsules_host, int P, int H,
+                                      int NH, int points_per_path, int M, const double *q, const double *qd,
+                                      const double *humans, double *d, double *w, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, capsules_host, q, qd, humans, d, w)) return rc;
+  DynModel m;
+  DynCapsules caps;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_capsules(capsules_host, P, H, NH, points_per_path, M, m, nv, &caps, __func__)) return rc;
+  return launch(__func__, capsule_separation_kernel, M, stream, m, caps, nv, H, points_per_path, M, q, qd, humans, d,
+                w);
+}
+
+extern "C" int tbd_capsule_separation_terms(const double *model_host, int nv, const double *capsules_host, int P,
+                                            int H, int NH, int points_per_path, double reaction_time,
+                                            double stopping_deceleration, double human_speed, double clearance, int M,
+                                            const double *q, const double *qs, const double *humans, double *b,
+                                            double *c, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, capsules_host, q, qs, humans, b, c)) return rc;
+  double vhTr, twoa, k, kk;
+  if (const int rc = load_limit(reaction_time, stopping_deceleration, human_speed, clearance, &vhTr, &twoa, &k, &kk,
+                                __func__))
+    return rc;
+  DynModel m;
+  DynCapsules caps;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_capsules(capsules_host, P, H, NH, points_per_path, M, m, nv, &caps, __func__)) return rc;
+  return launch(__func__, capsule_separation_terms_kernel, M, stream, m, caps, nv, H, points_per_path, clearance, vhTr,
+                twoa, k, kk, M, q, qs, humans, b, c);
 }
 
 extern "C" int tbd_drive_torque(const double *model_host, int nv, const double *drive_host, int M, const double *q,

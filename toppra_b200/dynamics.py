@@ -23,6 +23,7 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     pc = SupportStabilityConstraint(floor, half_lengths=(X, Y), friction=mu)  # the robot must not tip over or slide
     pc = SeparationMonitoringConstraint([(tcp, 0.05)], humans, T_r, a_s)  # speed and separation monitoring
     d, w = model.separation(pack_points([(tcp, 0.05)])[1], humans, q, qd)  # (M, P, H) separations, approach speeds
+    pc = SeparationMonitoringConstraint([(elbow, tcp, 0.06)], torsos, T_r, a_s)  # capsules: links and body parts
     drives = Drives(model, gear_ratio=n, rotor_inertia=I_r)   # geared motors (or transmission=T for coupled joints)
     tau_m = drives.torque(q, qd, qdd)                         # (M, nv) motor torques, one launch
     pc = MotorTorqueConstraint(drives, motor_limits)          # torque limits on the motor side
@@ -214,21 +215,24 @@ class RigidBodyModel(object):
         tensors (M, nv): one tbd_separation launch.  points: packed (P, TBD_POINT_DOUBLES) (pack_points); humans:
         (H, 4) or (NH, H, 4) spheres (centre, radius) in base coordinates, point m reading set m // points_per_path
         (set 0 when points_per_path is 0).  With e = c_h - x_p, l = |e|: d = l - r_p - r_h, w = e.v / l (|v| where
-        l == 0), v the point's linear velocity.  Returns (d, w), each (M, P, H)."""
-        P, hum = _check_packed_points(points), _human_sets(humans, q)
-        NH, H = hum.shape[:2]
-        return _launch(self, "tbd_separation", (points, P, H, NH, int(points_per_path)), (q, qd), [(P, H)] * 2,
-                       extra=(hum,))
+        l == 0), v the point's linear velocity.  Returns (d, w), each (M, P, H).
+
+        Capsules on either side (packed (P, TBD_CAPSULE_DOUBLES) robot capsules, or (..., 7) human capsules c0, c1,
+        r_h) make one tbd_capsule_separation launch instead, with the spheres of the other side as capsules of zero
+        length: d and w of the closest pair of every two capsules (include/toppra_b200_dyn.h)."""
+        entry, points, hum = _separation_args(points, humans, q)
+        P, (NH, H) = points.shape[0], hum.shape[:2]
+        return _launch(self, entry, (points, P, H, NH, int(points_per_path)), (q, qd), [(P, H)] * 2, extra=(hum,))
 
     def separation_terms(self, points, humans, reaction_time, stopping_deceleration, human_speed, clearance, q, qs,
                          points_per_path=0):
         """The row (b, c) of SeparationMonitoringConstraint at (q, qs = q') for CUDA tensors (M, nv): one
         tbd_separation_terms launch; the arguments are those of `separation` and the four scalars of the limit
         (include/toppra_b200_dyn.h).  b = w*^2, c = 0 - vmax*^2 of the binding pair, or b = 0, c = -1 where no pair
-        approaches.  Returns (b, c), each (M,)."""
-        P, hum = _check_packed_points(points), _human_sets(humans, q)
-        NH, H = hum.shape[:2]
-        return _launch(self, "tbd_separation_terms",
+        approaches.  Returns (b, c), each (M,).  Capsules on either side: one tbd_capsule_separation_terms launch."""
+        entry, points, hum = _separation_args(points, humans, q)
+        P, (NH, H) = points.shape[0], hum.shape[:2]
+        return _launch(self, entry + "_terms",
                        (points, P, H, NH, int(points_per_path), float(reaction_time), float(stopping_deceleration),
                         float(human_speed), float(clearance)), (q, qs), [(), ()], extra=(hum,))
 
@@ -645,49 +649,90 @@ def _packed_base(base):
 
 FRAME_DOUBLES = 14
 POINT_DOUBLES = FRAME_DOUBLES + 1
+CAPSULE_DOUBLES = 2 * FRAME_DOUBLES + 1
+HUMAN_SPHERE_DOUBLES, HUMAN_CAPSULE_DOUBLES = 4, 7
 MAX_POINTS = MAX_HUMANS = 16
 
 
 def pack_points(points):
-    """The robot points of speed and separation monitoring: a sequence of (RigidBodyFrame, radius) of one model, the
-    sphere of that radius about the frame's origin.  Returns (model, packed (P, TBD_POINT_DOUBLES)): each row the
-    frame's packed doubles and the radius.  ValueError for anything else, frames of different models, a radius that is
-    not finite or is negative, or P outside 1..16."""
+    """The robot points of speed and separation monitoring: a sequence of one model's (RigidBodyFrame, radius), the
+    sphere of that radius about the frame's origin, and (RigidBodyFrame, RigidBodyFrame, radius), the capsule of that
+    radius about the segment between the two origins.  Returns (model, packed): (P, TBD_POINT_DOUBLES) rows of the
+    frame's packed doubles and the radius when every entry is a sphere, else (P, TBD_CAPSULE_DOUBLES) rows of frame a,
+    frame b and the radius, a sphere being the capsule from its frame to itself.  ValueError for anything else, frames
+    of different models, a radius that is not finite or is negative, or P outside 1..16."""
     try:
-        items = [(f, r) for f, r in points]
-    except (TypeError, ValueError):
-        raise ValueError("points: expected a sequence of (RigidBodyFrame, radius)")
+        items = [tuple(it) for it in points]
+    except TypeError:
+        raise ValueError("points: expected a sequence of (RigidBodyFrame, radius) or (RigidBodyFrame, RigidBodyFrame, "
+                         "radius)")
     if not 1 <= len(items) <= MAX_POINTS:
         raise ValueError("points: %d points, supported 1..%d" % (len(items), MAX_POINTS))
-    if not all(isinstance(f, RigidBodyFrame) and np.ndim(r) == 0 for f, r in items):
-        raise ValueError("points: expected a sequence of (RigidBodyFrame, radius)")
+    if not all(len(it) in (2, 3) and all(isinstance(f, RigidBodyFrame) for f in it[:-1])
+               and not isinstance(it[-1], RigidBodyFrame) and np.ndim(it[-1]) == 0 for it in items):
+        raise ValueError("points: expected a sequence of (RigidBodyFrame, radius) or (RigidBodyFrame, RigidBodyFrame, "
+                         "radius)")
     model = items[0][0].model
-    if any(f.model is not model for f, _ in items):
+    if any(f.model is not model for it in items for f in it[:-1]):
         raise ValueError("points: every frame must belong to the same RigidBodyModel")
-    radii = np.array([float(r) for _, r in items])
+    radii = np.array([float(it[-1]) for it in items])
     if not (np.isfinite(radii).all() and (radii >= 0).all()):
         raise ValueError("points: radii must be finite and >= 0; got %s" % radii.tolist())
-    packed = np.concatenate([np.stack([f.packed for f, _ in items]), radii[:, None]], axis=1)
+    capsules = any(len(it) == 3 for it in items)
+    frames = [np.concatenate([it[0].packed, it[-2].packed]) if capsules else it[0].packed for it in items]
+    packed = np.concatenate([np.stack(frames), radii[:, None]], axis=1)
     return model, np.ascontiguousarray(packed)
 
 
+def sphere_points_as_capsules(points):
+    """Packed sphere points (P, TBD_POINT_DOUBLES) as packed capsules (P, TBD_CAPSULE_DOUBLES): frame b = frame a."""
+    f = points[:, :FRAME_DOUBLES]
+    return np.ascontiguousarray(np.concatenate((f, f, points[:, FRAME_DOUBLES:]), axis=1))
+
+
+def sphere_humans_as_capsules(humans):
+    """Human spheres (..., 4) (numpy or torch) as human capsules (..., 7): c1 = c0."""
+    if isinstance(humans, np.ndarray):
+        return np.concatenate((humans[..., :3], humans), axis=-1)
+    torch = _lib.require_cuda()
+    return torch.cat((humans[..., :3], humans), dim=-1).contiguous()
+
+
 def _check_packed_points(points):
-    """P of packed points (P, TBD_POINT_DOUBLES), a contiguous float64 array: the library reads exactly that."""
+    """P of packed points (P, TBD_POINT_DOUBLES) or capsules (P, TBD_CAPSULE_DOUBLES), a contiguous float64 array: the
+    library reads exactly that."""
     if not (isinstance(points, np.ndarray) and points.dtype == np.float64 and points.flags.c_contiguous
-            and points.ndim == 2 and points.shape[1] == POINT_DOUBLES):
-        raise ValueError("packed points: expected a contiguous float64 (P, %d) array (pack_points)" % POINT_DOUBLES)
+            and points.ndim == 2 and points.shape[1] in (POINT_DOUBLES, CAPSULE_DOUBLES)):
+        raise ValueError("packed points: expected a contiguous float64 (P, %d) or (P, %d) array (pack_points)"
+                         % (POINT_DOUBLES, CAPSULE_DOUBLES))
     return points.shape[0]
 
 
 def _human_sets(humans, q):
-    """Human spheres (H, 4) or (NH, H, 4) as a contiguous float64 CUDA tensor (NH, H, 4) on q's device."""
+    """Human spheres (H, 4) or (NH, H, 4), or capsules (H, 7) or (NH, H, 7), as a contiguous float64 CUDA tensor
+    (NH, H, 4 or 7) on q's device."""
     torch = _lib.require_cuda()
     h = torch.as_tensor(humans, dtype=torch.float64, device=q.device if _is_cuda(q) else "cuda")
     if h.dim() == 2:
         h = h.unsqueeze(0)
-    if h.dim() != 3 or h.shape[2] != 4 or h.shape[0] < 1:
-        raise ValueError("humans: expected (H, 4) or (NH, H, 4) spheres (centre, radius); got %s" % (tuple(h.shape),))
+    if h.dim() != 3 or h.shape[2] not in (HUMAN_SPHERE_DOUBLES, HUMAN_CAPSULE_DOUBLES) or h.shape[0] < 1:
+        raise ValueError("humans: expected (H, 4) or (NH, H, 4) spheres (centre, radius), or (H, 7) or (NH, H, 7) "
+                         "capsules (c0, c1, radius); got %s" % (tuple(h.shape),))
     return h.contiguous()
+
+
+def _separation_args(points, humans, q):
+    """(entry, packed points, human sets) of a separation call: "tbd_separation" for sphere points and human spheres,
+    else "tbd_capsule_separation" with the spheres of either side widened to capsules of zero length."""
+    _check_packed_points(points)
+    hum = _human_sets(humans, q)
+    if points.shape[1] == POINT_DOUBLES and hum.shape[2] == HUMAN_SPHERE_DOUBLES:
+        return "tbd_separation", points, hum
+    if points.shape[1] == POINT_DOUBLES:
+        points = sphere_points_as_capsules(points)
+    if hum.shape[2] == HUMAN_SPHERE_DOUBLES:
+        hum = sphere_humans_as_capsules(hum)
+    return "tbd_capsule_separation", points, hum
 
 
 def component_indices(components):
