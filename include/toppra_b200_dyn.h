@@ -328,6 +328,35 @@ int tbd_drive_torque_terms(const double *model_host, int nv, const double *drive
 int tbd_drive_speed_terms(int nv, const double *drive_host, const double *speed_limit, int M, const double *qs,
                           double *b, void *stream);
 
+/* w = the wrench [f(3); n(3)] across joint k, for M points, one thread per point (toppra_b200.constraint.
+ * JointWrenchConstraint): the force and moment the parent side of joint k exerts on everything beyond it, with k the
+ * moving joint of the body frame_host is attached to.  That subtree is body k and every body below it (with the links
+ * folded into them and a payload folded in by the model), and gravity is included: w is the subtree's rate of change of
+ * momentum minus its weight, the moment taken about the frame origin.  Bearings and reducers rate the axial force, the
+ * radial force and the tilting moment of this wrench; tbd_rnea's tau_k is only its component along the joint axis.
+ * With (f_k, n_k) the force of the recursive Newton-Euler pass of tbd_rnea at body k (about body k's origin, body-k
+ * coordinates; gravity as base acceleration -g) and (R_f, p_f) the frame's placement in body k:
+ *   TBD_LOCAL                 w = [R_f^T f_k; R_f^T (n_k - p_f x f_k)]                   (the frame's own axes)
+ *   TBD_LOCAL_WORLD_ALIGNED   w = [R_k f_k; R_k (n_k - p_f x f_k)]                       (world axes)
+ * where R_k = R_c0 R_c1 ... R_k is body k's world orientation, the product of the joint rotations along its root chain.
+ * The order [f; n] is that of tbd_contact_wrench (tbd_rnea's pass stores [n; f]).
+ *   q, qd, qdd [M][nv]; w [M][6].  TB_ERR_UNSUPPORTED for a TBD_WORLD frame; TB_ERR_ARG for a frame on the base
+ *   (body -1: its load is the support wrench of tbd_support_wrench); otherwise the checks of tbd_frame_velocity. */
+int tbd_joint_wrench(const double *model_host, int nv, const double *frame_host, int M, const double *q,
+                     const double *qd, const double *qdd, double *w, void *stream);
+
+/* The three terms of SecondOrderConstraint with the joint wrench as inverse dynamics, in one launch; the joint
+ * transforms and the axes are computed once per point and shared by the three passes:
+ *   c = w(q, 0, 0);  a = w(q, 0, qs) - c;  b = w(q, qs, qss) - c
+ * restricted to the components of the bit mask `components`: bit j selects component j of [fx, fy, fz, nx, ny, nz];
+ * the k = popcount(components) columns come in increasing j.  Bit-identical to three tbd_joint_wrench launches
+ * followed by the two subtractions and that column selection.
+ *   q, qs, qss [M][nv]; a, b, c [M][k].  TB_ERR_ARG for components outside 1..63; otherwise the checks of
+ *   tbd_joint_wrench. */
+int tbd_joint_wrench_terms(const double *model_host, int nv, const double *frame_host, int components, int M,
+                           const double *q, const double *qs, const double *qss, double *a, double *b, double *c,
+                           void *stream);
+
 #ifdef __cplusplus
 }
 #endif

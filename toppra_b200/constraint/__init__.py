@@ -12,6 +12,7 @@ from .collision_energy import CollisionEnergyConstraint
 from .support_stability import SupportStabilityConstraint, support_polygon_rows
 from .separation_monitoring import SeparationMonitoringConstraint
 from .motor_limits import MotorSpeedConstraint, MotorTorqueConstraint
+from .joint_wrench import JointWrenchConstraint
 from ..dynamics import Drives
 from .conic_constraint import ConicConstraint, RobustLinearConstraint
 
@@ -20,5 +21,5 @@ __all__ = ["ConstraintType", "DiscretizationType", "Constraint", "LinearConstrai
            "SecondOrderConstraint", "JointTorqueConstraint", "CartesianVelocityNorm", "CartesianAccelerationConstraint",
            "ContactStabilityConstraint", "contact_wrench_cone", "CollisionEnergyConstraint",
            "SupportStabilityConstraint", "support_polygon_rows", "SeparationMonitoringConstraint", "RecordContext",
-           "Drives", "MotorTorqueConstraint", "MotorSpeedConstraint",
+           "Drives", "MotorTorqueConstraint", "MotorSpeedConstraint", "JointWrenchConstraint",
            "ConicConstraint", "RobustLinearConstraint"]

@@ -48,7 +48,8 @@ class SecondOrderConstraint(LinearConstraint):
         self.device_model = None  # (name, params): inverse dynamics evaluated by tb_coeff_second_order
         self.device_terms = None  # (q, qs, qss) -> (a, b, c): the fused terms launch of the batched route
         self._eye_form = None  # (g [k] or [B,k], friction [m] or None): F = [I;-I] fast form
-        self._const_F = None  # F (k, m) shared by every gridpoint, g = 0
+        self._const_F = None  # F (k, m) shared by every gridpoint
+        self._const_g = None  # g (k,) shared by every gridpoint with _const_F; None: g = 0
         self._format_string = "    Kind: Generalized Second-order constraint\n"
         self._format_string = "    Dimension:\n"
         if not batched:
@@ -190,7 +191,8 @@ class SecondOrderConstraint(LinearConstraint):
             engine.rows_canlinear(a, b, c, None, gd, mode, ctx.d_grid, self.interpolation, records, R_total, row0)
         elif self._const_F is not None:
             Fd = engine.as_device(self._const_F, ctx.device)
-            gd = engine.as_device(np.zeros(self._const_F.shape[0]), ctx.device)
+            g = np.zeros(self._const_F.shape[0]) if self._const_g is None else self._const_g
+            gd = engine.as_device(g, ctx.device)
             engine.rows_canlinear(a, b, c, Fd, gd, 0, ctx.d_grid, self.interpolation, records, R_total, row0)
         else:
             F, g = self._host_Fg

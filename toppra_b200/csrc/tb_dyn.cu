@@ -47,6 +47,10 @@
 //   drive_speed_terms_kernel   b = max_i ((T q')_i / omega_i)^2, the row of MotorSpeedConstraint (no model).
 // The torque kernels run joint_transforms and rnea_pass as rnea_kernel does, then motor_torque.
 //
+//   joint_wrench_kernel        w = the wrench across the joint of a frame's body (on its whole subtree) at (q, qd, qdd);
+//   joint_wrench_terms_kernel  the terms of JointWrenchConstraint, the selected components, from the three passes.
+// Both run joint_transforms and rnea_pass as rnea_kernel does, then joint_wrench on the body's force f[k].
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -1116,6 +1120,81 @@ drive_speed_terms_kernel(const __grid_constant__ DynDrive d, const int nv, const
   b[pt] = mx;
 }
 
+// The axes A of a joint wrench, out = A^T x: R_f for a TBD_LOCAL frame f on body k; for TBD_LOCAL_WORLD_ALIGNED the
+// transpose of body k's world orientation Rw = R_c0 R_c1 ... R_k, the rotations of X along f's chain from the root.
+__device__ __forceinline__ void joint_wrench_axes(const DynFrame &fr, const double (*X)[12], double *A) {
+  if (fr.ref == TBD_LOCAL) {
+    for (int j = 0; j < 9; ++j) A[j] = fr.R[j];
+    return;
+  }
+  double Rw[9], Rn[9];
+  for (int j = 0; j < 9; ++j) Rw[j] = X[fr.chain[0]][j];
+  for (int i = 1; i < fr.n; ++i) {
+    mul33(Rw, X[fr.chain[i]], Rn);
+    for (int j = 0; j < 9; ++j) Rw[j] = Rn[j];
+  }
+  const double Rt[9] = {Rw[0], Rw[3], Rw[6], Rw[1], Rw[4], Rw[7], Rw[2], Rw[5], Rw[8]};
+  for (int j = 0; j < 9; ++j) A[j] = Rt[j];
+}
+
+// The wrench [f; n] the parent side of joint k exerts on k's subtree, at the origin p_f of frame fr (on body k), from
+// the forces of a finished rnea_pass: f[k] = [n_k; f_k] about body k's origin in body-k coordinates, the momentum rate
+// of the subtree minus its weight (gravity enters as base acceleration -g).
+//   out = [A^T f_k; A^T (n_k - p_f x f_k)]   (A: joint_wrench_axes)
+__device__ __forceinline__ void joint_wrench(const DynFrame &fr, const double *A, const double (*f)[6], double *out) {
+  const double *fk = f[fr.chain[fr.n - 1]];
+  double u[3], t[3];
+  cross3(fr.p, fk + 3, u);
+  for (int j = 0; j < 3; ++j) t[j] = fk[j] - u[j];
+  mul3t(A, fk + 3, out);
+  mul3t(A, t, out + 3);
+}
+
+__global__ void __launch_bounds__(THREADS)
+joint_wrench_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame fr, const int nv, const int M,
+                    const double *__restrict__ q, const double *__restrict__ qd, const double *__restrict__ qdd,
+                    double *__restrict__ w) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double X[NB][12], st[NB][12], f[NB][6], t[NB], A[9], y[6];
+  joint_transforms(m, nv, q + o, X);
+  joint_wrench_axes(fr, X, A);
+  rnea_pass(m, nv, X, qd + o, qdd + o, st, f, t);
+  joint_wrench(fr, A, f, y);
+  for (int j = 0; j < 6; ++j) w[(size_t)pt * 6 + j] = y[j];
+}
+
+// c = w(q, 0, 0), a = w(q, 0, q') - c, b = w(q, q', q'') - c: the terms of JointWrenchConstraint, the components of bit
+// mask `components` in increasing order (k = popcount columns); the joint transforms and the axes are computed once per
+// point and shared by the three passes.
+__global__ void __launch_bounds__(THREADS)
+joint_wrench_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynFrame fr, const int nv,
+                          const int components, const int k, const int M, const double *__restrict__ q,
+                          const double *__restrict__ qs, const double *__restrict__ qss, double *__restrict__ a,
+                          double *__restrict__ b, double *__restrict__ c) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double X[NB][12], st[NB][12], f[NB][6], zero[NB], t[NB], A[9], y0[6], y[6];
+  for (int j = 0; j < nv; ++j) zero[j] = 0.0;
+  joint_transforms(m, nv, q + o, X);
+  joint_wrench_axes(fr, X, A);
+  rnea_pass(m, nv, X, zero, zero, st, f, t);
+  joint_wrench(fr, A, f, y0);
+  double *ao = a + (size_t)pt * k, *bo = b + (size_t)pt * k, *co = c + (size_t)pt * k;
+  for (int j = 0, i = 0; j < 6; ++j)
+    if ((components >> j) & 1) co[i++] = y0[j];
+  rnea_pass(m, nv, X, zero, qs + o, st, f, t);
+  joint_wrench(fr, A, f, y);
+  for (int j = 0, i = 0; j < 6; ++j)
+    if ((components >> j) & 1) ao[i++] = y[j] - y0[j];
+  rnea_pass(m, nv, X, qs + o, qss + o, st, f, t);
+  joint_wrench(fr, A, f, y);
+  for (int j = 0, i = 0; j < 6; ++j)
+    if ((components >> j) & 1) bo[i++] = y[j] - y0[j];
+}
+
 // The point count and the number of bodies (or motors): 0, or the TB_ERR_* code (message set).
 int check_sizes(const int nv, const int M, const char *what) {
   if (M <= 0) { set_error("%s: M=%d must be positive", what, M); return TB_ERR_ARG; }
@@ -1217,6 +1296,19 @@ int load_support(const double *host, const DynModel &m, const int nv, DynFrame *
   if (const int rc = load_frame(host, m, nv, nullptr, TBD_LOCAL, s, what)) return rc;
   if (host[0] != -1.0) {
     set_error("%s: the support must be on the base (frame body %g, expected -1)", what, host[0]);
+    return TB_ERR_ARG;
+  }
+  return 0;
+}
+
+// The wrench across a joint is that of the moving joint of the frame's body, at the frame origin: TBD_WORLD is
+// TB_ERR_UNSUPPORTED (refuse_world), and a frame on the base has no joint (TB_ERR_ARG).
+int load_joint_frame(const double *host, const DynModel &m, const int nv, DynFrame *f, const char *what) {
+  if (const int rc = load_frame(host, m, nv, nullptr, -1, f, what)) return rc;
+  if (const int rc = refuse_world(*f, what, " for joint wrenches")) return rc;
+  if (f->n == 0) {
+    set_error("%s: the frame is on the base (body -1), which has no joint; the base's load is the support wrench "
+              "(SupportStabilityConstraint)", what);
     return TB_ERR_ARG;
   }
   return 0;
@@ -1641,4 +1733,32 @@ extern "C" int tbd_drive_speed_terms(int nv, const double *drive_host, const dou
   DynDrive d;
   if (const int rc = load_drive(drive_host, nv, speed_limit, &d, __func__)) return rc;
   return launch(__func__, drive_speed_terms_kernel, M, stream, d, nv, M, qs, b);
+}
+
+extern "C" int tbd_joint_wrench(const double *model_host, int nv, const double *frame_host, int M, const double *q,
+                                const double *qd, const double *qdd, double *w, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, frame_host, q, qd, qdd, w)) return rc;
+  DynModel m;
+  DynFrame f;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_joint_frame(frame_host, m, nv, &f, __func__)) return rc;
+  return launch(__func__, joint_wrench_kernel, M, stream, m, f, nv, M, q, qd, qdd, w);
+}
+
+extern "C" int tbd_joint_wrench_terms(const double *model_host, int nv, const double *frame_host, int components,
+                                      int M, const double *q, const double *qs, const double *qss, double *a, double *b,
+                                      double *c, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, frame_host, q, qs, qss, a, b, c)) return rc;
+  DynModel m;
+  DynFrame f;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_joint_frame(frame_host, m, nv, &f, __func__)) return rc;
+  if (components < 1 || components > 63) {
+    set_error("%s: components=%d must be a bit mask in 1..63", __func__, components);
+    return TB_ERR_ARG;
+  }
+  const int k = __builtin_popcount((unsigned)components);
+  return launch(__func__, joint_wrench_terms_kernel, M, stream, m, f, nv, components, k, M, q, qs, qss, a, b, c);
 }

@@ -27,7 +27,9 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     drives = Drives(model, gear_ratio=n, rotor_inertia=I_r)   # geared motors (or transmission=T for coupled joints)
     tau_m = drives.torque(q, qd, qdd)                         # (M, nv) motor torques, one launch
     pc = MotorTorqueConstraint(drives, motor_limits)          # torque limits on the motor side
-    pc = MotorSpeedConstraint(drives, omega_max)              # motor speed limits"""
+    pc = MotorSpeedConstraint(drives, omega_max)              # motor speed limits
+    w = wrist.joint_wrench(q, qd, qdd)                        # (M, 6) the wrench across the wrist's joint, one launch
+    pc = JointWrenchConstraint.bearing(wrist, axial=F_a, radial=F_r, tilting=M_k)  # bearing and reducer loads"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -482,6 +484,34 @@ class RigidBodyFrame(object):
         base = self._support_base(base)
         return _launch(self.model, "tbd_support_wrench_terms", (self.packed, base), (q, qs, qss), [(6,)] * 3)
 
+    def _check_joint_wrench(self):
+        """ValueError where this frame has no joint wrench: a frame on the base or a "world" frame."""
+        if self.body < 0:
+            raise ValueError("RigidBodyFrame %r is on the base (body -1), which has no joint; the base's load is the "
+                             "support wrench (SupportStabilityConstraint)" % self.name)
+        self._refuse_world("the joint wrench is taken about the frame origin")
+
+    def joint_wrench(self, q, qd, qdd):
+        """The wrench [fx, fy, fz, nx, ny, nz] across the joint of this frame's body: the force and moment the parent
+        side of that joint exerts on everything beyond it (the body, the bodies below it and what is folded into them),
+        gravity included, the moment about this frame's origin.  "local": in the frame's axes; "local_world_aligned":
+        in world axes; "world" and a frame on the base raise ValueError.  Its component along the joint axis at the
+        body origin is the joint torque.  CUDA tensors (M, nv) -> (M, 6), one tbd_joint_wrench launch on the current
+        stream; numpy (nv,) -> (6,) or (M, nv) -> (M, 6), through a device round trip."""
+        self._check_joint_wrench()
+        if not _is_cuda(q):
+            return _round_trip(self.joint_wrench, q, qd, qdd)
+        return _launch(self.model, "tbd_joint_wrench", (self.packed,), (q, qd, qdd), [(6,)])
+
+    def joint_wrench_terms(self, q, qs, qss, components=(0, 1, 2, 3, 4, 5)):
+        """c = w(q, 0, 0), a = w(q, 0, qs) - c, b = w(q, qs, qss) - c of the joint wrench (joint_wrench) for CUDA
+        tensors (M, nv), restricted to `components` (indices into [fx, fy, fz, nx, ny, nz]; the columns come in
+        increasing index order): one tbd_joint_wrench_terms launch.  Returns (a, b, c), each (M, k)."""
+        self._check_joint_wrench()
+        comps = component_indices(components, WRENCH_COMPONENTS)
+        mask = sum(1 << j for j in comps)
+        return _launch(self.model, "tbd_joint_wrench_terms", (self.packed, mask), (q, qs, qss), [(len(comps),)] * 3)
+
 
 class Drives(object):
     """The geared drives of a RigidBodyModel: motor positions theta = T q with a constant invertible transmission T.
@@ -735,12 +765,15 @@ def _separation_args(points, humans, q):
     return "tbd_capsule_separation", points, hum
 
 
-def component_indices(components):
-    """Sorted indices into [ax, ay, az, wx, wy, wz] of a frame acceleration; ValueError when `components` is empty,
-    repeats an index or has one outside 0..5."""
+ACCELERATION_COMPONENTS = "[ax, ay, az, wx, wy, wz]"
+WRENCH_COMPONENTS = "[fx, fy, fz, nx, ny, nz]"
+
+
+def component_indices(components, names=ACCELERATION_COMPONENTS):
+    """Sorted indices into `names` (a frame acceleration's [ax, ay, az, wx, wy, wz] by default); ValueError when
+    `components` is empty, repeats an index or has one outside 0..5."""
     comps = np.asarray(components).reshape(-1)
     if (comps.size == 0 or comps.dtype.kind not in "iu" or len(set(comps.tolist())) != comps.size
             or comps.min() < 0 or comps.max() > 5):
-        raise ValueError("components %r: expected distinct indices in 0..5 of [ax, ay, az, wx, wy, wz]"
-                         % (components,))
+        raise ValueError("components %r: expected distinct indices in 0..5 of %s" % (components, names))
     return sorted(comps.tolist())
