@@ -66,6 +66,8 @@ extern "C" {
 #define TBD_HUMAN_CAPSULE_DOUBLES 7
 #define TBD_CAPSULE_PARALLEL 1e-12
 #define TBD_DRIVE_DOUBLES(nv) ((nv) * (nv) + 2 * (nv))
+#define TBD_KINETIC_ENERGY 0
+#define TBD_MOMENTUM 1
 
 int tbd_version(void);
 
@@ -356,6 +358,30 @@ int tbd_joint_wrench(const double *model_host, int nv, const double *frame_host,
 int tbd_joint_wrench_terms(const double *model_host, int nv, const double *frame_host, int components, int M,
                            const double *q, const double *qs, const double *qss, double *a, double *b, double *c,
                            void *stream);
+
+/* The kinetic energy T and the linear momentum p of the whole robot at (q, qd), for M points, one thread per point
+ * (toppra_b200.constraint.KineticEnergyConstraint, MomentumConstraint):
+ *   T = 1/2 qd^T M(q) qd = 1/2 sum_k (m_k |v_ck|^2 + w_k^T I_ck w_k);   p = sum_k m_k v_ck = m_total v_com
+ * summed over the moving bodies (with the links folded into them and a payload folded in by the model; the static base
+ * does not move), v_ck the velocity of body k's centre of mass, w_k its angular velocity and I_ck its rotational inertia
+ * about the centre of mass.  p is in base axes.  One forward walk of bodies 0..nv-1 gives each body's world rotation
+ * Rw_k, angular velocity w_k and origin velocity vo_k (as the walk of tbd_separation); then for each body, in body
+ * order, with d = Rw_k c_k, every sum left to right:
+ *   v_c = vo_k + w_k x d;  w_b = Rw_k^T w_k;  e += m_k (v_c . v_c) + w_b . (Ic_k w_b);  p += m_k v_c;  T = 0.5 e
+ * No mass-matrix inverse is involved: a model whose joints move no inertia is fine.
+ *   q, qd [M][nv]; out [M][4] = T, px, py, pz.  TB_ERR_UNSUPPORTED for nv outside 1..16; TB_ERR_ARG for a null pointer,
+ *   M <= 0 and the model checks of tbd_rnea. */
+int tbd_energy_momentum(const double *model_host, int nv, int M, const double *q, const double *qd, double *out,
+                        void *stream);
+
+/* The row of KineticEnergyConstraint or MomentumConstraint at (q, qs = q'): along a path qd = q' s', so T = b s'^2 and
+ * |p|^2 = b s'^2 with
+ *   which = TBD_KINETIC_ENERGY   b = T(q, qs)
+ *   which = TBD_MOMENTUM         b = (px px + py py) + pz pz,  p = p(q, qs)
+ * Bit-identical to tbd_energy_momentum followed by that choice.
+ *   q, qs [M][nv]; b [M].  TB_ERR_ARG for any other `which`; otherwise the checks of tbd_energy_momentum. */
+int tbd_energy_momentum_terms(const double *model_host, int nv, int which, int M, const double *q, const double *qs,
+                              double *b, void *stream);
 
 #ifdef __cplusplus
 }

@@ -13,6 +13,7 @@ from .support_stability import SupportStabilityConstraint, support_polygon_rows
 from .separation_monitoring import SeparationMonitoringConstraint
 from .motor_limits import MotorSpeedConstraint, MotorTorqueConstraint
 from .joint_wrench import JointWrenchConstraint
+from .kinetic_energy import KineticEnergyConstraint, MomentumConstraint
 from ..dynamics import Drives
 from .conic_constraint import ConicConstraint, RobustLinearConstraint
 
@@ -22,4 +23,5 @@ __all__ = ["ConstraintType", "DiscretizationType", "Constraint", "LinearConstrai
            "ContactStabilityConstraint", "contact_wrench_cone", "CollisionEnergyConstraint",
            "SupportStabilityConstraint", "support_polygon_rows", "SeparationMonitoringConstraint", "RecordContext",
            "Drives", "MotorTorqueConstraint", "MotorSpeedConstraint", "JointWrenchConstraint",
+           "KineticEnergyConstraint", "MomentumConstraint",
            "ConicConstraint", "RobustLinearConstraint"]

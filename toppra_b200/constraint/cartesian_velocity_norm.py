@@ -113,8 +113,9 @@ class CartesianVelocityNorm(LinearConstraint):
                         R_total, row0)
 
 
-# ---- a limit b(q, q') s'^2 <= limit: the parts shared by CartesianVelocityNorm and CollisionEnergyConstraint, whose
-# `cons` has dof, limit (a float, or None) and _path_limits ((Bfull,) or None) and _interp() ------------------------
+# ---- a limit b(q, q') s'^2 <= limit: the parts shared by CartesianVelocityNorm, CollisionEnergyConstraint,
+# KineticEnergyConstraint and MomentumConstraint, whose `cons` has dof, limit (a float, or None) and _path_limits
+# ((Bfull,) or None) and _interp() ----------------------------------------------------------------------------------
 def single_path_limit(cons):
     """The limit of the single-path route: the float, or the only per-path limit."""
     if cons._path_limits is None:

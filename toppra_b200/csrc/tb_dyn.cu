@@ -51,6 +51,10 @@
 //   joint_wrench_terms_kernel  the terms of JointWrenchConstraint, the selected components, from the three passes.
 // Both run joint_transforms and rnea_pass as rnea_kernel does, then joint_wrench on the body's force f[k].
 //
+//   energy_momentum_kernel        T, p = the kinetic energy and the linear momentum of the whole tree at (q, qd);
+//   energy_momentum_terms_kernel  b = T or p.p at (q, q'): the row of KineticEnergyConstraint or MomentumConstraint.
+// Both run energy_momentum, one forward velocity walk of the tree (no force pass), one thread per point.
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -1195,6 +1199,82 @@ joint_wrench_terms_kernel(const __grid_constant__ DynModel m, const __grid_const
     if ((components >> j) & 1) bo[i++] = y[j] - y0[j];
 }
 
+// The kinetic energy T and the linear momentum p (base axes) of the whole tree at (q, qd): one walk of bodies [0, nv)
+// with each body's world rotation Rw, angular velocity w and origin velocity vo in per-thread local arrays (the per-body
+// operations of point_states), and for each body, in body order, with d = Rw c:
+//   vc = vo + w x d;  wb = Rw^T w;  e += m ((vc0 vc0 + vc1 vc1) + vc2 vc2) + ((wb0 Iwb0 + wb1 Iwb1) + wb2 Iwb2);
+//   p += m vc;        (Iwb = Ic wb)
+// and T = 0.5 e.  No world origin is kept: neither sum depends on where a body is.
+__device__ __forceinline__ void energy_momentum(const DynModel &m, const int nv, const double *__restrict__ q,
+                                                const double *__restrict__ qd, double &T, double *p) {
+  double Rw[NB][9], w[NB][3], vo[NB][3];
+  double e = 0.0;
+  for (int j = 0; j < 3; ++j) p[j] = 0.0;
+  for (int k = 0; k < nv; ++k) {
+    const double *bd = m.body[k];
+    const int par = (int)bd[0];
+    double Rp[9] = {1.0, 0.0, 0.0, 0.0, 1.0, 0.0, 0.0, 0.0, 1.0};
+    double wp[3] = {0.0, 0.0, 0.0}, vp[3] = {0.0, 0.0, 0.0};
+    if (par >= 0) {
+      for (int j = 0; j < 9; ++j) Rp[j] = Rw[par][j];
+      for (int j = 0; j < 3; ++j) { wp[j] = w[par][j]; vp[j] = vo[par][j]; }
+    }
+    double R[9], po[3], d[3], t[3];
+    const double qk = q[k];
+    TB_BODY_TRANSFORM(bd, qk, R, po);
+    mul3(Rp, po, d);                    // origin of body k relative to its parent's, world coordinates
+    cross3(wp, d, t);
+    for (int j = 0; j < 3; ++j) vo[k][j] = vp[j] + t[j];
+    mul33(Rp, R, Rw[k]);
+    double s[3];
+    mul3(Rw[k], bd + 2, s);             // joint axis, world coordinates
+    const double qdk = qd[k];
+    if (bd[1] == TBD_REVOLUTE) {
+      for (int j = 0; j < 3; ++j) { w[k][j] = wp[j] + s[j] * qdk; }
+    } else {
+      for (int j = 0; j < 3; ++j) { w[k][j] = wp[j]; vo[k][j] = vo[k][j] + s[j] * qdk; }
+    }
+    const double mass = bd[17], *c = bd + 18, *Ic = bd + 21;
+    double vc[3], wb[3], Iwb[3];
+    mul3(Rw[k], c, d);                  // centre of mass relative to the body origin, world coordinates
+    cross3(w[k], d, t);
+    for (int j = 0; j < 3; ++j) vc[j] = vo[k][j] + t[j];
+    mul3t(Rw[k], w[k], wb);             // angular velocity, body coordinates
+    mul_inertia(Ic, wb, Iwb);
+    const double vv = vc[0] * vc[0] + vc[1] * vc[1] + vc[2] * vc[2];
+    const double ww = wb[0] * Iwb[0] + wb[1] * Iwb[1] + wb[2] * Iwb[2];
+    e = e + (mass * vv + ww);
+    for (int j = 0; j < 3; ++j) p[j] = p[j] + mass * vc[j];
+  }
+  T = 0.5 * e;
+}
+
+__global__ void __launch_bounds__(THREADS)
+energy_momentum_kernel(const __grid_constant__ DynModel m, const int nv, const int M, const double *__restrict__ q,
+                       const double *__restrict__ qd, double *__restrict__ out) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double T, p[3];
+  energy_momentum(m, nv, q + o, qd + o, T, p);
+  double *y = out + (size_t)pt * 4;
+  y[0] = T;
+  for (int j = 0; j < 3; ++j) y[1 + j] = p[j];
+}
+
+// b = T(q, q') (which = TBD_KINETIC_ENERGY) or (px px + py py) + pz pz (TBD_MOMENTUM): the row of KineticEnergyConstraint
+// or MomentumConstraint.
+__global__ void __launch_bounds__(THREADS)
+energy_momentum_terms_kernel(const __grid_constant__ DynModel m, const int nv, const int which, const int M,
+                             const double *__restrict__ q, const double *__restrict__ qs, double *__restrict__ b) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nv;
+  double T, p[3];
+  energy_momentum(m, nv, q + o, qs + o, T, p);
+  b[pt] = which == TBD_KINETIC_ENERGY ? T : p[0] * p[0] + p[1] * p[1] + p[2] * p[2];
+}
+
 // The point count and the number of bodies (or motors): 0, or the TB_ERR_* code (message set).
 int check_sizes(const int nv, const int M, const char *what) {
   if (M <= 0) { set_error("%s: M=%d must be positive", what, M); return TB_ERR_ARG; }
@@ -1761,4 +1841,26 @@ extern "C" int tbd_joint_wrench_terms(const double *model_host, int nv, const do
   }
   const int k = __builtin_popcount((unsigned)components);
   return launch(__func__, joint_wrench_terms_kernel, M, stream, m, f, nv, components, k, M, q, qs, qss, a, b, c);
+}
+
+extern "C" int tbd_energy_momentum(const double *model_host, int nv, int M, const double *q, const double *qd,
+                                   double *out, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, q, qd, out)) return rc;
+  DynModel m;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  return launch(__func__, energy_momentum_kernel, M, stream, m, nv, M, q, qd, out);
+}
+
+extern "C" int tbd_energy_momentum_terms(const double *model_host, int nv, int which, int M, const double *q,
+                                         const double *qs, double *b, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, q, qs, b)) return rc;
+  if (which != TBD_KINETIC_ENERGY && which != TBD_MOMENTUM) {
+    set_error("%s: which=%d must be TBD_KINETIC_ENERGY (0) or TBD_MOMENTUM (1)", __func__, which);
+    return TB_ERR_ARG;
+  }
+  DynModel m;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  return launch(__func__, energy_momentum_terms_kernel, M, stream, m, nv, which, M, q, qs, b);
 }

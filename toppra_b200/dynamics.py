@@ -29,7 +29,10 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     pc = MotorTorqueConstraint(drives, motor_limits)          # torque limits on the motor side
     pc = MotorSpeedConstraint(drives, omega_max)              # motor speed limits
     w = wrist.joint_wrench(q, qd, qdd)                        # (M, 6) the wrench across the wrist's joint, one launch
-    pc = JointWrenchConstraint.bearing(wrist, axial=F_a, radial=F_r, tilting=M_k)  # bearing and reducer loads"""
+    pc = JointWrenchConstraint.bearing(wrist, axial=F_a, radial=F_r, tilting=M_k)  # bearing and reducer loads
+    T, p = model.energy_momentum(q, qd)                       # (M,), (M, 3) kinetic energy and momentum, one launch
+    pc = KineticEnergyConstraint(model, E_max)                # the energy of the whole arm in motion
+    pc = MomentumConstraint(model, p_max)                     # its linear momentum"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -43,6 +46,8 @@ REVOLUTE, PRISMATIC = 0, 1
 _JOINT_TYPES = {"revolute": REVOLUTE, "continuous": REVOLUTE, "prismatic": PRISMATIC}
 # pinocchio's ReferenceFrame values (include/toppra_b200_dyn.h TBD_WORLD, TBD_LOCAL, TBD_LOCAL_WORLD_ALIGNED)
 REFERENCE_FRAMES = {"world": 0, "local": 1, "local_world_aligned": 2}
+# the row of tbd_energy_momentum_terms (include/toppra_b200_dyn.h TBD_KINETIC_ENERGY, TBD_MOMENTUM)
+ENERGY_MOMENTUM = {"energy": 0, "momentum": 1}
 
 
 def rpy_matrix(rpy):
@@ -237,6 +242,24 @@ class RigidBodyModel(object):
         return _launch(self, entry + "_terms",
                        (points, P, H, NH, int(points_per_path), float(reaction_time), float(stopping_deceleration),
                         float(human_speed), float(clearance)), (q, qs), [(), ()], extra=(hum,))
+
+    def energy_momentum(self, q, qd):
+        """The kinetic energy T = 1/2 qd^T M(q) qd (J) and the linear momentum p = m_total v_com (kg m/s, base axes) of
+        the whole robot at (q, qd): every moving body, with what is folded into it (fixed and locked links, payloads).
+        CUDA tensors (M, nv) -> (T (M,), p (M, 3)), one tbd_energy_momentum launch on the current stream; numpy (nv,)
+        -> (float, (3,)) or (M, nv) -> ((M,), (M, 3)), through a device round trip."""
+        if not _is_cuda(q):
+            out = _round_trip(lambda *x: _launch(self, "tbd_energy_momentum", (), x, [(4,)]), q, qd)
+            return (float(out[0]), out[1:]) if np.ndim(q) == 1 else (out[:, 0], out[:, 1:])
+        out = _launch(self, "tbd_energy_momentum", (), (q, qd), [(4,)])
+        return out[:, 0], out[:, 1:]
+
+    def energy_momentum_terms(self, q, qs, which):
+        """b of KineticEnergyConstraint (which = "energy": T(q, qs)) or MomentumConstraint (which = "momentum":
+        |p(q, qs)|^2) for CUDA tensors (M, nv): one tbd_energy_momentum_terms launch.  Returns b (M,)."""
+        if which not in ENERGY_MOMENTUM:
+            raise ValueError("energy_momentum_terms: which=%r, expected one of %s" % (which, sorted(ENERGY_MOMENTUM)))
+        return _launch(self, "tbd_energy_momentum_terms", (ENERGY_MOMENTUM[which],), (q, qs), [()])
 
     # ---- URDF ---------------------------------------------------------------------------------------------------
     @classmethod
