@@ -68,6 +68,7 @@ extern "C" {
 #define TBD_DRIVE_DOUBLES(nv) ((nv) * (nv) + 2 * (nv))
 #define TBD_KINETIC_ENERGY 0
 #define TBD_MOMENTUM 1
+#define TBD_COUPLING_DOUBLES(nv, nq) ((nv) * (nq) + (nv))
 
 int tbd_version(void);
 
@@ -382,6 +383,48 @@ int tbd_energy_momentum(const double *model_host, int nv, int M, const double *q
  *   q, qs [M][nv]; b [M].  TB_ERR_ARG for any other `which`; otherwise the checks of tbd_energy_momentum. */
 int tbd_energy_momentum_terms(const double *model_host, int nv, int which, int M, const double *q, const double *qs,
                               double *b, void *stream);
+
+/* Coupled joints (toppra_b200.RigidBodyModel with a coupling: URDF mimic joints, RigidBodyModel.with_coupling): the nv
+ * body joint positions are affine in nq <= nv independent path DOFs, q_b = E q + o, so qd_b = E qd and qdd_b = E qdd.
+ * A URDF mimic joint is a row of E with one nonzero entry, q_k = multiplier q_src + offset; an uncoupled model is
+ * E = I, o = 0.  coupling_host is a HOST array of TBD_COUPLING_DOUBLES(nv, nq) doubles:
+ *
+ *   [0, nv*nq)            E (nv x nq), row-major
+ *   [nv*nq, nv*nq + nv)   o
+ *
+ * The generalized forces on the DOFs follow from virtual work, tau_q = E^T ID(q_b, qd_b, qdd_b), exact for the
+ * holonomic constraint q_b = E q + o: forces inside the mechanism that realises the coupling do no virtual work.
+ * Operation order, fixed with __dmul_rn / __dadd_rn whatever the contraction flags:
+ *   expansion   (E x)_k: the nonzero terms E[k][j] x[j] in ascending j, starting from the first term (0 for a row
+ *               without one); positions then add o[k] where o[k] != 0
+ *   reduction   (E^T t)_j: the nonzero terms E[k][j] t[k] in ascending k, starting from the first term
+ * With E = I and o = 0 both dynamics entries are bit-identical to tbd_rnea and tbd_torque_terms.  Every entry refuses
+ * nq outside 1..nv (TB_ERR_UNSUPPORTED), a non-finite E or o and a zero column of E, a DOF that moves no body
+ * (TB_ERR_ARG).  The coupling travels to the kernel by value next to the model (2176 bytes): the kernel parameters are
+ * above the classic 4 KB, within the 32 KB that CUDA 12.1+ allows on sm_90a.
+ *
+ * tau_q = E^T ID(E q + o, E qd, E qdd) for M points, one thread per point: the expansion, the RNEA of tbd_rnea on the
+ * nv bodies, then the reduction.
+ *   q, qd, qdd, tau [M][nq].  TB_ERR_ARG for a null pointer and the model checks of tbd_rnea, then the coupling's. */
+int tbd_coupled_rnea(const double *model_host, int nv, const double *coupling_host, int nq, int M, const double *q,
+                     const double *qd, const double *qdd, double *tau, void *stream);
+
+/* The terms of tbd_torque_terms on the nq DOFs, one thread per point, with q_b = E q + o, qs_b = E qs, qss_b = E qss:
+ *   c = E^T ID(q_b, 0, 0);  a = E^T (ID(q_b, 0, qs_b) - ID(q_b, 0, 0));  b = E^T (ID(q_b, qs_b, qss_b) - ID(q_b, 0, 0));
+ *   c = c + sign(qs) * friction  (friction != NULL, per DOF)
+ * the subtractions in body space as in tbd_torque_terms, then the reduction.  Bit-identical to tbd_coupling_expand,
+ * tbd_torque_terms without friction on the expanded points, the reduction of a, b and c, then the friction term.
+ *   q, qs, qss, a, b, c [M][nq]; friction (nullable) [nq].  The checks of tbd_coupled_rnea. */
+int tbd_coupled_torque_terms(const double *model_host, int nv, const double *coupling_host, int nq, int M,
+                             const double *q, const double *qs, const double *qss, const double *friction, double *a,
+                             double *b, double *c, void *stream);
+
+/* q_out = E q + o, qd_out = E qd, qdd_out = E qdd for M points, one thread per point: the body-space inputs of every
+ * other entry on a coupled model.  qd and qd_out (qdd and qdd_out) are both given or both NULL.
+ *   q, qd, qdd [M][nq]; q_out, qd_out, qdd_out [M][nv].  TB_ERR_UNSUPPORTED for nv outside 1..16; TB_ERR_ARG for a
+ *   null q, q_out or coupling, a rate without its output (or the reverse) and M <= 0; then the coupling's checks. */
+int tbd_coupling_expand(int nv, const double *coupling_host, int nq, int M, const double *q, const double *qd,
+                        const double *qdd, double *q_out, double *qd_out, double *qdd_out, void *stream);
 
 #ifdef __cplusplus
 }

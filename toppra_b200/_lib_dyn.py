@@ -1,6 +1,6 @@
 """ctypes binding of libtoppra_b200_dyn.so (include/toppra_b200_dyn.h): rigid-body inverse dynamics (RNEA) of a
-fixed-base tree, the motor side of its geared drives, the wrench across a joint and the kinetic energy and momentum of
-the whole tree.
+fixed-base tree, the motor side of its geared drives, the wrench across a joint, the kinetic energy and momentum of
+the whole tree, and linearly coupled joints (URDF mimic joints).
 
 The companion library links against libtoppra_b200.so and reports errors through its tb_last_error(), so errors are
 read with `_lib.check`.  There is NO CPU fallback: if the library is missing or a call fails, this module raises."""
@@ -48,6 +48,10 @@ _PROTOS = {
                                _int),
     "tbd_energy_momentum": ([_c_dp, _int, _int, _c_dp, _c_dp, _c_dp, _stream], _int),
     "tbd_energy_momentum_terms": ([_c_dp, _int, _int, _int, _c_dp, _c_dp, _c_dp, _stream], _int),
+    "tbd_coupled_rnea": ([_c_dp, _int, _c_dp, _int, _int, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
+    "tbd_coupled_torque_terms": ([_c_dp, _int, _c_dp, _int, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp,
+                                  _stream], _int),
+    "tbd_coupling_expand": ([_int, _c_dp, _int, _int, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _stream], _int),
 }
 
 _dlib = None

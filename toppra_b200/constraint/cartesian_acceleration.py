@@ -46,7 +46,7 @@ class CartesianAccelerationConstraint(SecondOrderConstraint):
         g_aug = np.concatenate((alim[..., 1], -alim[..., 0]), axis=-1)
         g_single = g_aug if g_aug.ndim == 1 else g_aug[0]
         super(CartesianAccelerationConstraint, self).__init__(frame.acceleration, lambda _: eyes, lambda _: g_single,
-                                                              frame.nv, discretization_scheme=discretization_scheme,
+                                                              frame.dof, discretization_scheme=discretization_scheme,
                                                               batched=True)
         self._eye_form = (g_aug, np.zeros(k))
         self.device_terms = self._terms

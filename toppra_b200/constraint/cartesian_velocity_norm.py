@@ -34,10 +34,10 @@ class CartesianVelocityNorm(LinearConstraint):
         self.compute_velocity = compute_velocity
         self.velocity_limit = velocity_limit
         frame = isinstance(compute_velocity, RigidBodyFrame)
-        if frame and dof is not None and dof != compute_velocity.nv:
+        if frame and dof is not None and dof != compute_velocity.dof:
             raise ValueError("Wrong dimension: constraint dof ({:d}) not equal to the frame's model dof ({:d})".format(
-                dof, compute_velocity.nv))
-        self.dof = compute_velocity.nv if frame and dof is None else dof
+                dof, compute_velocity.dof))
+        self.dof = compute_velocity.dof if frame and dof is None else dof
         self._path_limits = None   # (B,) limits of the device route
         if velocity_limit is None:
             if S is None or limit is None:

@@ -37,6 +37,7 @@ class CollisionEnergyConstraint(LinearConstraint):
         if not isinstance(frame, RigidBodyFrame):
             raise ValueError("CollisionEnergyConstraint needs a RigidBodyFrame (RigidBodyModel.frame(...)) as the "
                              "contact point")
+        frame.model._refuse_coupled("CollisionEnergyConstraint")
         self.set_discretization_type(discretization_scheme)
         lim = np.array(limit, dtype=np.float64)
         if lim.ndim > 1:
@@ -51,7 +52,7 @@ class CollisionEnergyConstraint(LinearConstraint):
             raise ValueError("CollisionEnergyConstraint: joint(s) %s move no inertia (their bodies and descendants have "
                              "zero mass and inertia), so the mass matrix is singular" % ", ".join(map(repr, dead)))
         self.frame = frame
-        self.dof = frame.nv
+        self.dof = frame.dof
         self.human_mass = human_mass
         self.limit, self._path_limits = (float(lim), None) if lim.ndim == 0 else (None, lim)
         self.identical = True

@@ -91,7 +91,7 @@ class ContactStabilityConstraint(SecondOrderConstraint):
         mass, com, _ = _rigid_inertia("ContactStabilityConstraint", mass, com, inertia)
         F = contact_wrench_cone(half_lengths, friction)
         zeros = np.zeros(NUM_ROWS)
-        super(ContactStabilityConstraint, self).__init__(self.wrench, lambda _: F, lambda _: zeros, frame.nv,
+        super(ContactStabilityConstraint, self).__init__(self.wrench, lambda _: F, lambda _: zeros, frame.dof,
                                                          discretization_scheme=discretization_scheme, batched=True)
         self.frame = frame
         self.F = self._const_F = F

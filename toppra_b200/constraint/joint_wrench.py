@@ -103,7 +103,7 @@ class JointWrenchConstraint(SecondOrderConstraint):
         eyes = np.vstack((np.eye(k), -np.eye(k)))
         g_aug = np.concatenate((wlim[..., 1], -wlim[..., 0]), axis=-1)
         g_single = g_aug if g_aug.ndim == 1 else g_aug[0]
-        super(JointWrenchConstraint, self).__init__(self._selected, lambda _: eyes, lambda _: g_single, frame.nv,
+        super(JointWrenchConstraint, self).__init__(self._selected, lambda _: eyes, lambda _: g_single, frame.dof,
                                                     discretization_scheme=discretization_scheme, batched=True)
         self._eye_form = (g_aug, np.zeros(k))
         self.frame = frame
@@ -136,7 +136,7 @@ class JointWrenchConstraint(SecondOrderConstraint):
         axis = frame.R.T @ frame.model.body(frame.body)[2:5]  # the joint axis in body k's coordinates, in frame axes
         F, g = bearing_rows(axis, *(None if v is None else float(v) for v in limits.values()), sides=int(sides))
         obj = cls.__new__(cls)
-        SecondOrderConstraint.__init__(obj, frame.joint_wrench, lambda _: F, lambda _: g, frame.nv,
+        SecondOrderConstraint.__init__(obj, frame.joint_wrench, lambda _: F, lambda _: g, frame.dof,
                                        discretization_scheme=discretization_scheme, batched=True)
         obj._const_F, obj._const_g = F, g
         obj.F, obj.g = F, g

@@ -45,7 +45,7 @@ class _WholeRobotLimit(LinearConstraint):
         if np.isnan(lim).any() or (lim < 0).any():
             raise ValueError("%s: the limit must be >= 0 (not NaN); got %s" % (name, limit))
         self.model = model
-        self.dof = model.nv
+        self.dof = model.dof
         rows = self._row_limit(lim)
         self.limit, self._path_limits = (float(rows), None) if lim.ndim == 0 else (None, rows)
         self.identical = True

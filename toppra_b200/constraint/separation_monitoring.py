@@ -71,7 +71,7 @@ class SeparationMonitoringConstraint(LinearConstraint):
             hum = sphere_humans_as_capsules(hum)
         self.humans = hum
         self.per_path = hum.ndim == 3
-        self.dof = self.model.nv
+        self.dof = self.model.dof
         self.identical = True
         self._dev_humans = None
         self._format_string = "    Speed and separation monitoring: {:d} {:}, {:d} human {:}{:}\n".format(

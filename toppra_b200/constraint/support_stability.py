@@ -108,7 +108,7 @@ class SupportStabilityConstraint(SecondOrderConstraint):
             F = support_polygon_rows(polygon, friction)
             self.half_lengths, self.polygon = None, _polygon(polygon).copy()
         zeros = np.zeros(F.shape[0])
-        super(SupportStabilityConstraint, self).__init__(self.wrench, lambda _: F, lambda _: zeros, support.nv,
+        super(SupportStabilityConstraint, self).__init__(self.wrench, lambda _: F, lambda _: zeros, support.dof,
                                                          discretization_scheme=discretization_scheme, batched=True)
         self.support = support
         self.F = self._const_F = F

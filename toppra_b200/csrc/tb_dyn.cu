@@ -55,6 +55,13 @@
 //   energy_momentum_terms_kernel  b = T or p.p at (q, q'): the row of KineticEnergyConstraint or MomentumConstraint.
 // Both run energy_momentum, one forward velocity walk of the tree (no force pass), one thread per point.
 //
+//   coupled_rnea_kernel          tau_q = E^T ID(E q + o, E qd, E qdd): the torques on the nq independent DOFs of a
+//                                linearly coupled model (URDF mimic joints), one thread per point;
+//   coupled_torque_terms_kernel  the terms of torque_terms_kernel on the expanded state, reduced by E^T;
+//   coupling_expand_kernel       q_b = E q + o and the rates E qd, E qdd: the expanded inputs of every other entry.
+// The two dynamics kernels expand into per-thread arrays and run joint_transforms and rnea_pass unchanged;
+// coupling_expand and coupling_reduce fix their operation order with __dmul_rn / __dadd_rn.
+//
 // Featherstone's spatial RNEA in body coordinates: motion vectors (w, v) and forces (n, f) about the body origin.
 // X[k] = (R, p): R maps body-k coordinates to parent coordinates, p is the body origin in the parent frame.
 //   forward   w = R^T wp,  v = R^T (vp + wp x p),  dw = R^T dwp,  dv = R^T (dvp + dwp x p)  (base: 0, 0, 0, -g),
@@ -1275,6 +1282,114 @@ energy_momentum_terms_kernel(const __grid_constant__ DynModel m, const int nv, c
   b[pt] = which == TBD_KINETIC_ENERGY ? T : p[0] * p[0] + p[1] * p[1] + p[2] * p[2];
 }
 
+// A linear joint coupling (include/toppra_b200_dyn.h), passed by value next to the model: body joint positions
+// q_b = E q + o, E (nv x nq) in entries [0, nv) x [0, nq) of E.
+struct DynCoupling {
+  double E[NB][NB], o[NB];
+};
+
+// xb = E x, plus o where `pos` (positions): per body k the nonzero terms E[k][j] x[j] in ascending j, starting from the
+// first term, then + o[k] where o[k] != 0.  __dmul_rn / __dadd_rn keep that order whatever the contraction flags.
+__device__ __forceinline__ void coupling_expand(const DynCoupling &cp, const int nv, const int nq,
+                                                const double *__restrict__ x, const bool pos, double *xb) {
+  for (int k = 0; k < nv; ++k) {
+    double s = 0.0;
+    bool first = true;
+    for (int j = 0; j < nq; ++j) {
+      const double e = cp.E[k][j];
+      if (e == 0.0) continue;
+      const double t = __dmul_rn(e, x[j]);
+      s = first ? t : __dadd_rn(s, t);
+      first = false;
+    }
+    if (pos && cp.o[k] != 0.0) s = __dadd_rn(s, cp.o[k]);
+    xb[k] = s;
+  }
+}
+
+// y = E^T t: per DOF j the nonzero terms E[k][j] t[k] in ascending k, starting from the first term (every column of E
+// has one: load_coupling).
+__device__ __forceinline__ void coupling_reduce(const DynCoupling &cp, const int nv, const int nq, const double *t,
+                                                double *y) {
+  for (int j = 0; j < nq; ++j) {
+    double s = 0.0;
+    bool first = true;
+    for (int k = 0; k < nv; ++k) {
+      const double e = cp.E[k][j];
+      if (e == 0.0) continue;
+      const double u = __dmul_rn(e, t[k]);
+      s = first ? u : __dadd_rn(s, u);
+      first = false;
+    }
+    y[j] = s;
+  }
+}
+
+// tau_q = E^T ID(E q + o, E qd, E qdd): joint_transforms and rnea_pass of rnea_kernel on the expanded state.
+__global__ void __launch_bounds__(THREADS)
+coupled_rnea_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynCoupling cp, const int nv,
+                    const int nq, const int M, const double *__restrict__ q, const double *__restrict__ qd,
+                    const double *__restrict__ qdd, double *__restrict__ tau) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nq;
+  double X[NB][12], st[NB][12], f[NB][6], qb[NB], qdb[NB], qddb[NB], t[NB];
+  coupling_expand(cp, nv, nq, q + o, true, qb);
+  coupling_expand(cp, nv, nq, qd + o, false, qdb);
+  coupling_expand(cp, nv, nq, qdd + o, false, qddb);
+  joint_transforms(m, nv, qb, X);
+  rnea_pass(m, nv, X, qdb, qddb, st, f, t);
+  coupling_reduce(cp, nv, nq, t, tau + o);
+}
+
+// The terms of torque_terms_kernel on the expanded state, each subtracted in body space and then reduced by E^T;
+// c += sign(q') friction on the nq DOFs.
+__global__ void __launch_bounds__(THREADS)
+coupled_torque_terms_kernel(const __grid_constant__ DynModel m, const __grid_constant__ DynCoupling cp, const int nv,
+                            const int nq, const int M, const double *__restrict__ q, const double *__restrict__ qs,
+                            const double *__restrict__ qss, const double *__restrict__ friction,
+                            double *__restrict__ a, double *__restrict__ b, double *__restrict__ c) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nq;
+  double X[NB][12], st[NB][12], f[NB][6], zero[NB], qb[NB], qsb[NB], qssb[NB], tc[NB], t[NB];
+  for (int k = 0; k < nv; ++k) zero[k] = 0.0;
+  coupling_expand(cp, nv, nq, q + o, true, qb);
+  coupling_expand(cp, nv, nq, qs + o, false, qsb);
+  coupling_expand(cp, nv, nq, qss + o, false, qssb);
+  joint_transforms(m, nv, qb, X);
+  rnea_pass(m, nv, X, zero, zero, st, f, tc);
+  rnea_pass(m, nv, X, zero, qsb, st, f, t);
+  for (int k = 0; k < nv; ++k) t[k] = t[k] - tc[k];
+  coupling_reduce(cp, nv, nq, t, a + o);
+  rnea_pass(m, nv, X, qsb, qssb, st, f, t);
+  for (int k = 0; k < nv; ++k) t[k] = t[k] - tc[k];
+  coupling_reduce(cp, nv, nq, t, b + o);
+  coupling_reduce(cp, nv, nq, tc, t);
+  for (int j = 0; j < nq; ++j) {
+    double cj = t[j];
+    if (friction) {
+      const double x = qs[o + j];
+      const double sgn = (double)((0.0 < x) - (x < 0.0));   // torch.sign: 0 at +-0 and NaN
+      cj = __dadd_rn(cj, __dmul_rn(sgn, friction[j]));
+    }
+    c[o + j] = cj;
+  }
+}
+
+// q_b = E q + o and, where given, the rates E qd, E qdd.
+__global__ void __launch_bounds__(THREADS)
+coupling_expand_kernel(const __grid_constant__ DynCoupling cp, const int nv, const int nq, const int M,
+                       const double *__restrict__ q, const double *__restrict__ qd, const double *__restrict__ qdd,
+                       double *__restrict__ q_out, double *__restrict__ qd_out, double *__restrict__ qdd_out) {
+  const long pt = (long)blockIdx.x * THREADS + threadIdx.x;
+  if (pt >= M) return;
+  const size_t o = (size_t)pt * nq, ob = (size_t)pt * nv;
+  coupling_expand(cp, nv, nq, q + o, true, q_out + ob);
+  if (qd) coupling_expand(cp, nv, nq, qd + o, false, qd_out + ob);
+  if (qdd) coupling_expand(cp, nv, nq, qdd + o, false, qdd_out + ob);
+}
+
 // The point count and the number of bodies (or motors): 0, or the TB_ERR_* code (message set).
 int check_sizes(const int nv, const int M, const char *what) {
   if (M <= 0) { set_error("%s: M=%d must be positive", what, M); return TB_ERR_ARG; }
@@ -1534,6 +1649,25 @@ int load_drive(const double *host, const int nv, const double *omega, DynDrive *
       if (!std::isfinite(A[i][nv + j])) { set_error("%s: the inverse of transmission T is not finite", what); return TB_ERR_ARG; }
       d->Tit[j][i] = A[i][nv + j];
     }
+  return 0;
+}
+
+// Validates the packed coupling (TBD_COUPLING_DOUBLES(nv, nq): E row-major, then o) of nv bodies, already checked to
+// be in 1..NB, and copies it into the by-value launch parameter: 0, or the TB_ERR_* code (message set).
+int load_coupling(const double *host, const int nv, const int nq, DynCoupling *cp, const char *what) {
+  if (nq < 1 || nq > nv) { set_error("%s: nq=%d outside 1..nv=%d", what, nq, nv); return TB_ERR_UNSUPPORTED; }
+  *cp = DynCoupling{};
+  for (int j = 0; j < nv * nq + nv; ++j)
+    if (!std::isfinite(host[j])) { set_error("%s: coupling E or o is not finite", what); return TB_ERR_ARG; }
+  for (int k = 0; k < nv; ++k) {
+    for (int j = 0; j < nq; ++j) cp->E[k][j] = host[nq * k + j];
+    cp->o[k] = host[nv * nq + k];
+  }
+  for (int j = 0; j < nq; ++j) {
+    bool moves = false;
+    for (int k = 0; k < nv; ++k) moves = moves || cp->E[k][j] != 0.0;
+    if (!moves) { set_error("%s: DOF %d moves no body (column %d of E is zero)", what, j, j); return TB_ERR_ARG; }
+  }
   return 0;
 }
 
@@ -1863,4 +1997,43 @@ extern "C" int tbd_energy_momentum_terms(const double *model_host, int nv, int w
   DynModel m;
   if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
   return launch(__func__, energy_momentum_terms_kernel, M, stream, m, nv, which, M, q, qs, b);
+}
+
+extern "C" int tbd_coupled_rnea(const double *model_host, int nv, const double *coupling, int nq, int M,
+                                const double *q, const double *qd, const double *qdd, double *tau, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, coupling, q, qd, qdd, tau)) return rc;
+  DynModel m;
+  DynCoupling cp;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_coupling(coupling, nv, nq, &cp, __func__)) return rc;
+  return launch(__func__, coupled_rnea_kernel, M, stream, m, cp, nv, nq, M, q, qd, qdd, tau);
+}
+
+// friction may be null (no friction).
+extern "C" int tbd_coupled_torque_terms(const double *model_host, int nv, const double *coupling, int nq, int M,
+                                        const double *q, const double *qs, const double *qss, const double *friction,
+                                        double *a, double *b, double *c, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, model_host, coupling, q, qs, qss, a, b, c)) return rc;
+  DynModel m;
+  DynCoupling cp;
+  if (const int rc = load_model(model_host, nv, M, &m, __func__)) return rc;
+  if (const int rc = load_coupling(coupling, nv, nq, &cp, __func__)) return rc;
+  return launch(__func__, coupled_torque_terms_kernel, M, stream, m, cp, nv, nq, M, q, qs, qss, friction, a, b, c);
+}
+
+// No model: the expansion needs only the coupling.  qd and qd_out, and qdd and qdd_out, are both given or both NULL.
+extern "C" int tbd_coupling_expand(int nv, const double *coupling, int nq, int M, const double *q, const double *qd,
+                                   const double *qdd, double *q_out, double *qd_out, double *qdd_out, void *stream) {
+  using namespace tb;
+  if (const int rc = nonnull(__func__, coupling, q, q_out)) return rc;
+  if (!qd != !qd_out || !qdd != !qdd_out) {
+    set_error("%s: qd and qd_out (and qdd and qdd_out) must both be given or both be NULL", __func__);
+    return TB_ERR_ARG;
+  }
+  if (const int rc = check_sizes(nv, M, __func__)) return rc;
+  DynCoupling cp;
+  if (const int rc = load_coupling(coupling, nv, nq, &cp, __func__)) return rc;
+  return launch(__func__, coupling_expand_kernel, M, stream, cp, nv, nq, M, q, qd, qdd, q_out, qd_out, qdd_out);
 }

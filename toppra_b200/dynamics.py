@@ -32,7 +32,10 @@ launch (`torque_terms`).  The packed layout the library takes is documented in i
     pc = JointWrenchConstraint.bearing(wrist, axial=F_a, radial=F_r, tilting=M_k)  # bearing and reducer loads
     T, p = model.energy_momentum(q, qd)                       # (M,), (M, 3) kinetic energy and momentum, one launch
     pc = KineticEnergyConstraint(model, E_max)                # the energy of the whole arm in motion
-    pc = MomentumConstraint(model, p_max)                     # its linear momentum"""
+    pc = MomentumConstraint(model, p_max)                     # its linear momentum
+    pal = RigidBodyModel.from_urdf("palletizer.urdf", couple_mimic=True)  # mimic joints coupled: q_b = E q + o
+    lev = pal.with_coupling(E, offset)                        # couplings URDF cannot express (a levelling link)
+    tau = lev(q, qd, qdd)                                     # (M, nq) generalized forces E^T ID(q_b, qd_b, qdd_b)"""
 import ctypes
 import xml.etree.ElementTree as ET
 
@@ -76,10 +79,18 @@ class RigidBodyModel(object):
     coordinates); mass (nv,); com (nv, 3) in the body frame; inertia (nv, 6) = Ixx, Ixy, Ixz, Iyy, Iyz, Izz about the
     centre of mass in the body frame; gravity (3,) in the base frame; base_mass >= 0 and base_com (3,), in base
     coordinates, of the static base itself, which moves no joint and enters only the support wrench
-    (RigidBodyFrame.support_wrench)."""
+    (RigidBodyFrame.support_wrench).
+
+    coupling: None, or (E (nv, nq), o (nv,)) for coupled joints (URDF mimic joints, parallelogram bars, levelling
+    links): the body joint positions are affine in nq <= nv independent path DOFs, q_b = E q + o, so qd_b = E qd and
+    qdd_b = E qdd (include/toppra_b200_dyn.h).  Every method then takes (M, nq) path states; `joint_names`,
+    `effort_limit` and `velocity_limit` are those of the nq DOFs, `body_joint_names` those of the nv moving joints in
+    body order, and the joint torques are the generalized forces E^T ID(q_b, qd_b, qdd_b) on the DOFs.  Kinematic
+    quantities and whole-body sums are those of the tree at the expanded state."""
 
     def __init__(self, parent, joint_type, axis, E, r, mass, com, inertia, gravity=(0.0, 0.0, -9.81), joint_names=None,
-                 effort_limit=None, velocity_limit=None, frames=None, base_mass=0.0, base_com=(0.0, 0.0, 0.0)):
+                 effort_limit=None, velocity_limit=None, frames=None, base_mass=0.0, base_com=(0.0, 0.0, 0.0),
+                 coupling=None, body_joint_names=None):
         parent = np.asarray(parent, dtype=np.float64).reshape(-1)
         nv = parent.shape[0]
         if not 1 <= nv <= MAX_BODIES:
@@ -102,8 +113,15 @@ class RigidBodyModel(object):
         body[:, 21:27] = np.asarray(inertia, dtype=np.float64).reshape(nv, 6)
         self.packed = packed
         self.nv = nv
-        self.joint_names = list(joint_names) if joint_names is not None else ["joint%d" % k for k in range(nv)]
-        inf = np.full(nv, np.inf)
+        self.coupling, self.packed_coupling = _coupling("RigidBodyModel", coupling, nv)
+        self.nq = nq = nv if self.coupling is None else self.coupling[0].shape[1]
+        self.joint_names = list(joint_names) if joint_names is not None else ["joint%d" % k for k in range(nq)]
+        if body_joint_names is not None:
+            self.body_joint_names = list(body_joint_names)
+        else:
+            self.body_joint_names = list(self.joint_names) if self.coupling is None else ["body%d" % k
+                                                                                           for k in range(nv)]
+        inf = np.full(nq, np.inf)
         self.effort_limit = inf.copy() if effort_limit is None else np.asarray(effort_limit, dtype=np.float64)
         self.velocity_limit = inf.copy() if velocity_limit is None else np.asarray(velocity_limit, dtype=np.float64)
         # name -> (body index, R, p): frames rigidly attached to a body (-1 = the base), in that body's coordinates
@@ -113,7 +131,8 @@ class RigidBodyModel(object):
 
     @property
     def dof(self):
-        return self.nv
+        """The number of path DOFs: nq (nv without a coupling)."""
+        return self.nq
 
     @property
     def gravity(self):
@@ -141,14 +160,14 @@ class RigidBodyModel(object):
         return np.concatenate(([self.base_mass], self.base_com))
 
     def torque_limits(self):
-        """(nv, 2) [-effort, effort] per joint, the tau_lim of JointTorqueConstraint (+-inf where the URDF has none)."""
+        """(nq, 2) [-effort, effort] per DOF, the tau_lim of JointTorqueConstraint (+-inf where the URDF has none)."""
         return np.stack([-self.effort_limit, self.effort_limit], axis=1)
 
     def with_payload(self, frame, mass, com, inertia):
         """A new model with a payload rigidly held by `frame` (a frame name or a RigidBodyFrame of this model) folded
         into the frame's body by the parallel-axis theorem: mass > 0, centre of mass com (3,) and rotational inertia
         (6,) = Ixx, Ixy, Ixz, Iyy, Iyz, Izz about it (positive semi-definite), both in the frame's axes.  Joint names,
-        limits, gravity, the frame table and the base's mass and centre of mass are kept."""
+        limits, gravity, the frame table, the base's mass and centre of mass and the coupling are kept."""
         if isinstance(frame, RigidBodyFrame):
             if frame.model is not self:
                 raise ValueError("with_payload: the frame %r belongs to another model" % frame.name)
@@ -177,7 +196,43 @@ class RigidBodyModel(object):
                               bodies[:, 14:17], bodies[:, 17], bodies[:, 18:21], bodies[:, 21:27], self.gravity,
                               joint_names=self.joint_names, effort_limit=self.effort_limit.copy(),
                               velocity_limit=self.velocity_limit.copy(), frames=self.frames, base_mass=self.base_mass,
-                              base_com=self.base_com)
+                              base_com=self.base_com, coupling=self.coupling, body_joint_names=self.body_joint_names)
+
+    def with_coupling(self, E, offset=None, joint_names=None):
+        """A new model whose path DOFs q_new are coupled to this model's DOFs by q = E q_new + offset: E (nq, n_new),
+        offset (nq,) or None (zero).  For couplings URDF cannot express, such as a levelling link at -(q2 + q3) or
+        motor-angle DOFs.  On a coupled model the couplings compose: E_b = E_old E, o_b = E_old offset + o_old.  New DOF
+        j takes the name and the limits of the first old DOF i whose row of E is the unit row e_j (old DOF i is new
+        DOF j), else the name "dof<j>" and no limits; `joint_names` (n_new,) overrides the names."""
+        E = np.asarray(E, dtype=np.float64)
+        if E.ndim != 2 or E.shape[0] != self.nq:
+            raise ValueError("with_coupling: E has shape %s; expected (%d, n_new)" % (E.shape, self.nq))
+        o = np.zeros(self.nq) if offset is None else np.asarray(offset, dtype=np.float64)
+        if o.shape != (self.nq,):
+            raise ValueError("with_coupling: offset has shape %s; expected (%d,)" % (o.shape, self.nq))
+        if not (np.isfinite(E).all() and np.isfinite(o).all()):
+            raise ValueError("with_coupling: E and offset must be finite")
+        n = E.shape[1]
+        names, effort, velocity = ["dof%d" % j for j in range(n)], np.full(n, np.inf), np.full(n, np.inf)
+        for j in range(n):
+            same = [i for i in range(self.nq) if E[i, j] == 1.0 and np.count_nonzero(E[i]) == 1]
+            if same:
+                names[j], effort[j], velocity[j] = (self.joint_names[same[0]], self.effort_limit[same[0]],
+                                                    self.velocity_limit[same[0]])
+        if joint_names is not None:
+            names = list(joint_names)
+            if len(names) != n:
+                raise ValueError("with_coupling: %d joint_names for %d DOFs" % (len(names), n))
+        if self.coupling is None:
+            Eb, ob = E, o
+        else:
+            Eb, ob = self.coupling[0] @ E, self.coupling[0] @ o + self.coupling[1]
+        bodies = self.packed[3:].reshape(self.nv, BODY_DOUBLES)
+        return RigidBodyModel(bodies[:, 0], bodies[:, 1], bodies[:, 2:5], bodies[:, 5:14].reshape(-1, 3, 3),
+                              bodies[:, 14:17], bodies[:, 17], bodies[:, 18:21], bodies[:, 21:27], self.gravity,
+                              joint_names=names, effort_limit=effort, velocity_limit=velocity, frames=self.frames,
+                              base_mass=self.base_mass, base_com=self.base_com, coupling=(Eb, ob),
+                              body_joint_names=self.body_joint_names)
 
     def inertialess_joints(self):
         """Names of the moving joints that move no inertia: the joint's body and all its descendants have zero mass and
@@ -188,14 +243,20 @@ class RigidBodyModel(object):
             par = int(bodies[k, 0])
             if par >= 0 and not empty[k]:
                 empty[par] = False
-        return [self.joint_names[k] for k in range(self.nv) if empty[k]]
+        return [self.body_joint_names[k] for k in range(self.nv) if empty[k]]
+
+    def _refuse_coupled(self, quantity):
+        """ValueError on a coupled model for `quantity`, which needs the mass matrix E^T M E of the DOFs."""
+        if self.coupling is not None:
+            raise ValueError("RigidBodyModel: %s is not supported on a model with coupled joints: the effective mass "
+                             "needs the mass matrix E^T M E of the path DOFs, not the tree's M^-1" % quantity)
 
     # ---- evaluation on the GPU ----------------------------------------------------------------------------------
     def _prepare(self, torch, *xs):
         out = []
         for x in xs:
-            if x.dim() != 2 or x.shape[1] != self.nv:
-                raise ValueError("RigidBodyModel: expected (M, %d) tensors, got %s" % (self.nv, tuple(x.shape)))
+            if x.dim() != 2 or x.shape[1] != self.nq:
+                raise ValueError("RigidBodyModel: expected (M, %d) tensors, got %s" % (self.nq, tuple(x.shape)))
             out.append(x.to(dtype=torch.float64).contiguous())
         if any(x.shape != out[0].shape or x.device != out[0].device for x in out):
             raise ValueError("RigidBodyModel: q, qd, qdd must share shape and device")
@@ -203,19 +264,21 @@ class RigidBodyModel(object):
 
     def __call__(self, q, qd, qdd):
         """Joint torques tau = M(q) qdd + h(q, qd) + g(q).  CUDA tensors (M, nv) -> (M, nv), one tbd_rnea launch on the
-        current stream; numpy (nv,) or (M, nv) -> numpy, through a device round trip."""
+        current stream; numpy (nv,) or (M, nv) -> numpy, through a device round trip.  On a coupled model the
+        generalized forces E^T ID(E q + o, E qd, E qdd) on the DOFs, (M, nq) -> (M, nq): one tbd_coupled_rnea launch."""
         if not _is_cuda(q):
             return _round_trip(self, q, qd, qdd)
-        return _launch(self, "tbd_rnea", (), (q, qd, qdd), [(self.nv,)])
+        return _launch(self, "tbd_rnea", (), (q, qd, qdd), [(self.nq,)])
 
     def torque_terms(self, q, qs, qss, friction=None):
         """The terms of SecondOrderConstraint for CUDA tensors (M, nv), one tbd_torque_terms launch:
         c = ID(q, 0, 0), a = ID(q, 0, qs) - c, b = ID(q, qs, qss) - c, c += sign(qs) * friction (friction (nv,) or
-        None).  Returns (a, b, c)."""
+        None).  Returns (a, b, c).  On a coupled model the same terms on the nq DOFs (each reduced by E^T, friction per
+        DOF): one tbd_coupled_torque_terms launch."""
         fric = None
         if friction is not None and np.any(np.asarray(friction) != 0):
-            fric = np.broadcast_to(np.asarray(friction, dtype=np.float64), (self.nv,)).copy()
-        return _launch(self, "tbd_torque_terms", (), (q, qs, qss), [(self.nv,)] * 3, extra=(fric,))
+            fric = np.broadcast_to(np.asarray(friction, dtype=np.float64), (self.nq,)).copy()
+        return _launch(self, "tbd_torque_terms", (), (q, qs, qss), [(self.nq,)] * 3, extra=(fric,))
 
     def separation(self, points, humans, q, qd, points_per_path=0):
         """Surface separation d and approach speed w of robot points and human spheres at the state (q, qd), for CUDA
@@ -263,7 +326,7 @@ class RigidBodyModel(object):
 
     # ---- URDF ---------------------------------------------------------------------------------------------------
     @classmethod
-    def from_urdf(cls, urdf, locked_joints=None, gravity=(0.0, 0.0, -9.81)):
+    def from_urdf(cls, urdf, locked_joints=None, gravity=(0.0, 0.0, -9.81), couple_mimic=False):
         """Build the model from a URDF file name or XML string (xml.etree only).
 
         revolute / continuous joints become revolute bodies, prismatic ones prismatic; fixed joints and the joints named
@@ -271,10 +334,16 @@ class RigidBodyModel(object):
         by the parallel-axis theorem).  DOF order is depth-first with children in file order; `joint_names` lists it.
         The root link and the links folded into it (e.g. locked wheels) make the static base: `base_mass` and
         `base_com` (base coordinates).  floating, planar and unlocked mimic joints, a missing or ambiguous root and more
-        than 16 moving bodies raise ValueError."""
+        than 16 moving bodies raise ValueError.
+
+        couple_mimic=True makes every unlocked moving mimic joint a moving body coupled to its source joint: its row of
+        the coupling E is `multiplier` (default 1) at the source's DOF, its offset `offset` (default 0).  The DOFs are
+        then the other moving joints, in the same depth-first order (`joint_names`), and the bodies keep that order
+        (`body_joint_names`).  A mimic of an unknown, fixed, locked or mimic joint raises ValueError."""
         text = urdf if urdf.lstrip().startswith("<") else open(urdf).read()
         robot = ET.fromstring(text)
         locked = dict(locked_joints or {})
+        mimics = {}          # mimic joint name -> (source joint name, multiplier, offset)
         links = {}
         for el in robot.findall("link"):
             links[el.get("name")] = el
@@ -291,14 +360,33 @@ class RigidBodyModel(object):
                                  % (name, jtype))
             if jtype not in _JOINT_TYPES and jtype != "fixed":
                 raise ValueError("URDF joint %r: unknown type %r" % (name, jtype))
-            if el.find("mimic") is not None and name not in locked:
-                raise ValueError("URDF joint %r mimics another joint; lock it (locked_joints)" % name)
+            mimic = el.find("mimic")
+            if mimic is not None and name not in locked:
+                if not couple_mimic:
+                    raise ValueError("URDF joint %r mimics another joint; lock it (locked_joints) or pass "
+                                     "couple_mimic=True" % name)
+                if jtype != "fixed":
+                    mimics[name] = (mimic.get("joint"), float(mimic.get("multiplier", 1.0)),
+                                    float(mimic.get("offset", 0.0)))
             parent_of[chi] = name
             joints.append(el)
             children[par].append(el)
         unknown = set(locked) - {j.get("name") for j in joints}
         if unknown:
             raise ValueError("locked_joints names unknown joints: %s" % sorted(unknown))
+        types = {j.get("name"): j.get("type") for j in joints}
+        for name, (src, mult, off) in mimics.items():
+            if src not in types:
+                raise ValueError("URDF joint %r mimics unknown joint %r" % (name, src))
+            if types[src] == "fixed":
+                raise ValueError("URDF joint %r mimics the fixed joint %r" % (name, src))
+            if src in locked:
+                raise ValueError("URDF joint %r mimics the locked joint %r; lock %r too" % (name, src, name))
+            if src in mimics:
+                raise ValueError("URDF joint %r mimics %r, itself a mimic joint: mimic chains are not supported"
+                                 % (name, src))
+            if not (np.isfinite(mult) and np.isfinite(off)):
+                raise ValueError("URDF joint %r: mimic multiplier and offset must be finite" % name)
         roots = [name for name in links if name not in parent_of]
         if len(roots) != 1:
             raise ValueError("URDF needs exactly one root link, found %s" % (roots or "none"))
@@ -374,11 +462,21 @@ class RigidBodyModel(object):
             inertia.append([Ic[0, 0], Ic[0, 1], Ic[0, 2], Ic[1, 1], Ic[1, 2], Ic[2, 2]])
         base_mass = sum(pm for pm, _, _ in parts[-1])
         base_com = sum(pm * pc for pm, pc, _ in parts[-1]) / base_mass if base_mass > 0 else np.zeros(3)
+        names = [b["name"] for b in bodies]
+        dofs = [k for k, n in enumerate(names) if n not in mimics]
+        coupling = None
+        if mimics:
+            col = {names[k]: j for j, k in enumerate(dofs)}
+            E, o = np.zeros((len(bodies), len(dofs))), np.zeros(len(bodies))
+            for k, n in enumerate(names):
+                src, mult, off = mimics.get(n, (n, 1.0, 0.0))
+                E[k, col[src]], o[k] = mult, off
+            coupling = (E, o)
         return cls([b["parent"] for b in bodies], [b["type"] for b in bodies], [b["axis"] for b in bodies],
                    [b["E"] for b in bodies], [b["r"] for b in bodies], mass, com, inertia, gravity,
-                   joint_names=[b["name"] for b in bodies], effort_limit=[b["effort"] for b in bodies],
-                   velocity_limit=[b["velocity"] for b in bodies], frames=frames, base_mass=base_mass,
-                   base_com=base_com)
+                   joint_names=[names[k] for k in dofs], effort_limit=[bodies[k]["effort"] for k in dofs],
+                   velocity_limit=[bodies[k]["velocity"] for k in dofs], frames=frames, base_mass=base_mass,
+                   base_com=base_com, coupling=coupling, body_joint_names=names)
 
 
 class RigidBodyFrame(object):
@@ -404,6 +502,11 @@ class RigidBodyFrame(object):
     @property
     def nv(self):
         return self.model.nv
+
+    @property
+    def dof(self):
+        """The model's number of path DOFs (RigidBodyModel.dof)."""
+        return self.model.dof
 
     def __call__(self, q, qd):
         """Frame velocities.  CUDA tensors (M, nv) -> (M, 6), one tbd_frame_velocity launch on the current stream;
@@ -471,6 +574,7 @@ class RigidBodyFrame(object):
         NaN where M(q) is singular.  CUDA tensors (M, nv) -> (M, 3, 3), one tbd_frame_inverse_inertia launch on the
         current stream; numpy (nv,) -> (3, 3) or (M, nv) -> (M, 3, 3), through a device round trip."""
         self._refuse_world("the inverse inertia is that of the frame origin")
+        self.model._refuse_coupled("the inverse inertia")
         if not _is_cuda(q):
             return _round_trip(self.inverse_inertia, q)
         return _launch(self.model, "tbd_frame_inverse_inertia", (self.packed,), (q,), [(3, 3)])
@@ -480,6 +584,7 @@ class RigidBodyFrame(object):
         (q, qs = q'), m_H = human_mass (> 0, inf allowed): the collision energy E = b s'^2 of
         CollisionEnergyConstraint, for CUDA tensors (M, nv) -> (M,): one tbd_collision_energy_terms launch.  The
         reference frame is ignored."""
+        self.model._refuse_coupled("the collision energy")
         return _launch(self.model, "tbd_collision_energy_terms", (self.packed, float(human_mass)), (q, qs), [()])
 
     def _support_base(self, base):
@@ -508,11 +613,28 @@ class RigidBodyFrame(object):
         return _launch(self.model, "tbd_support_wrench_terms", (self.packed, base), (q, qs, qss), [(6,)] * 3)
 
     def _check_joint_wrench(self):
-        """ValueError where this frame has no joint wrench: a frame on the base or a "world" frame."""
+        """ValueError where this frame has no joint wrench: a frame on the base, a "world" frame, or on a coupled model
+        a joint whose subtree holds some but not all of the bodies one DOF moves.  The mechanism of such a coupling (a
+        bar, a belt) carries force across the joint, which the open tree does not know; every other joint wrench of a
+        coupled model is that of the open tree at the expanded state."""
         if self.body < 0:
             raise ValueError("RigidBodyFrame %r is on the base (body -1), which has no joint; the base's load is the "
                              "support wrench (SupportStabilityConstraint)" % self.name)
         self._refuse_world("the joint wrench is taken about the frame origin")
+        model = self.model
+        if model.coupling is None:
+            return
+        parent = model.packed[3:].reshape(model.nv, BODY_DOUBLES)[:, 0].astype(int)
+        inside = np.zeros(model.nv, dtype=bool)
+        for k in range(model.nv):                               # parents come before their children
+            inside[k] = k == self.body or (parent[k] >= 0 and inside[parent[k]])
+        moved = model.coupling[0] != 0
+        for j in range(model.nq):
+            if moved[inside, j].any() and moved[~inside, j].any():
+                raise ValueError("RigidBodyFrame %r: DOF %r moves bodies on both sides of joint %r, so the coupling "
+                                 "carries force across it; the joint wrench of the open tree is not that of the "
+                                 "coupled mechanism" % (self.name, model.joint_names[j],
+                                                        model.body_joint_names[self.body]))
 
     def joint_wrench(self, q, qd, qdd):
         """The wrench [fx, fy, fz, nx, ny, nz] across the joint of this frame's body: the force and moment the parent
@@ -550,6 +672,9 @@ class Drives(object):
     def __init__(self, model, gear_ratio=None, transmission=None, rotor_inertia=0.0, friction=0.0):
         if not isinstance(model, RigidBodyModel):
             raise ValueError("Drives needs a RigidBodyModel")
+        if model.coupling is not None:
+            raise ValueError("Drives: geared drives of a model with coupled joints are not supported (the motor map "
+                             "would need the reduction E^T inside the drive kernels)")
         nv = model.nv
         if (gear_ratio is None) == (transmission is None):
             raise ValueError("Drives: pass exactly one of gear_ratio (nv,) or transmission (nv, nv)")
@@ -623,20 +748,64 @@ def _round_trip(fn, *xs):
 
 def _launch(model, name, params, inputs, out_shapes, extra=()):
     """One launch of the dyn entry `name` on the current stream; every entry takes (model, nv, *params, M, *inputs,
-    *extra, *outputs, stream).  params: host numpy arrays (passed by pointer) and scalars; inputs: (M, nv) CUDA tensors;
-    extra: host vectors copied to their device, or None for a null pointer; outputs: new float64 tensors (M,) + shape
-    for each of `out_shapes`.  Returns the output, or the tuple of outputs."""
+    *extra, *outputs, stream).  params: host numpy arrays (passed by pointer) and scalars; inputs: (M, nq) CUDA tensors,
+    the position first; extra: host vectors copied to their device, or None for a null pointer; outputs: new float64
+    tensors (M,) + shape for each of `out_shapes`.  Returns the output, or the tuple of outputs.
+
+    On a coupled model tbd_rnea and tbd_torque_terms become their coupled entries (the packed coupling and nq before
+    M); every other entry gets its inputs through one tbd_coupling_expand launch and is called unchanged."""
     torch = _lib.require_cuda()
     inputs = model._prepare(torch, *inputs)
     q = inputs[0]
     extra = [None if x is None else torch.as_tensor(x, device=q.device) for x in extra]
     outs = [torch.empty((q.shape[0],) + tuple(s), dtype=torch.float64, device=q.device) for s in out_shapes]
     host = [ctypes.c_void_p(p.ctypes.data) if isinstance(p, np.ndarray) else p for p in params]
+    lib = _lib_dyn.load()
     with torch.cuda.device(q.device):
-        _lib.check(getattr(_lib_dyn.load(), name)(ctypes.c_void_p(model.packed.ctypes.data), model.nv, *host,
-                                                  q.shape[0], *[_lib.ptr(x) for x in inputs + extra],
-                                                  *[_lib.ptr(o) for o in outs], _lib.stream_ptr()), name)
+        if model.coupling is not None and name in _COUPLED_ENTRIES:
+            name = _COUPLED_ENTRIES[name]
+            host = [ctypes.c_void_p(model.packed_coupling.ctypes.data), model.nq] + host
+        elif model.coupling is not None:
+            inputs = _expand(torch, lib, model, inputs)
+        _lib.check(getattr(lib, name)(ctypes.c_void_p(model.packed.ctypes.data), model.nv, *host, q.shape[0],
+                                      *[_lib.ptr(x) for x in inputs + extra], *[_lib.ptr(o) for o in outs],
+                                      _lib.stream_ptr()), name)
     return outs[0] if len(outs) == 1 else tuple(outs)
+
+
+_COUPLED_ENTRIES = {"tbd_rnea": "tbd_coupled_rnea", "tbd_torque_terms": "tbd_coupled_torque_terms"}
+
+
+def _expand(torch, lib, model, inputs):
+    """The body states (M, nv) of a coupled model's (M, nq) inputs (a position, then up to two rates): q_b = E q + o,
+    E x for the rates, one tbd_coupling_expand launch on the current stream."""
+    M = inputs[0].shape[0]
+    outs = [torch.empty((M, model.nv), dtype=torch.float64, device=inputs[0].device) for _ in inputs]
+    pad = [None] * (3 - len(inputs))
+    _lib.check(lib.tbd_coupling_expand(model.nv, ctypes.c_void_p(model.packed_coupling.ctypes.data), model.nq, M,
+                                       *[_lib.ptr(x) for x in inputs + pad], *[_lib.ptr(o) for o in outs + pad],
+                                       _lib.stream_ptr()), "tbd_coupling_expand")
+    return outs
+
+
+def _coupling(what, coupling, nv):
+    """((E (nv, nq), o (nv,)), packed E row-major then o) of a coupling, or (None, None); ValueError unless
+    1 <= nq <= nv, E and o are finite and every DOF moves a body (no zero column of E)."""
+    if coupling is None:
+        return None, None
+    try:
+        E, o = (np.array(x, dtype=np.float64) for x in coupling)
+    except (TypeError, ValueError):
+        raise ValueError("%s: coupling must be a pair (E (nv, nq), o (nv,))" % what)
+    if E.ndim != 2 or E.shape[0] != nv or not 1 <= E.shape[1] <= nv or o.shape != (nv,):
+        raise ValueError("%s: coupling E has shape %s and o %s; expected (%d, nq) with 1 <= nq <= %d and (%d,)"
+                         % (what, E.shape, o.shape, nv, nv, nv))
+    if not (np.isfinite(E).all() and np.isfinite(o).all()):
+        raise ValueError("%s: coupling E and o must be finite" % what)
+    idle = [j for j in range(E.shape[1]) if not E[:, j].any()]
+    if idle:
+        raise ValueError("%s: DOF(s) %s move no body (zero columns of the coupling E)" % (what, idle))
+    return (E, o), np.ascontiguousarray(np.concatenate((E.reshape(-1), o)))
 
 
 def _inertia3(I6):
