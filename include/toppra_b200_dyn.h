@@ -255,8 +255,8 @@ int tbd_separation_terms(const double *model_host, int nv, const double *points_
  * Per pair, capsule-major then h, the closest pair (t, tau) of the two segments (Ericson, Real-Time Collision
  * Detection 5.1.9), each dot product summed left to right, clamp(x) = x < 0 ? 0 : (x > 1 ? 1 : x) (NaN passes):
  *   d1 = x_b - x_a;  d2 = c1 - c0;  r0 = x_a - c0;  a = d1.d1;  e = d2.d2;  f = d2.r0
- *   a == 0 and e == 0:  t = tau = 0
- *   a == 0:             t = 0;  tau = clamp(f / e)
+ *   a == 0:             tau = 0 where e == 0, else clamp(f / e); the pairs (0, tau) and (1, tau) (below): the ends
+ *                       coincide, every t is a closest pair, and the ends may move apart (frames on different bodies)
  *   otherwise c = d1.r0, and
  *   e == 0:             tau = 0;  t = clamp(-c / a)            (-c: the negation of c)
  *   otherwise b = d1.d2;  denom = a * e - b * b;
@@ -268,9 +268,9 @@ int tbd_separation_terms(const double *model_host, int nv, const double *points_
  *     re-clamp:  tau = (b * t + f) / e;  tau < 0: tau = 0, t = clamp(-c / a);  tau > 1: tau = 1, t = clamp((b - c) / a)
  * then with p = x_a + t * d1, v = v_a + t * (v_b - v_a), h = c0 + tau * d2 (per component) the operations of
  * tbd_separation:  E = h - p;  l = sqrt(E.E);  d = l - r_p - r_h;  w = (E.v) / l, or sqrt(v.v) where l == 0.
- * Parallel segments whose projections overlap have a segment of closest pairs, along which w is affine in t; the rate
- * at which the distance closes is the largest w over that set (Danskin's theorem), so both ends are evaluated and
- * d = the smaller d, w = the larger w of the two.  A capsule with frame a == frame b and a human capsule with
+ * Parallel segments whose projections overlap, and a robot capsule whose ends coincide, have a segment of closest
+ * pairs, along which w is affine in t; the rate at which the distance closes is the largest w over that set (Danskin's
+ * theorem), so both ends are evaluated and d = the smaller d, w = the larger w of the two.  A capsule with frame a == frame b and a human capsule with
  * c0 == c1 give the numbers of tbd_separation (signed zeros aside).
  *   q, qd [M][nv]; d, w [M][P][H].  TB_ERR_UNSUPPORTED for P or H outside 1..16; TB_ERR_ARG for a null pointer, a
  *   radius r_p that is not finite or is negative, NH < 1, points_per_path < 0 or a points_per_path that reads past set

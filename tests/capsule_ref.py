@@ -139,6 +139,7 @@ def capsule_pair_np(xa, va, xb, vb, rp, hc):
     if a == 0.0:
         if e != 0.0:
             tau = _clamp(f / e)
+        pairs = [(0.0, tau), (1.0, tau)]                # the ends coincide: every t is a closest pair
     else:
         c = d1[0] * r0[0] + d1[1] * r0[1] + d1[2] * r0[2]
         if e == 0.0:

@@ -859,7 +859,8 @@ __device__ __forceinline__ double clamp01(const double x) { return x < 0.0 ? 0.0
 // Collision Detection 5.1.9), then separation_pair of p(t) = xa + t (xb - xa), v(t) = va + t (vb - va) and the sphere
 // (c0 + tau (c1 - c0), r_h).  Parallel segments (denom <= TBD_CAPSULE_PARALLEL a e) whose projections overlap on
 // [t_lo, t_hi] have a segment of closest pairs: both ends are evaluated, dd is the smaller and ww the larger (Danskin).
-// Operation order in include/toppra_b200_dyn.h.
+// So does a robot capsule whose ends coincide (a == 0): every t is a closest pair, and where the two ends move apart
+// (frames on different bodies) the speed differs between t = 0 and t = 1.  Operation order in include/toppra_b200_dyn.h.
 __device__ __forceinline__ void capsule_pair(const double *xa, const double *va, const double *xb, const double *vb,
                                              const double rp, const double *hc, double &dd, double &ww) {
   double d1[3], d2[3], r0[3];
@@ -871,6 +872,9 @@ __device__ __forceinline__ void capsule_pair(const double *xa, const double *va,
   bool two = false;
   if (a == 0.0) {
     if (e != 0.0) tau = clamp01(f / e);
+    t2 = 1.0;
+    tau2 = tau;
+    two = true;
   } else {
     const double c = d1[0] * r0[0] + d1[1] * r0[1] + d1[2] * r0[2];
     if (e == 0.0) {
