@@ -247,6 +247,14 @@ int tb_scan_robust_ragged(const double *records, int W, int R, int conic_row0, i
                           const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
                           const int *glen, const double *sd_start, const double *sd_end, int flags, double *K,
                           double *sd, double *u, int *status, int *fail_stage, int *counters, void *stream);
+/* compute_controllable_sets(sdmin, sdmax) of robust problems: tb_scan_robust_ragged with
+ *   sd_end_hi (nullable): [B] upper terminal velocity, K[N] = [sd_end^2, sd_end_hi^2], the convention of tb_scan_ex.
+ * NULL is tb_scan_robust_ragged itself (K[N] = [sd_end^2, sd_end^2]).  Status, fail_stage and the zero rows before a
+ * failed stage as there. */
+int tb_scan_robust_ex(const double *records, int W, int R, int conic_row0, int conic_rows, const double *ellipsoid_host3,
+                      const double *grid, int grid_shared, int B, int G, const int *glen, const double *sd_start,
+                      const double *sd_end, const double *sd_end_hi, int flags, double *K, double *sd, double *u,
+                      int *status, int *fail_stage, int *counters, void *stream);
 int tb_sd_bisect_ragged(const double *x_fast, const double *u_fast, const double *x_slow, const double *u_slow,
                         const double *grid, int grid_shared, int B, int G, const int *glen,
                         const double *desired_duration, double atol, int max_iter, const int *status_in, double *sd,

@@ -59,6 +59,8 @@ _PROTOS = {
                                   _c_ip, ctypes.c_void_p], _int),
     "tb_scan_robust_ragged": ([_c_dp, _int, _int, _int, _int, _c_dp, _c_dp, _int, _int, _int, _c_ip, _c_dp, _c_dp, _int,
                                _c_dp, _c_dp, _c_dp, _c_ip, _c_ip, _c_ip, ctypes.c_void_p], _int),
+    "tb_scan_robust_ex": ([_c_dp, _int, _int, _int, _int, _c_dp, _c_dp, _int, _int, _int, _c_ip, _c_dp, _c_dp, _c_dp,
+                           _int, _c_dp, _c_dp, _c_dp, _c_ip, _c_ip, _c_ip, ctypes.c_void_p], _int),
     "tb_sd_bisect_ragged": ([_c_dp, _c_dp, _c_dp, _c_dp, _c_dp, _int, _int, _int, _c_ip, _c_dp, ctypes.c_double, _int,
                              _c_ip, _c_dp, _c_dp, _c_dp, _c_ip, ctypes.c_void_p], _int),
     "tb_propose_gridpoints": ([_c_dp, _c_dp, _int, _int, _int, _int, ctypes.c_double, _int, ctypes.c_double, _int, _int,

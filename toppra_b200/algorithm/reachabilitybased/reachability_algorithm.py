@@ -61,7 +61,8 @@ class ReachabilityAlgorithm(ParameterizationAlgorithm):
     def compute_reachable_sets(self, sdmin, sdmax):
         """Sets of reachable squared velocities L (N+1, 2) (reference :378-431): the feasible-set pass and the forward
         recursion run as ONE launch of tb_reachable_sets (csrc/tb_scan.cu) — the B = 1 case of
-        `BatchTOPPRA.compute_reachable_sets`.  Rows after a failed stage stay 0 like the reference's."""
+        `BatchTOPPRA.compute_reachable_sets`; robust problems run a feasible-set launch and one launch of
+        tbr_reachable_sets_robust (csrc/tb_reach.cu).  Rows after a failed stage stay 0 like the reference's."""
         assert sdmin <= sdmax and 0 <= sdmin
         X, L, fail_stage = self.solver_wrapper.reachable_sets(sdmin, sdmax)
         self._problem_data.X = X

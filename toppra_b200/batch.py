@@ -32,10 +32,16 @@ def scan_any(records, R, grid, conic, sd_start=None, sd_end=None, sd_end_hi=None
     if conic is None:
         return engine.scan(records, R, grid, sd_start, sd_end, sd_end_hi, backward_only, counters,
                            fast_lower=fast_lower, glen=glen)
-    if sd_end_hi is not None:
-        raise NotImplementedError("robust problems: compute_controllable_sets needs sdmin == sdmax")
+    kw = {} if sd_end_hi is None else {"sd_end_hi": sd_end_hi}   # a velocity range: tb_scan_robust_ex
     return engine.scan_robust(records, R, conic[0], conic[1], conic[2], grid, sd_start, sd_end, backward_only, counters,
-                              **ragged(glen))
+                              **ragged(glen), **kw)
+
+
+def reachable_sets_any(records, R, grid, conic, sdmin=None, sdmax=None, glen=None):
+    """compute_reachable_sets: tb_reachable_sets for purely linear problems, the robust pair of launches otherwise."""
+    if conic is None:
+        return engine.reachable_sets(records, R, grid, sdmin, sdmax, **ragged(glen))
+    return engine.reachable_sets_robust(records, R, conic[0], conic[1], conic[2], grid, sdmin, sdmax, **ragged(glen))
 
 
 def build_records(ctx, constraints, out=None):
@@ -265,11 +271,9 @@ class BatchTOPPRA(object):
         if self.conic is None:
             return engine.scan(self.records, self.R, self.d_grid, s0, s1, sd_end_hi, fast_lower=not self.exact,
                                glen=self.glen, **kw)
-        if sd_end_hi is not None:
-            raise NotImplementedError("robust problems: compute_controllable_sets needs sdmin == sdmax")
         kw.pop("forward_from", None)
-        return engine.scan_robust(self.records, self.R, self.conic[0], self.conic[1], self.conic[2], self.d_grid, s0, s1,
-                                  kw.get("backward_only", False), kw.get("counters", False), **ragged(self.glen))
+        return scan_any(self.records, self.R, self.d_grid, self.conic, s0, s1, sd_end_hi, kw.get("backward_only", False),
+                        kw.get("counters", False), glen=self.glen)
 
     def _vel_tensor(self, v):
         if v is None:
@@ -432,6 +436,9 @@ class BatchTOPPRA(object):
         hi = np.ascontiguousarray(np.broadcast_to(np.asarray(sdmax, dtype=np.float64), (self.B,)))
         assert np.all(lo <= hi) and np.all(0 <= lo)
         same = bool(np.all(lo == hi))
+        if not same and self.conic is not None and self.glen is not None:
+            raise NotImplementedError("robust problems: compute_controllable_sets with sdmin != sdmax runs on common "
+                                      "gridpoints, not on per-path proposed grids (gridpoints=None)")
         s1, s1_hi = engine.as_device(lo, self.device), None if same else engine.as_device(hi, self.device)
         nchunk = self.chunk_size()
         if nchunk >= self.B:
@@ -444,20 +451,23 @@ class BatchTOPPRA(object):
 
     def compute_reachable_sets(self, sdmin, sdmax):
         """Reachable sets L [B, G, 2] of every path (reference compute_reachable_sets, reachability_algorithm.py:378-431)
-        in one launch of tb_reachable_sets (feasible-set pass + forward recursion) per record chunk.
+        in one launch of tb_reachable_sets (feasible-set pass + forward recursion) per record chunk; robust problems in
+        a feasible-set launch and a tbr_reachable_sets_robust launch per chunk (reachable_sets_any), on common
+        gridpoints only.
         Returns (L, X, fail_stage)."""
-        if self.conic is not None:
-            raise NotImplementedError("compute_reachable_sets: linear problems only")
+        if self.conic is not None and self.glen is not None:
+            raise NotImplementedError("robust problems: compute_reachable_sets runs on common gridpoints, not on per-path "
+                                      "proposed grids (gridpoints=None)")
         lo = np.ascontiguousarray(np.broadcast_to(np.asarray(sdmin, dtype=np.float64), (self.B,)))
         hi = np.ascontiguousarray(np.broadcast_to(np.asarray(sdmax, dtype=np.float64), (self.B,)))
         assert np.all(lo <= hi) and np.all(0 <= lo)
         lo, hi = engine.as_device(lo, self.device), engine.as_device(hi, self.device)
         nchunk = self.record_chunk_size()
         if nchunk >= self.B:
-            out = engine.reachable_sets(self._records(), self.R, self.d_grid, lo, hi, **ragged(self.glen))
+            out = reachable_sets_any(self._records(), self.R, self.d_grid, self.conic, lo, hi, self.glen)
         else:
             out = self._chunked(nchunk, self._shapes("L", "X", "fail_stage"), lambda a, b, rec, grid, glen:
-                                engine.reachable_sets(rec, self.R, grid, lo[a:b], hi[a:b], **ragged(glen)))
+                                reachable_sets_any(rec, self.R, grid, self.conic, lo[a:b], hi[a:b], glen))
         return out["L"], out["X"], out["fail_stage"]
 
     def compute_feasible_sets(self):

@@ -8,7 +8,8 @@
 //                             tb_scan_robust_ragged launch: at stage i x is fixed, so the stage problem is the
 //                             u-interval at x, and the fastest pass takes u = uhi(x), the slowest u = ulo(x);
 //   socp_stage_kernel         min g0 u + g1 x over one stage: the feasible x-interval by extreme_x, then the convex
-//                             phi(x) = g1 x + g0 (g0 < 0 ? uhi(x) : ulo(x)) by golden-section search on it.
+//                             phi(x) = g1 x + g0 (g0 < 0 ? uhi(x) : ulo(x)) by golden-section search on it
+//                             (socp_stage_solve, tb_robust_common.cuh).
 //
 // This library is linked against libtoppra_b200.so and uses its error slot (set_error / tb_last_error).  Each library
 // carries its own static CUDA runtime, so launch errors are read here (launch_status).
@@ -128,67 +129,9 @@ socp_stage_kernel(const double *__restrict__ g, const double *__restrict__ ra, c
     if (lane == 0) { a[0] = -2 * delta; b[0] = -1.0; c[0] = xnext[3 * p + 1]; }
     if (lane == 1) { a[0] = 2 * delta; b[0] = 1.0; c[0] = -xnext[3 * p + 2]; }
   }
-  const double nan_d = __longlong_as_double(0x7ff8000000000000LL);
-  const double xl = xbox[2 * p], xh = xbox[2 * p + 1];
-  const double g0 = g[2 * p], g1 = g[2 * p + 1];
-  int n_eval = 0;
-  double xmin = nan_d, xmax = nan_d, xs = nan_d, us = nan_d;
-  const bool feasible = extreme_x<RPL>(-1, xl, xh, a, b, c, cmask, lane, ru, rx, rc, xmin, n_eval, nan_d) &&
-                        extreme_x<RPL>(+1, xl, xh, a, b, c, cmask, lane, ru, rx, rc, xmax, n_eval, nan_d);
-  if (feasible && g0 == 0.0) {
-    // the objective does not depend on u: the x end g1 points to (xmin for g1 == 0), u the middle of the u-interval
-    // there.  An interior-point solver returns some u of that face; which one is solver-dependent.
-    xs = (g1 < 0.0) ? xmax : xmin;
-    double ulo, uhi;
-    if (u_bounds<RPL>(xs, a, b, c, cmask, ru, rx, rc, ulo, uhi)) us = 0.5 * (ulo + uhi);
-    else xs = nan_d;
-  } else if (feasible) {
-    // phi(x) = g1 x + g0 u*(x), u*(x) = uhi(x) (g0 < 0) or ulo(x) (g0 > 0): convex on [xmin, xmax] (uhi is concave and
-    // ulo convex on the convex feasible set).  Golden-section search down to a few-ulp bracket; the best point
-    // evaluated, the two ends included, wins (the first one on ties).
-    const double inf = __longlong_as_double(0x7ff0000000000000LL);
-    const auto phi = [&](const double x, double &u) {
-      double ulo, uhi;
-      const bool ok = u_bounds<RPL>(x, a, b, c, cmask, ru, rx, rc, ulo, uhi);
-      u = (g0 < 0.0) ? uhi : ulo;
-      return ok ? g1 * x + g0 * u : inf;
-    };
-    double ua, ub;
-    const double fa = phi(xmin, ua), fb = phi(xmax, ub);
-    double fbest;
-    if (fa <= fb) { xs = xmin; us = ua; fbest = fa; } else { xs = xmax; us = ub; fbest = fb; }
-    const double invphi = 0.6180339887498949;
-    double lo = xmin, hi = xmax;
-    double x1 = hi - invphi * (hi - lo), x2 = lo + invphi * (hi - lo);
-    double u1, u2;
-    double f1 = phi(x1, u1), f2 = phi(x2, u2);
-    if (f1 < fbest) { xs = x1; us = u1; fbest = f1; }
-    if (f2 < fbest) { xs = x2; us = u2; fbest = f2; }
-    for (int it = 0; it < 200; ++it) {
-      if (!(hi - lo > 2.3e-16 * (fabs(hi) + fabs(lo)) + 1e-300)) break;
-      if (f1 <= f2) {
-        hi = x2; x2 = x1; f2 = f1; u2 = u1;
-        x1 = hi - invphi * (hi - lo);
-        f1 = phi(x1, u1);
-        if (f1 < fbest) { xs = x1; us = u1; fbest = f1; }
-      } else {
-        lo = x1; x1 = x2; f1 = f2; u1 = u2;
-        x2 = lo + invphi * (hi - lo);
-        f2 = phi(x2, u2);
-        if (f2 < fbest) { xs = x2; us = u2; fbest = f2; }
-      }
-    }
-    if (!(fbest < inf)) { xs = nan_d; us = nan_d; }
-  }
+  double us, xs;
+  socp_stage_solve<RPL>(g[2 * p], g[2 * p + 1], xbox[2 * p], xbox[2 * p + 1], a, b, c, cmask, lane, ru, rx, rc, us, xs);
   if (lane == 0) { out[2 * p] = us; out[2 * p + 1] = xs; }
-}
-
-// Checks shared by both entries: 0, or the TB_ERR_* code (message set).
-int check_conic(const int R, const int conic_row0, const int conic_rows, const double *ell, const char *what) {
-  if (R > MAX_ROWS) { set_error("%s: R=%d > %d rows", what, R, MAX_ROWS); return TB_ERR_UNSUPPORTED; }
-  if (conic_row0 < 0 || conic_rows < 0 || conic_row0 + conic_rows > R) { set_error("%s: bad conic row range", what); return TB_ERR_ARG; }
-  if (!(ell[0] >= 0) || !(ell[1] >= 0) || !(ell[2] >= 0)) { set_error("%s: negative ellipsoid axis", what); return TB_ERR_ARG; }
-  return 0;
 }
 
 }  // namespace

@@ -29,7 +29,8 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
                    const int grid_shared, const int B, const int G, const double *__restrict__ sd_start,
                    const double *__restrict__ sd_end, const int flags, double *__restrict__ Kout,
                    double *__restrict__ sdout, double *__restrict__ uout, int *__restrict__ status,
-                   int *__restrict__ fail_stage, int *__restrict__ counters, const int *__restrict__ glen) {
+                   int *__restrict__ fail_stage, int *__restrict__ counters, const int *__restrict__ glen,
+                   const double *__restrict__ sd_end_hi /* last: the other parameters keep their offsets */) {
   const int lane = threadIdx.x & 31;
   const long path = warp_path();
   if (path >= B) return;
@@ -83,8 +84,9 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
     return;
   }
   const double sde = sd_end ? sd_end[path] : 0.0;
+  const double sdeh = sd_end_hi ? sd_end_hi[path] : sde;   // K[N] = [sd_end^2, sd_end_hi^2]
   const double sds = sd_start ? sd_start[path] : 0.0;
-  double kn0 = sde * sde, kn1 = sde * sde;
+  double kn0 = sde * sde, kn1 = sdeh * sdeh;
   if (lane == 0) { Kp[2 * N] = kn0; Kp[2 * N + 1] = kn1; }
   int st = TB_STATUS_OK, fstage = -1;
   for (int i = N - 1; i >= 0; --i) {
@@ -187,10 +189,11 @@ scan_robust_kernel(const double *__restrict__ records, const int W, const int R,
 }  // namespace
 }  // namespace tb
 
-extern "C" int tb_scan_robust_ragged(const double *records, int W, int R, int conic_row0, int conic_rows,
-                                     const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
-                                     const int *glen, const double *sd_start, const double *sd_end, int flags, double *K,
-                                     double *sd, double *u, int *status, int *fail_stage, int *counters, void *stream) {
+extern "C" int tb_scan_robust_ex(const double *records, int W, int R, int conic_row0, int conic_rows,
+                                 const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
+                                 const int *glen, const double *sd_start, const double *sd_end, const double *sd_end_hi,
+                                 int flags, double *K, double *sd, double *u, int *status, int *fail_stage, int *counters,
+                                 void *stream) {
   using namespace tb;
   if (!records || !grid || !ellipsoid_host3 || !K || !status || B <= 0 || G <= 0 || R < 0) {
     set_error("tb_scan_robust: bad argument");
@@ -206,16 +209,25 @@ extern "C" int tb_scan_robust_ragged(const double *records, int W, int R, int co
   const double ru = ellipsoid_host3[0], rx = ellipsoid_host3[1], rc = ellipsoid_host3[2];
   with_rows_per_lane(R + 2, [&](auto rpl) {
     scan_robust_kernel<rpl.value><<<B, 32, 0, (cudaStream_t)stream>>>(records, W, R, conic_row0, conic_rows, ru, rx, rc,
-                                                                      grid, grid_shared, B, G, sd_start, sd_end, flags,
-                                                                      K, sd, u, status, fail_stage, counters, glen);
+                                                                      grid, grid_shared, B, G, sd_start, sd_end,
+                                                                      flags, K, sd, u, status, fail_stage, counters,
+                                                                      glen, sd_end_hi);
   });
   return check_launch("tb_scan_robust");
+}
+
+extern "C" int tb_scan_robust_ragged(const double *records, int W, int R, int conic_row0, int conic_rows,
+                                     const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
+                                     const int *glen, const double *sd_start, const double *sd_end, int flags, double *K,
+                                     double *sd, double *u, int *status, int *fail_stage, int *counters, void *stream) {
+  return tb_scan_robust_ex(records, W, R, conic_row0, conic_rows, ellipsoid_host3, grid, grid_shared, B, G, glen,
+                           sd_start, sd_end, nullptr, flags, K, sd, u, status, fail_stage, counters, stream);
 }
 
 extern "C" int tb_scan_robust(const double *records, int W, int R, int conic_row0, int conic_rows,
                               const double *ellipsoid_host3, const double *grid, int grid_shared, int B, int G,
                               const double *sd_start, const double *sd_end, int flags, double *K, double *sd, double *u,
                               int *status, int *fail_stage, int *counters, void *stream) {
-  return tb_scan_robust_ragged(records, W, R, conic_row0, conic_rows, ellipsoid_host3, grid, grid_shared, B, G, nullptr,
-                               sd_start, sd_end, flags, K, sd, u, status, fail_stage, counters, stream);
+  return tb_scan_robust_ex(records, W, R, conic_row0, conic_rows, ellipsoid_host3, grid, grid_shared, B, G, nullptr,
+                           sd_start, sd_end, nullptr, flags, K, sd, u, status, fail_stage, counters, stream);
 }

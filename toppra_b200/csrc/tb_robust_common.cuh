@@ -10,6 +10,8 @@
 //     so the feasible u-interval [ulo(x), uhi(x)] is a max / min over the lanes (redux.sync reductions);
 //   * the feasible x form an interval (the feasible set is convex), w(x) = uhi(x) - ulo(x) is concave: max x / min x
 //     are found by a bracketed secant/bisection on w(x) >= 0 (extreme_x).
+//   * min g0 u + g1 x over one stage: the feasible x-interval, then golden-section search on a convex phi(x)
+//     (socp_stage_solve, shared by the stage solves and the reachable sets of the companion libraries).
 // Lane `lane` holds rows lane + 32 s, s < RPL; rows 0 and 1 are the x_next rows, the records' rows start at row 2.
 #pragma once
 #include "tb_common.cuh"
@@ -189,6 +191,77 @@ __device__ __forceinline__ void rload_rows(const double *__restrict__ rec, const
       a[s] = 0.0; b[s] = 0.0; c[s] = -1.0; cmask[s] = 0u;
     }
   }
+}
+
+// min g0 u + g1 x over one stage whose rows (x_next rows included) the warp holds, on xl <= x <= xh: the feasible
+// x-interval [xmin, xmax] by extreme_x, then (g0 != 0) the convex phi(x) by golden-section search on it.  us / xs out,
+// NaN NaN when infeasible.
+template <int RPL>
+__device__ __forceinline__ void socp_stage_solve(const double g0, const double g1, const double xl, const double xh,
+                                                 const double (&a)[RPL], const double (&b)[RPL],
+                                                 const double (&c)[RPL], const unsigned (&cmask)[RPL], const int lane,
+                                                 const double ru, const double rx, const double rc, double &us,
+                                                 double &xs) {
+  const double nan_d = __longlong_as_double(0x7ff8000000000000LL);
+  int n_eval = 0;
+  double xmin = nan_d, xmax = nan_d;
+  xs = nan_d;
+  us = nan_d;
+  const bool feasible = extreme_x<RPL>(-1, xl, xh, a, b, c, cmask, lane, ru, rx, rc, xmin, n_eval, nan_d) &&
+                        extreme_x<RPL>(+1, xl, xh, a, b, c, cmask, lane, ru, rx, rc, xmax, n_eval, nan_d);
+  if (feasible && g0 == 0.0) {
+    // the objective does not depend on u: the x end g1 points to (xmin for g1 == 0), u the middle of the u-interval
+    // there.  An interior-point solver returns some u of that face; which one is solver-dependent.
+    xs = (g1 < 0.0) ? xmax : xmin;
+    double ulo, uhi;
+    if (u_bounds<RPL>(xs, a, b, c, cmask, ru, rx, rc, ulo, uhi)) us = 0.5 * (ulo + uhi);
+    else xs = nan_d;
+  } else if (feasible) {
+    // phi(x) = g1 x + g0 u*(x), u*(x) = uhi(x) (g0 < 0) or ulo(x) (g0 > 0): convex on [xmin, xmax] (uhi is concave and
+    // ulo convex on the convex feasible set).  Golden-section search down to a few-ulp bracket; the best point
+    // evaluated, the two ends included, wins (the first one on ties).
+    const double inf = __longlong_as_double(0x7ff0000000000000LL);
+    const auto phi = [&](const double x, double &u) {
+      double ulo, uhi;
+      const bool ok = u_bounds<RPL>(x, a, b, c, cmask, ru, rx, rc, ulo, uhi);
+      u = (g0 < 0.0) ? uhi : ulo;
+      return ok ? g1 * x + g0 * u : inf;
+    };
+    double ua, ub;
+    const double fa = phi(xmin, ua), fb = phi(xmax, ub);
+    double fbest;
+    if (fa <= fb) { xs = xmin; us = ua; fbest = fa; } else { xs = xmax; us = ub; fbest = fb; }
+    const double invphi = 0.6180339887498949;
+    double lo = xmin, hi = xmax;
+    double x1 = hi - invphi * (hi - lo), x2 = lo + invphi * (hi - lo);
+    double u1, u2;
+    double f1 = phi(x1, u1), f2 = phi(x2, u2);
+    if (f1 < fbest) { xs = x1; us = u1; fbest = f1; }
+    if (f2 < fbest) { xs = x2; us = u2; fbest = f2; }
+    for (int it = 0; it < 200; ++it) {
+      if (!(hi - lo > 2.3e-16 * (fabs(hi) + fabs(lo)) + 1e-300)) break;
+      if (f1 <= f2) {
+        hi = x2; x2 = x1; f2 = f1; u2 = u1;
+        x1 = hi - invphi * (hi - lo);
+        f1 = phi(x1, u1);
+        if (f1 < fbest) { xs = x1; us = u1; fbest = f1; }
+      } else {
+        lo = x1; x1 = x2; f1 = f2; u1 = u2;
+        x2 = lo + invphi * (hi - lo);
+        f2 = phi(x2, u2);
+        if (f2 < fbest) { xs = x2; us = u2; fbest = f2; }
+      }
+    }
+    if (!(fbest < inf)) { xs = nan_d; us = nan_d; }
+  }
+}
+
+// Host checks of the robust libraries' entries: 0, or the TB_ERR_* code (message set).
+inline int check_conic(const int R, const int conic_row0, const int conic_rows, const double *ell, const char *what) {
+  if (R > MAX_ROWS) { set_error("%s: R=%d > %d rows", what, R, MAX_ROWS); return TB_ERR_UNSUPPORTED; }
+  if (conic_row0 < 0 || conic_rows < 0 || conic_row0 + conic_rows > R) { set_error("%s: bad conic row range", what); return TB_ERR_ARG; }
+  if (!(ell[0] >= 0) || !(ell[1] >= 0) || !(ell[2] >= 0)) { set_error("%s: negative ellipsoid axis", what); return TB_ERR_ARG; }
+  return 0;
 }
 
 }  // namespace

@@ -6,7 +6,7 @@ import ctypes
 
 import numpy as np
 
-from . import _lib, _lib_poly, _lib_robust
+from . import _lib, _lib_poly, _lib_reach, _lib_robust
 
 BC_KINDS = {"not-a-knot": 0, "clamped": 1, "natural": 2, "periodic": 3}
 
@@ -421,9 +421,10 @@ def scan_velacc(ppoly, breaks, grid, alim, interp, xbound, sd_start=None, sd_end
 
 
 def scan_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, sd_start=None, sd_end=None, backward_only=False,
-                counters=False, feasible_sets=False, glen=None):
+                counters=False, feasible_sets=False, glen=None, sd_end_hi=None):
     """K2r: like scan() with rows [conic_row0, conic_row0+conic_rows) robustified by the ellipsoid (ru, rx, rc).
-    glen: optional int32 [B] gridpoints per path (ragged batch, tb_scan_robust_ragged)."""
+    glen: optional int32 [B] gridpoints per path (ragged batch, tb_scan_robust_ragged).  sd_end_hi: optional [B] upper
+    terminal velocity, K[N] = [sd_end^2, sd_end_hi^2] (compute_controllable_sets(sdmin, sdmax), tb_scan_robust_ex)."""
     torch = torch_mod()
     B, G, W = records.shape
     dev = records.device
@@ -434,19 +435,25 @@ def scan_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, sd_start=No
     lib = _lib.load()
     args = (_lib.ptr(records), W, int(R), int(conic_row0), int(conic_rows), ctypes.c_void_p(ell.ctypes.data),
             _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G)
-    rest = (_lib.ptr(sd_start), _lib.ptr(sd_end), 2 if feasible_sets else (1 if backward_only else 0),
+    rest = (2 if feasible_sets else (1 if backward_only else 0),
             _lib.ptr(out["K"]), _lib.ptr(out["sd"]), _lib.ptr(u_arg), _lib.ptr(out["status"]),
             _lib.ptr(out["fail_stage"]), _lib.ptr(out.get("counters")), _lib.stream_ptr())
+    ends = (_lib.ptr(sd_start), _lib.ptr(sd_end))
     if glen is not None:
         check_grid(grid, B, G)
         check_glen(glen, B, grid)
-        with torch.cuda.device(dev):
-            rc = lib.tb_scan_robust_ragged(*args, _lib.ptr(glen), *rest)
-        _lib.check(rc, "tb_scan_robust_ragged")
-        return out
+    check_path_vector(sd_end_hi, B, "sd_end_hi")
     with torch.cuda.device(dev):
-        rc = lib.tb_scan_robust(*args, *rest)
-    _lib.check(rc, "tb_scan_robust")
+        if sd_end_hi is not None:
+            name = "tb_scan_robust_ex"
+            rc = lib.tb_scan_robust_ex(*args, _lib.ptr(glen), *ends, _lib.ptr(sd_end_hi), *rest)
+        elif glen is not None:
+            name = "tb_scan_robust_ragged"
+            rc = lib.tb_scan_robust_ragged(*args, _lib.ptr(glen), *ends, *rest)
+        else:
+            name = "tb_scan_robust"
+            rc = lib.tb_scan_robust(*args, *ends, *rest)
+    _lib.check(rc, name)
     return out
 
 
@@ -550,6 +557,30 @@ def reachable_sets(records, R, grid, sdmin=None, sdmax=None, glen=None):
         else:
             rc = lib.tb_reachable_sets_ragged(*args, _lib.ptr(glen), *rest)
     _lib.check(rc, "tb_reachable_sets")
+    return dict(X=X, L=L, fail_stage=fs)
+
+
+def reachable_sets_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, sdmin=None, sdmax=None, glen=None):
+    """compute_reachable_sets of robust problems: the feasible sets X of one tb_scan_robust[_ragged]
+    (TB_SCAN_FEASIBLE_SETS) launch, then the forward recursion in one tbr_reachable_sets_robust launch.  Same arguments
+    and result as reachable_sets(): dict(X [B,G,2], L [B,G,2], fail_stage [B] int32)."""
+    torch = torch_mod()
+    B, G, W = records.shape
+    dev = records.device
+    check_grid(grid, B, G)
+    check_glen(glen, B, grid)
+    for t, what in ((sdmin, "sdmin"), (sdmax, "sdmax")):
+        check_path_vector(t, B, what)
+    X = scan_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, feasible_sets=True, glen=glen)["K"]
+    ell = np.ascontiguousarray(ellipsoid, dtype=np.float64)
+    L = torch.empty((B, G, 2), dtype=torch.float64, device=dev)
+    fs = torch.empty((B,), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib_reach.load().tbr_reachable_sets_robust(
+            _lib.ptr(records), W, int(R), int(conic_row0), int(conic_rows), ctypes.c_void_p(ell.ctypes.data),
+            _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G, _lib.ptr(glen), _lib.ptr(X), _lib.ptr(sdmin),
+            _lib.ptr(sdmax), _lib.ptr(L), _lib.ptr(fs), _lib.stream_ptr())
+    _lib.check(rc, "tbr_reachable_sets_robust")
     return dict(X=X, L=L, fail_stage=fs)
 
 

@@ -218,9 +218,11 @@ class B200SolverWrapper(SolverWrapper):
         return out["K"][0].cpu().numpy(), int(out["status"][0].item())
 
     def reachable_sets(self, sdmin, sdmax):
-        """(X, L, fail_stage) of compute_reachable_sets: one launch (tb_reachable_sets)."""
-        self._no_conic("compute_reachable_sets")
-        out = engine.reachable_sets(self.records, self.R, self.ctx.d_grid, self._scalar(sdmin), self._scalar(sdmax))
+        """(X, L, fail_stage) of compute_reachable_sets: one launch (tb_reachable_sets); robust problems a feasible-set
+        launch and a tbr_reachable_sets_robust launch."""
+        from ..batch import reachable_sets_any
+        out = reachable_sets_any(self.records, self.R, self.ctx.d_grid, self.conic, self._scalar(sdmin),
+                                 self._scalar(sdmax))
         return out["X"][0].cpu().numpy(), out["L"][0].cpu().numpy(), int(out["fail_stage"][0].item())
 
     def feasible_sets(self):
