@@ -10,15 +10,42 @@ from .exceptions import BadInputVelocities
 from .interpolator import BatchSplineInterpolator
 
 
+class Cones(object):
+    """The robust constraints of a problem that the entries for one robust constraint cannot take: spans
+    [(row0, nrows, ellipsoid)] of every robust constraint, R and whether a linear constraint has a ubound (the records then
+    carry the u-bound pair).  table() is the cone table of libtoppra_b200_cones.so."""
+
+    def __init__(self, spans, R, ubound):
+        self.spans = spans
+        self.R = int(R)
+        self.ubound = bool(ubound)
+
+    def table(self):
+        """[R, 4]: (robust flag, ru, rx, rc) per row."""
+        t = np.zeros((self.R, 4))
+        for row0, n, ell in self.spans:
+            t[row0:row0 + n, 0] = 1.0
+            t[row0:row0 + n, 1:] = ell
+        return t
+
+
 def conic_info(ctx, constraints):
-    """(row0, nrows, ellipsoid) of the robust constraint of the list, or None."""
-    row0 = 0
+    """How the problem's robust constraints reach the kernels; this choice is the one route of every robust call.
+    None: no robust constraint.  (row0, nrows, ellipsoid): exactly one robust constraint and no ubound, the entries of
+    libtoppra_b200.so, _robust.so and _reach.so (tb_scan_robust*, tbr_*).  A Cones: anything else, the tbc_* entries of
+    libtoppra_b200_cones.so."""
+    row0, spans = 0, []
     for c in constraints:
         n = c.num_rows(ctx)
         if c.get_constraint_type() == ConstraintType.CanonicalConic:
-            return row0, n, c.ellipsoid()
+            spans.append((row0, n, c.ellipsoid()))
         row0 += n
-    return None
+    if not spans:
+        return None
+    ubound = any(getattr(c, "has_ubound", lambda _ctx: False)(ctx) for c in constraints)
+    if len(spans) == 1 and not ubound:
+        return spans[0]
+    return Cones(spans, row0, ubound)
 
 
 def ragged(glen):
@@ -28,10 +55,13 @@ def ragged(glen):
 
 def scan_any(records, R, grid, conic, sd_start=None, sd_end=None, sd_end_hi=None, backward_only=False,
              counters=False, fast_lower=False, glen=None):
-    """K2 for purely linear problems, K2r when a robust constraint is present."""
+    """K2 for purely linear problems, K2r when a robust constraint is present (tbc_scan for a Cones)."""
     if conic is None:
         return engine.scan(records, R, grid, sd_start, sd_end, sd_end_hi, backward_only, counters,
                            fast_lower=fast_lower, glen=glen)
+    if isinstance(conic, Cones):
+        return engine.scan_cones(records, R, conic.table(), grid, sd_start, sd_end, backward_only, counters,
+                                 glen=glen, sd_end_hi=sd_end_hi)
     kw = {} if sd_end_hi is None else {"sd_end_hi": sd_end_hi}   # a velocity range: tb_scan_robust_ex
     return engine.scan_robust(records, R, conic[0], conic[1], conic[2], grid, sd_start, sd_end, backward_only, counters,
                               **ragged(glen), **kw)
@@ -41,6 +71,8 @@ def reachable_sets_any(records, R, grid, conic, sdmin=None, sdmax=None, glen=Non
     """compute_reachable_sets: tb_reachable_sets for purely linear problems, the robust pair of launches otherwise."""
     if conic is None:
         return engine.reachable_sets(records, R, grid, sdmin, sdmax, **ragged(glen))
+    if isinstance(conic, Cones):
+        return engine.reachable_sets_cones(records, R, conic.table(), grid, sdmin, sdmax, glen=glen)
     return engine.reachable_sets_robust(records, R, conic[0], conic[1], conic[2], grid, sdmin, sdmax, **ragged(glen))
 
 
@@ -48,17 +80,20 @@ def build_records(ctx, constraints, out=None):
     """Stage records [B, G, W] for a list of CanonicalLinear constraints (= seidelWrapper.__init__,
     cy_seidel_solverwrapper.pyx:425-531).  Returns (records, R).  `out`: optional preallocated buffer whose first
     ctx.B records are (re)used (chunked solves)."""
-    conic = [c for c in constraints if c.get_constraint_type() == ConstraintType.CanonicalConic]
-    if len(conic) > 1:
-        raise NotImplementedError("toppra_b200: at most one robust (conic) constraint per problem")
     for c in constraints:
         if c.get_constraint_type() not in (ConstraintType.CanonicalLinear, ConstraintType.CanonicalConic):
             raise NotImplementedError("constraint type %s cannot be turned into stage rows" % c.get_constraint_type())
+        if c.get_constraint_type() == ConstraintType.CanonicalConic:
+            base = getattr(c, "base_constraint", None)
+            if base is None or not hasattr(c, "ellipsoid"):
+                raise NotImplementedError("toppra_b200: the only robust (conic) constraint is RobustLinearConstraint; "
+                                          "got %s" % type(c).__name__)
+            if getattr(base, "has_ubound", lambda _ctx: False)(ctx):
+                # ecosWrapper drops the ubound of a robustified base constraint (it reads ubound only from linear ones)
+                raise NotImplementedError("toppra_b200: a RobustLinearConstraint whose base constraint has a ubound")
     rows = [c.num_rows(ctx) for c in constraints]
     R = int(sum(rows))
     ubound = any(getattr(c, "has_ubound", lambda _ctx: False)(ctx) for c in constraints)
-    if ubound and conic:
-        raise NotImplementedError("toppra_b200: a constraint with a ubound next to a robust (conic) constraint")
     if out is not None:
         records = out[:ctx.B]
     else:
@@ -475,8 +510,7 @@ class BatchTOPPRA(object):
         per record chunk."""
         def solve(lo, hi, rec, grid, glen):
             if self.conic is not None:
-                return engine.scan_robust(rec, self.R, self.conic[0], self.conic[1], self.conic[2], grid,
-                                          feasible_sets=True, **ragged(glen))
+                return feasible_sets_robust(rec, self.R, grid, self.conic, glen)
             return dict(K=engine.feasible_sets(rec, self.R, grid, **ragged(glen)))
 
         nchunk = self.record_chunk_size()
@@ -532,15 +566,37 @@ def _rows(t, lo, hi):
 
 
 def sd_passes_robust(records, R, conic, grid, sd_start, sd_end, glen=None):
-    """TOPPRAsd's fastest and slowest pass of robust problems: the conic backward pass once (tb_scan_robust, backward
-    only), then both forward passes in one tbr_sd_forward_robust launch.  Returns (fast, slow) in the form of
-    engine.scan(..., sd_forward=...): K, sd (= x = sd^2), u, status, fail_stage (K / status / fail_stage in `fast`)."""
-    back = engine.scan_robust(records, R, conic[0], conic[1], conic[2], grid, None, sd_end, backward_only=True,
-                              **ragged(glen))
-    fwd = engine.sd_forward_robust(records, R, conic[0], conic[1], conic[2], grid, back["K"], back["status"], sd_start,
-                                   **ragged(glen))
+    """TOPPRAsd's fastest and slowest pass of robust problems: the conic backward pass once (tb_scan_robust or tbc_scan,
+    backward only), then both forward passes in one tbr_sd_forward_robust or tbc_sd_forward launch.  Returns (fast, slow)
+    in the form of engine.scan(..., sd_forward=...): K, sd (= x = sd^2), u, status, fail_stage (K / status / fail_stage
+    in `fast`)."""
+    if isinstance(conic, Cones):
+        table = conic.table()
+        back = engine.scan_cones(records, R, table, grid, None, sd_end, backward_only=True, glen=glen)
+        fwd = engine.sd_forward_cones(records, R, table, grid, back["K"], back["status"], sd_start, glen=glen)
+    else:
+        back = engine.scan_robust(records, R, conic[0], conic[1], conic[2], grid, None, sd_end, backward_only=True,
+                                  **ragged(glen))
+        fwd = engine.sd_forward_robust(records, R, conic[0], conic[1], conic[2], grid, back["K"], back["status"],
+                                       sd_start, **ragged(glen))
     fast = dict(K=back["K"], sd=fwd["x_fast"], u=fwd["u_fast"], status=fwd["status"], fail_stage=fwd["fail_stage"])
     return fast, dict(sd=fwd["x_slow"], u=fwd["u_slow"])
+
+
+def feasible_sets_robust(records, R, grid, conic, glen=None):
+    """compute_feasible_sets of robust problems: one tb_scan_robust or tbc_scan launch (TB_SCAN_FEASIBLE_SETS).
+    Returns the scan's result dict; K holds the feasible sets."""
+    if isinstance(conic, Cones):
+        return engine.scan_cones(records, R, conic.table(), grid, feasible_sets=True, glen=glen)
+    return engine.scan_robust(records, R, conic[0], conic[1], conic[2], grid, feasible_sets=True, **ragged(glen))
+
+
+def socp_stage_robust(g, a, b, c, conic, xbox, xnext=None, ubox=None):
+    """One batch of robust stage problems (solve_stagewise_optim): tbr_socp_stage_batch, or tbc_socp_stage_batch with
+    the u box ubox [B, 2] for a Cones."""
+    if isinstance(conic, Cones):
+        return engine.socp_stage_batch_cones(g, a, b, c, conic.table(), xbox, xnext, ubox)
+    return engine.socp_stage_batch(g, a, b, c, conic[0], conic[1], conic[2], xbox, xnext)
 
 
 def solve_batch(ss_waypoints, waypoints, gridpoints, vlim, alim, sd_start=0.0, sd_end=0.0,

@@ -6,7 +6,7 @@ import ctypes
 
 import numpy as np
 
-from . import _lib, _lib_poly, _lib_reach, _lib_robust
+from . import _lib, _lib_cones, _lib_poly, _lib_reach, _lib_robust
 
 BC_KINDS = {"not-a-knot": 0, "clamped": 1, "natural": 2, "periodic": 3}
 
@@ -581,6 +581,115 @@ def reachable_sets_robust(records, R, conic_row0, conic_rows, ellipsoid, grid, s
             _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G, _lib.ptr(glen), _lib.ptr(X), _lib.ptr(sdmin),
             _lib.ptr(sdmax), _lib.ptr(L), _lib.ptr(fs), _lib.stream_ptr())
     _lib.check(rc, "tbr_reachable_sets_robust")
+    return dict(X=X, L=L, fail_stage=fs)
+
+
+def _cone_table(cones, R):
+    """The host cone table [R][4] = (robust flag 0/1, ru, rx, rc) per row, C-contiguous float64."""
+    t = np.ascontiguousarray(cones, dtype=np.float64)
+    if t.shape != (int(R), 4):
+        raise ValueError("cone table must have shape (%d, 4); got %s" % (int(R), t.shape))
+    return t
+
+
+def scan_cones(records, R, cones, grid, sd_start=None, sd_end=None, backward_only=False, counters=False,
+               feasible_sets=False, glen=None, sd_end_hi=None):
+    """scan_robust() on the cone table cones [R, 4] (tbc_scan): every row its own robust flag and axes; records with a
+    u-bound pair (W >= 3R+4) add the u box (TB_SCAN_UBOUND).  Same arguments otherwise, same result."""
+    torch = torch_mod()
+    B, G, W = records.shape
+    dev = records.device
+    backward_only = backward_only or feasible_sets
+    out, u_arg = _scan_outputs(B, G, dev, backward_only, counters)
+    table = _cone_table(cones, R)
+    if glen is not None:
+        check_grid(grid, B, G)
+        check_glen(glen, B, grid)
+    check_path_vector(sd_end_hi, B, "sd_end_hi")
+    flags = ((2 if feasible_sets else (1 if backward_only else 0))
+             | (SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0))
+    with torch.cuda.device(dev):
+        rc = _lib_cones.load().tbc_scan(
+            _lib.ptr(records), W, int(R), ctypes.c_void_p(table.ctypes.data), _lib.ptr(grid), 1 if grid.dim() == 1 else 0,
+            B, G, _lib.ptr(glen), _lib.ptr(sd_start), _lib.ptr(sd_end), _lib.ptr(sd_end_hi), flags, _lib.ptr(out["K"]),
+            _lib.ptr(out["sd"]), _lib.ptr(u_arg), _lib.ptr(out["status"]), _lib.ptr(out["fail_stage"]),
+            _lib.ptr(out.get("counters")), _lib.stream_ptr())
+    _lib.check(rc, "tbc_scan")
+    return out
+
+
+def sd_forward_cones(records, R, cones, grid, K, status_in, sd_start=None, glen=None):
+    """sd_forward_robust() on the cone table cones [R, 4] (tbc_sd_forward), with the u box of records that carry one."""
+    torch = torch_mod()
+    B, G, W = records.shape
+    dev = records.device
+    check_grid(grid, B, G)
+    check_glen(glen, B, grid)
+    check_path_vector(sd_start, B, "sd_start")
+    check_shape(K, (B, G, 2), "K")
+    if status_in.dtype != torch.int32 or tuple(status_in.shape) != (B,):
+        raise ValueError("status_in must be an int32 tensor of shape (%d,)" % B)
+    table = _cone_table(cones, R)
+    out = {key: torch.empty((B, G), dtype=torch.float64, device=dev) for key in ("x_fast", "x_slow")}
+    out.update({key: torch.empty((B, max(G - 1, 0)), dtype=torch.float64, device=dev) for key in ("u_fast", "u_slow")})
+    out["status"] = torch.empty((B,), dtype=torch.int32, device=dev)
+    out["fail_stage"] = torch.empty((B,), dtype=torch.int32, device=dev)
+    u_fast, u_slow = (out[k] if G > 1 else None for k in ("u_fast", "u_slow"))
+    with torch.cuda.device(dev):
+        rc = _lib_cones.load().tbc_sd_forward(
+            _lib.ptr(records), W, int(R), ctypes.c_void_p(table.ctypes.data),
+            SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0, _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G,
+            _lib.ptr(glen), _lib.ptr(K), _lib.ptr(status_in), _lib.ptr(sd_start), _lib.ptr(out["x_fast"]),
+            _lib.ptr(u_fast), _lib.ptr(out["x_slow"]), _lib.ptr(u_slow), _lib.ptr(out["status"]),
+            _lib.ptr(out["fail_stage"]), _lib.stream_ptr())
+    _lib.check(rc, "tbc_sd_forward")
+    return out
+
+
+def socp_stage_batch_cones(g, a, b, c, cones, xbox, xnext=None, ubox=None):
+    """socp_stage_batch() on the cone table cones [n, 4] (tbc_socp_stage_batch), with the optional u box ubox [B, 2].
+    Returns numpy optvar [B, 2] = (u, x), NaN if infeasible."""
+    torch = torch_mod()
+    dev = default_device()
+    g = as_device(g, dev).reshape(-1, 2)
+    B = g.shape[0]
+    a, b, c = (as_device(t, dev).reshape(B, -1) for t in (a, b, c))
+    n = a.shape[1]
+    xbox = as_device(xbox, dev).reshape(B, 2)
+    xnext = None if xnext is None else as_device(xnext, dev).reshape(B, 3)
+    ubox = None if ubox is None else as_device(ubox, dev).reshape(B, 2)
+    table = _cone_table(cones, n)
+    optvar = torch.empty((B, 2), dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib_cones.load().tbc_socp_stage_batch(
+            _lib.ptr(g), _lib.ptr(a) if n else None, _lib.ptr(b) if n else None, _lib.ptr(c) if n else None, n,
+            ctypes.c_void_p(table.ctypes.data), _lib.ptr(xbox), _lib.ptr(xnext), _lib.ptr(ubox), B, _lib.ptr(optvar),
+            _lib.stream_ptr())
+    _lib.check(rc, "tbc_socp_stage_batch")
+    return optvar.cpu().numpy()
+
+
+def reachable_sets_cones(records, R, cones, grid, sdmin=None, sdmax=None, glen=None):
+    """reachable_sets_robust() on the cone table cones [R, 4]: the feasible sets of one tbc_scan
+    (TB_SCAN_FEASIBLE_SETS) launch, then one tbc_reachable_sets launch.  Same result: dict(X, L, fail_stage)."""
+    torch = torch_mod()
+    B, G, W = records.shape
+    dev = records.device
+    check_grid(grid, B, G)
+    check_glen(glen, B, grid)
+    for t, what in ((sdmin, "sdmin"), (sdmax, "sdmax")):
+        check_path_vector(t, B, what)
+    X = scan_cones(records, R, cones, grid, feasible_sets=True, glen=glen)["K"]
+    table = _cone_table(cones, R)
+    L = torch.empty((B, G, 2), dtype=torch.float64, device=dev)
+    fs = torch.empty((B,), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        rc = _lib_cones.load().tbc_reachable_sets(
+            _lib.ptr(records), W, int(R), ctypes.c_void_p(table.ctypes.data),
+            SCAN_FLAGS["ubound"] if has_ubound(records, R) else 0, _lib.ptr(grid), 1 if grid.dim() == 1 else 0, B, G,
+            _lib.ptr(glen), _lib.ptr(X), _lib.ptr(sdmin), _lib.ptr(sdmax), _lib.ptr(L), _lib.ptr(fs),
+            _lib.stream_ptr())
+    _lib.check(rc, "tbc_reachable_sets")
     return dict(X=X, L=L, fail_stage=fs)
 
 

@@ -158,6 +158,7 @@ class B200SolverWrapper(SolverWrapper):
     def _solve_stage_conic(self, i, H, g, x_min, x_max, x_next_min, x_next_max):
         """ecos_solverwrapper.py:90-207: absent x / x_next bounds are -/+ECOS_INFTY, the xbound rows give
         x >= xbound_lo and x <= min(ECOS_MAXX, xbound_hi); no x_next rows at the last stage."""
+        from ..batch import socp_stage_robust
         assert H is None or np.allclose(H, np.zeros(2))
         if self._rows_host is None:
             self._rows_host = self.rows()
@@ -170,9 +171,11 @@ class B200SolverWrapper(SolverWrapper):
             xnext = [[self.deltas[i], -ECOS_INFTY if np.isnan(x_next_min) else x_next_min,
                       ECOS_INFTY if np.isnan(x_next_max) else x_next_max]]
         g = np.asarray(g, dtype=np.float64)[:2]
-        return engine.socp_stage_batch(g[None], rows["a"][i][None, 2:2 + R], rows["b"][i][None, 2:2 + R],
-                                       rows["c"][i][None, 2:2 + R], self.conic[0], self.conic[1], self.conic[2],
-                                       np.array([xbox]), xnext)[0]
+        ubox = None
+        if engine.has_ubound(self.records, R):   # the u box of the linear constraints' ubounds (ecos_solverwrapper.py:138-150)
+            ubox = np.array([[rows["low"][i][0], rows["high"][i][0]]])
+        return socp_stage_robust(g[None], rows["a"][i][None, 2:2 + R], rows["b"][i][None, 2:2 + R],
+                                 rows["c"][i][None, 2:2 + R], self.conic, np.array([xbox]), xnext, ubox)[0]
 
     # ---- whole-pass entry points ---------------------------------------------------------------------
     def _scalar(self, v):
@@ -227,6 +230,6 @@ class B200SolverWrapper(SolverWrapper):
 
     def feasible_sets(self):
         if self.conic is not None:
-            return engine.scan_robust(self.records, self.R, self.conic[0], self.conic[1], self.conic[2],
-                                      self.ctx.d_grid, feasible_sets=True)["K"][0].cpu().numpy()
+            from ..batch import feasible_sets_robust
+            return feasible_sets_robust(self.records, self.R, self.ctx.d_grid, self.conic)["K"][0].cpu().numpy()
         return engine.feasible_sets(self.records, self.R, self.ctx.d_grid)[0].cpu().numpy()
