@@ -1,4 +1,5 @@
-"""Large-scale CPU check of the Seidel-shortcut model (oracle/shortcut_model.c) against the sequential restatement:
+"""Large-scale CPU check of the Seidel-shortcut model with the min-x closure (tests/closure_model.c on top of
+oracle/shortcut_model.c) against the sequential restatement:
 random 7-DOF / 200-gridpoint paths in four flavours (benchmark-like, velocity-limited, randomly scaled waypoints and
 limits, non-uniform grids), 4096 paths per job, every 2-variable LP compared bit for bit.
 usage: python scripts/shortcut_campaign.py <processes> <jobs>      (10000 jobs = 1.63e10 LPs, about 25 min on 8 cores)
@@ -12,8 +13,9 @@ def work(args):
     seed, B, kind = args
     from oracle import oracle as orc
     from problems import make_batch_fast
+    from closure_model import closure_model
     rng=np.random.RandomState(seed)
-    with orc.shortcut_model() as sm:
+    with closure_model() as sm:
         grid=np.linspace(0,1,200)
         ss,way,vlim,alim=make_batch_fast(B, seed)
         if kind==1: vlim=vlim*0.03           # velocity-limited
@@ -22,12 +24,13 @@ def work(args):
         c=np.stack([orc.cubic_spline_fit(ss,way[b]) for b in range(B)])
         r=orc.solve_velacc_batch(c,np.tile(ss,(B,1)),grid,vlim,alim,nthreads=1)
         st=sm.stats()
-    return st['lps'], st['mismatches'], st['a_used'], st['a_declined'], st['b_used'], st['b_declined'], int((r['status']!=0).sum())
+    return st['lps'], st['mismatches'], st['a_used'], st['a_declined'], st['b_used'], st['b_declined'], st['closed'], st['close_declined'], int((r['status']!=0).sum())
 def work_varied(seed):
     from oracle import oracle as orc
     from problems import make_torque_problem, inv_dyn_numpy
+    from closure_model import closure_model
     rng=np.random.RandomState(seed)
-    with orc.shortcut_model() as sm:
+    with closure_model() as sm:
         nfail=0
         for it in range(24):
             dof=rng.randint(1,15); nway=rng.randint(3,11); G=rng.randint(20,400); B=16
@@ -58,15 +61,16 @@ def work_varied(seed):
             rows=np.concatenate((base['rows'],rows),axis=2)
             o=orc.solve_rows(rows,base['xbound'],grid,0,0); nfail+=o['status']!=0
         st=sm.stats()
-    return st['lps'], st['mismatches'], st['a_used'], st['a_declined'], st['b_used'], st['b_declined'], nfail
+    return st['lps'], st['mismatches'], st['a_used'], st['a_declined'], st['b_used'], st['b_declined'], st['closed'], st['close_declined'], nfail
 if __name__=='__main__':
     nproc=int(sys.argv[1]); njobs=int(sys.argv[2]); B=4096
     varied = len(sys.argv) > 3 and sys.argv[3] == 'varied'
-    t=time.time(); tot=np.zeros(7,dtype=np.int64)
+    t=time.time(); tot=np.zeros(9,dtype=np.int64)
+    import closure_model; closure_model.build()
     with mp.Pool(nproc) as pool:
         jobs = pool.imap_unordered(work_varied, range(700000, 700000 + njobs)) if varied else \
             pool.imap_unordered(work, [(5000000 + j, B, j % 4) for j in range(njobs)])
         for i, res in enumerate(jobs):
             tot+=np.array(res)
             if (i+1)%500==0: print(i+1,'jobs', tot, '%.0fs'%(time.time()-t), flush=True)
-    print('TOTAL lps mismatches a_used a_decl b_used b_decl failed_paths:', tot, '%.0fs'%(time.time()-t))
+    print('TOTAL lps mismatches a_used a_decl b_used b_decl closed close_decl failed_paths:', tot, '%.0fs'%(time.time()-t))

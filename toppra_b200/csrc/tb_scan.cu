@@ -182,6 +182,52 @@ __device__ __forceinline__ bool lp2d_impl(const double v0, const double v1, cons
           const double ur = sg * um;
           bad = bad || (ur < low0 + 1.0) || (ur > high0 - 1.0);
           if (!__any_sync(FULL, bad)) knew = m;
+          if (knew == m && v0 > 0.0) {
+            // Closure (min-x LP; DESIGN.md §4 K2).  The re-solve on m ends on the x-box item x >= low1 unless another
+            // item binds: compute that outcome with the re-solve's own arithmetic (z, then t of box row (0, -1, low1)
+            // as project_item forms it) and take it if every other row, the u box and x <= high1 hold at the closed
+            // point q with a relative margin.  Then every earlier row's item lies strictly on the far side of t (no
+            // tie, cross or parallel-infeasible item, |t| * TINY < SMALL), and the search after the re-solve finds no
+            // violated row.  The closure is the one re-solve it replaces.  Scalar model: tests/closure_model.c.
+            double am = a[0], bm = b[0], cm = c[0];
+#pragma unroll
+            for (int s = 1; s < RPL; ++s)
+              if ((m >> 5) == s) { am = a[s]; bm = b[s]; cm = c[s]; }
+            am = __shfl_sync(FULL, am, m & 31);
+            bm = __shfl_sync(FULL, bm, m & 31);
+            cm = __shfl_sync(FULL, cm, m & 31);
+            const double nrm = am * am + bm * bm;
+            const double zq = ((lane & 1) ? (-bm * cm) : (-am * cm)) / nrm;
+            const double z0 = __shfl_sync(FULL, zq, 0);
+            const double z1 = __shfl_sync(FULL, zq, 1);
+            const double dt0 = -bm, dt1 = am;
+            const double num = low1 + z1 * -1.0 + z0 * 0.0;
+            const double den = dt0 * 0.0 + dt1 * -1.0;
+            const double t = -num / den;
+            const double q0 = z0 + t * dt0, q1 = z1 + t * dt1;
+            const double qs = fabs(q0) + fabs(q1);
+            bool miss = !(fabs(t) < SKIP_TMAX);
+#pragma unroll
+            for (int s = 0; s < RPL; ++s) {
+              const double val = a[s] * q0 + b[s] * q1 + c[s];
+              miss = miss || ((pos[s] != INT_MAX) && (pos[s] != m) &&
+                              !(val <= -SKIP_GAP * (1.0 + fabs(c[s]) + (fabs(a[s]) + fabs(b[s])) * qs)));
+            }
+            {  // box rows u >= low0, u <= high0, x <= high1 on lanes 0..2
+              double ba, bb, bc;
+              box_row((lane == 2) ? 3 : lane, low0, high0, low1, high1, ba, bb, bc);
+              const double val = ba * q0 + bb * q1 + bc;
+              miss = miss || ((lane < 3) && !(val <= -SKIP_GAP * (1.0 + fabs(bc) + (fabs(ba) + fabs(bb)) * qs)));
+            }
+            if (!__any_sync(FULL, miss)) {
+              ++n_resolve;
+              ac0 = m;
+              ac1 = -3;
+              out_u = q0;
+              out_x = q1;
+              return true;
+            }
+          }
         }
       }
     }
